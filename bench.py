@@ -43,9 +43,10 @@ def parse_args():
     ap.add_argument("--e2e-steps", type=int, default=None, help="steps for the host-buffer e2e leg")
     ap.add_argument("--host-ring", type=int, default=256, help="distinct pinned host frames for e2e")
     ap.add_argument("--cpu-sample", type=int, default=400, help="frames in the cpu_baseline sample")
-    ap.add_argument("--edge-batch", type=int, default=2048,
+    ap.add_argument("--edge-batch", type=int, default=512,
                     help="frames per engine batch when the Canny/dilate edge component is on (its per-pixel "
-                         "scratch - V plane, class map, union-find labels - is 6 B/px per frame of a batch)")
+                         "scratch - V plane, class map, union-find labels - is 6 B/px per frame of a batch: "
+                         "6.4 GB at 1080p, which leaves room for the resident frames in 80 GB)")
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-cpu", action="store_true")
     ap.add_argument("--detector", default="content",
@@ -56,18 +57,24 @@ def parse_args():
     ap.add_argument("--parity-frames", type=int, default=None,
                     help="frames of the timed run re-scored with the oracle (default: the cpu sample, 48 with --no-cpu)")
     ap.add_argument("--ref-frames-per-proc", type=int, default=64, help="reference arm: frames per process per step")
-    ap.add_argument("--resident-gb", type=float, default=150.0,
-                    help="HBM budget for resident input per GPU; a larger shard cycles a resident ring of distinct frames")
+    ap.add_argument("--resident-gb", type=float, default=64.0,
+                    help="HBM budget for resident input per GPU (at most 85 %% of the free memory is used); a larger "
+                         "shard cycles a resident ring of distinct frames")
     ap.add_argument("--sweep", action="store_true",
                     help="BASELINE.json configs[4]: one line per (size, total frames) cell, strong scaling over the ranks")
     ap.add_argument("--sweep-cells", default="640x360,1280x720,1920x1080,3840x2160:1000,10000,100000")
     ap.add_argument("--auto-downscale", action="store_true",
                     help="score at SceneManager's default auto-downscaled size (256 px wide) instead of full resolution")
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the per-frame results of the last step as DIR/<name>.npy")
+    args = ap.parse_args()
+    if args.steps < 1 or args.warmup < 0:
+        ap.error("--steps must be >= 1 and --warmup >= 0")
+    return args
 
 
 # ------------------------------------------------------------------------------------------
-# clocks / throttle sampling (B200_PROFILING.md recipe)
+# clocks / throttle sampling
 # ------------------------------------------------------------------------------------------
 class ClockSampler:
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,"
@@ -140,7 +147,7 @@ def measured_peak_gbs() -> tuple[float, str]:
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+        return 3350.0, "data sheet (H100 SXM HBM3 3.35 TB/s), not measured"
 
 
 # ------------------------------------------------------------------------------------------
@@ -276,30 +283,29 @@ def run_reference(args):
 
 
 def workload_text(det_desc, frames_per_gpu, w, h, seed, scored) -> str:
-    """Same wording in both arms (the driver compares the `config.workload` strings)."""
+    """Same wording in both arms (so the two arms' `config.workload` strings can be compared)."""
     return (f"{det_desc} on {frames_per_gpu} synthetic {w}x{h} BGR24 frames per GPU (BASELINE.json configs[1]), "
             f"seed {seed}, " + ("full resolution" if tuple(scored) == (w, h) else f"auto-downscaled on the device to {scored[0]}x{scored[1]}"))
 
 
-def ncu_traffic_per_frame() -> tuple[float | None, str]:
-    """dram bytes per 1080p frame of the fused HSV pass from the committed ncu summary (a citation, not a
-    measurement of this run): newest profiles/r*_ncu_score_ws_kernel*.txt that holds the counters."""
-    import glob
-    import re
-    for path in sorted(glob.glob(os.path.join(ROOT, "profiles", "r*_ncu_score_ws_kernel*.txt")), reverse=True):
-        try:
-            text = open(path).read()
-            rd = re.search(r"dram__bytes_read\.sum\s+(\w+)\s+([0-9.]+)", text)
-            wr = re.search(r"dram__bytes_write\.sum\s+(\w+)\s+([0-9.]+)", text)
-            fr = re.search(r"(\d+) frames 1920x1080", text)
-            if not (rd and wr and fr):
-                continue
-            unit = {"Gbyte": 1e9, "Mbyte": 1e6, "Kbyte": 1e3, "byte": 1.0}
-            total = float(rd.group(2)) * unit[rd.group(1)] + float(wr.group(2)) * unit[wr.group(1)]
-            return total / int(fr.group(1)), os.path.relpath(path, ROOT)
-        except (OSError, KeyError, ValueError):
-            continue
-    return None, "no ncu summary with dram counters under profiles/"
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir: str, arrays: dict, seed: int, suffix: str = "") -> None:
+    """Write each per-frame result array as out_dir/<name><suffix>.npy (float64).  If together they exceed
+    DUMP_LIMIT_BYTES, the same seeded sample of frame indices is taken from every array and written as
+    frame_index<suffix>.npy beside them."""
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {k: np.asarray(v, dtype=np.float64) for k, v in arrays.items()}
+    n = next(iter(arrays.values())).shape[0]
+    row_bytes = sum(a[:1].nbytes for a in arrays.values())
+    if row_bytes * n > DUMP_LIMIT_BYTES:
+        keep = DUMP_LIMIT_BYTES // (row_bytes + 8)
+        idx = np.sort(np.random.default_rng(seed).choice(n, size=keep, replace=False))
+        arrays = {k: a[idx] for k, a in arrays.items()}
+        arrays["frame_index"] = idx.astype(np.float64)
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, f"{name}{suffix}.npy"), a)
 
 
 # ------------------------------------------------------------------------------------------
@@ -459,6 +465,20 @@ def run_ours(args):
     barrier()
     wall = time.perf_counter() - t0
     ev_ms_total = ev_begin.elapsed_time(ev_end)
+    if args.dump_outputs:
+        # the last timed step's per-frame results, as a caller of this path receives them
+        metric = {"threshold": "average_rgb", "histogram": "hist_diff", "hash": "hash_dist"}.get(args.detector,
+                                                                                                "content_val")
+        out = {metric: d_val.cpu().numpy()}
+        if args.detector in ("content", "content_edges", "adaptive"):
+            comp = d_comp.view(N, 4).cpu().numpy()
+            for j, name in enumerate(("delta_hue", "delta_sat", "delta_lum", "delta_edges")):
+                out[name] = comp[:, j]
+        if args.detector in ("content", "content_edges"):
+            out["above_threshold"] = d_flag.cpu().numpy()
+        if args.detector == "adaptive":
+            out["adaptive_ratio"] = d_ratio.cpu().numpy()
+        dump_outputs(args.dump_outputs, out, args.seed, "" if world == 1 else f"_rank{rank}")
     sampler.window = (t0, t0 + wall)
     clocks = sampler.stop() if rank == 0 else None
     launches = lib.psd_launch_count() - launches0
@@ -556,7 +576,7 @@ def run_ours(args):
         sbytes = sw * sh * 3  # bytes of a frame as the fused pass sees it (smaller than fbytes when auto-downscaled)
         alg_bytes = sbytes * N * args.steps  # per-rank algorithmic bytes through the score kernel
         achieved = alg_bytes / (score_ms_total / 1000.0) / 1e9
-        traffic_pf, traffic_src = ncu_traffic_per_frame()
+        l2_mb = getattr(torch.cuda.get_device_properties(dev), "L2_cache_size", 0) / 2**20
         line = {
             "metric": METRIC, "value": value, "unit": UNIT, "n_gpus": world, "steps": args.steps,
             "warmup": args.warmup, "ms_per_step": ev_ms, "higher_is_better": True, "scaling": args.scaling,
@@ -566,7 +586,7 @@ def run_ours(args):
                                           W, H, args.seed, (sw, sh)),
                 "frames_per_gpu": N, "total_frames": total_frames,
                 "parallelism": f"{world} contiguous time shards, 1-frame halo over NCCL p2p" if world > 1 else "single GPU",
-                "l2": f"inputs are {N * fbytes / 1e9:.1f} GB per step per GPU, larger than L2 (126 MB): no flush needed"
+                "l2": f"inputs are {N * fbytes / 1e9:.1f} GB per step per GPU, larger than L2 ({l2_mb:.0f} MB): no flush needed"
                       + ("" if R == N else f"; {R} distinct frames ({R * fbytes / 1e9:.1f} GB) stay resident and are walked {N / R:.2f} times per step"),
                 "timed_region": "halo exchange + fused score kernel + trailing device scan, inputs resident in HBM",
             },
@@ -581,11 +601,6 @@ def run_ours(args):
                 "unit": "GB/s", "frac": achieved / peak, "peak_source": peak_src,
                 "algorithmic_bytes_per_frame": sbytes,
                 "launches": int(score_launches), "avg_launch_ms": score_ms_total / max(1, score_launches),
-                # dram__bytes_read+write of one `ncu --set full` capture of this kernel (a citation from the
-                # committed summary, NOT measured in this run), scaled to the average launch of this run
-                "traffic": (traffic_pf * (N * args.steps / max(1, score_launches)) / 1e9
-                            if (traffic_pf and args.detector == "content" and (W, H) == (1920, 1080) and (sw, sh) == (W, H)) else None),
-                "traffic_unit": f"GB per launch, cited from {traffic_src} (one ncu capture, scaled by frames per launch; not measured in this run)",
                 "achieved_bytes_per_launch_gb": sbytes * N * args.steps / max(1, score_launches) / 1e9,
             },
         }
@@ -704,7 +719,6 @@ def main():
                 a.width, a.height = (int(v) for v in size.split("x"))
                 a.frames, a.scaling = int(total), "strong"
                 a.no_e2e = a.no_cpu = True
-                a.steps, a.warmup = min(args.steps, 5), 3
                 a.parity_frames = 8
                 run_ours(a)
     else:

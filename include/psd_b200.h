@@ -1,5 +1,5 @@
 /*
- * psd_b200.h - C ABI of the B200-native per-frame content-score engine for PySceneDetect.
+ * psd_b200.h - C ABI of the H100-native (sm_90a) per-frame content-score engine for PySceneDetect.
  *
  * This is the drop-in boundary for the hot path named in BASELINE.json: the
  * process_frame() arithmetic of ContentDetector / AdaptiveDetector / ThresholdDetector /
@@ -11,7 +11,7 @@
  * Conventions: every call returns an int status (PSD_OK == 0, negative = error class);
  * no C++ exception crosses this boundary; output buffers are caller-allocated;
  * psd_last_error() returns a thread-local human-readable message for the last failure.
- * There is NO CPU fallback: without an sm_100 device psd_engine_create fails.
+ * There is NO CPU fallback: without an sm_90 device psd_engine_create fails.
  */
 #ifndef PSD_B200_H
 #define PSD_B200_H
@@ -31,7 +31,7 @@ extern "C" {
 #define PSD_ERR_CUDA (-2)    /* CUDA runtime/driver failure (message has the cudaError) */
 #define PSD_ERR_OOM (-3)     /* host or device allocation failed */
 #define PSD_ERR_STATE (-4)   /* call not valid in the engine's current state */
-#define PSD_ERR_NODEVICE (-5)/* no usable sm_100 device */
+#define PSD_ERR_NODEVICE (-5)/* no usable sm_90 device */
 
 /* feature mask: which per-frame integer results the fused pass produces */
 #define PSD_F_HSV 1u    /* SAD of H,S,V planes vs previous frame: content_detector.py:29-36,155,166-175 */

@@ -2,7 +2,7 @@
 TEST INFRASTRUCTURE - see oracle/__init__.py.
 
 The arithmetic of this path is in OpenCV (opencv-python-headless 4.13.0.92 in this image;
-not vendored in /root/reference, unpinned in its pyproject.toml:43-57).  Each function below
+not vendored in the reference, unpinned in its pyproject.toml:43-57).  Each function below
 restates the published OpenCV algorithm the reference reaches through the call site cited,
 and is pinned against cv2 itself by tests/test_oracle_intmath.py.  The CUDA kernels implement
 exactly these formulas.

@@ -1,7 +1,7 @@
-"""pyscenedetect_b200 - Blackwell-native per-frame content-score engine for PySceneDetect.
+"""pyscenedetect_b200 - H100-native (sm_90a) per-frame content-score engine for PySceneDetect.
 
 Only the hot path is here: the four fast-cut detectors' `process_frame` arithmetic and the
-SceneManager downscale, as sm_100a CUDA kernels behind a C-ABI (include/psd_b200.h).
+SceneManager downscale, as sm_90a CUDA kernels behind a C-ABI (include/psd_b200.h).
 Importing the package does not need a GPU; constructing an engine does (no CPU fallback).
 """
 

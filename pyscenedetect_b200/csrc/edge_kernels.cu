@@ -15,7 +15,7 @@
 //   -> hysteresis: E grows inside C until nothing changes, bit-parallel          [1 cooperative launch]
 //   -> k x k max on the bits in one pass, popcount SAD against the previous frame [2 launches]
 // (the first version kept a byte class map, 4-byte union-find labels per pixel and 12 launches per
-// batch: profiles/r01w_launches_content_edges_summary.txt).
+// batch).
 #include <cooperative_groups.h>
 
 #include "canny_pairs.cuh"
@@ -83,7 +83,7 @@ __global__ void psd_edge_thresholds_kernel(const uint32_t* __restrict__ vhist, i
 // pixel PAIRS, two 16-bit lanes per register (canny_pairs.cuh).  No shared memory, no shuffles, no barrier;
 // neighbouring threads re-read overlapping words from L1.  (Round 2's first version of this kernel kept one
 // pixel per 32-bit register - IDP4A row sums, integer NMS: 476 instructions per 8-pixel row against 281,
-// profiles/r02i_edge_ab_summary.txt.)
+// earlier A/B runs.)
 //
 // The two planes it writes are TILE-MAJOR: tile (ty, tx) = rows 32 ty .. 32 ty + 31 x columns 64 tx .. 64 tx + 63
 // is 64 consecutive words, row r of the tile at words 2 r and 2 r + 1.  A warp of the hysteresis kernel then
@@ -271,7 +271,7 @@ __device__ __forceinline__ unsigned long long run_fill(unsigned long long t, uns
     return up | dn;
 }
 
-#if PSD_HYST_STATS   // alt build for tools/gpu_*.sh: per-round tile counts and times of the first launches
+#if PSD_HYST_STATS   // alt build: per-round tile counts and times of the first launches
 __device__ unsigned long long g_hs_visit[512], g_hs_work[512], g_hs_change[512], g_hs_time[512], g_hs_iter[512];
 __device__ int g_hs_launch;
 #define HS_COUNT(arr, round) do { if (lane == 0 && (round) < 512) atomicAdd(&arr[round], 1ull); } while (0)
@@ -293,8 +293,7 @@ __global__ void __launch_bounds__(256, 5) psd_hyst_bits_kernel(uint32_t* __restr
     // warp visits the dirty ones of a run one after the other, so a change walks along the run within the round).
     // Round-robin over the runs: the heavy frames of a batch are spread over all warps.  (A compacted work list
     // per round - perfectly even counts, but neighbouring tiles visited by different warps at the same time -
-    // took twice as long: profiles/r02i_edge_ab_summary.txt.)
-    // (one contiguous run per warp: 141.7 k against 148.9 k frames/s)
+    // took twice as long.)
     const int64_t t_begin = warp0 * 32, t_end = n_tiles, t_step = n_warps * 32;
 
     for (int round = 0; round < 100000; ++round) {

@@ -203,7 +203,7 @@ static int run_batch(psd_engine* e, const uint8_t* src, int64_t src_frame_stride
 extern "C" {
 
 int psd_abi_version(void) { return PSD_ABI_VERSION; }
-const char* psd_version(void) { return "psd_b200 0.1.0 (sm_100a)"; }
+const char* psd_version(void) { return "psd_b200 0.1.0 (sm_90a)"; }
 const char* psd_last_error(void) { return g_err; }
 uint64_t psd_launch_count(void) { return g_launches.load(); }
 
@@ -315,8 +315,8 @@ int psd_engine_create(const psd_config* cfg, psd_engine** out) {
     PSD_REQUIRE(cfg->device >= 0 && cfg->device < ndev, "device %d out of range (%d visible)", cfg->device, ndev);
     cudaDeviceProp prop{};
     PSD_CUDA(cudaGetDeviceProperties(&prop, cfg->device));
-    if (prop.major != 10) {
-        set_error("device %d is sm_%d%d; this library is built for sm_100a only", cfg->device, prop.major,
+    if (prop.major != 9 || prop.minor != 0) {  // sm_90a code loads on compute capability 9.0 only
+        set_error("device %d is sm_%d%d; this library is built for sm_90a only", cfg->device, prop.major,
                   prop.minor);
         return PSD_ERR_NODEVICE;
     }

@@ -38,7 +38,7 @@ __device__ __forceinline__ float byte_to_float(uint32_t g) { return __fadd_rn(__
 //      factors are integers, else OpenCV's float32 `buf += S * alpha` in source order (separate multiply and
 //      add: the order and the roundings decide the last bit, so this chain stays sequential).
 // (The first version had one thread per (row, column) read its 3 x 120 bytes straight from global memory, 32
-// lanes 360 bytes apart: 0.085 of the HBM roofline, profiles/r02i_edge_ab_summary.txt.)
+// lanes 360 bytes apart: 0.085 of the HBM roofline.)
 __global__ void __launch_bounds__(256) psd_hash_rows_kernel(const uint8_t* __restrict__ frames, int64_t frame_stride,
                                                             int W, int H, int n, int rows_per_cta, int pitch, int fast,
                                                             const int32_t* __restrict__ xstart,

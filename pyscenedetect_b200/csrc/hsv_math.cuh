@@ -19,7 +19,7 @@ struct Px16 {  // 16 pixels, planar, 4 pixels per 32-bit word (pixel 4j+i in byt
     uint32_t h[4], s[4], v[4];
 };
 
-// ---- generic-path arithmetic: float-domain pipeline on pixel PAIRS with packed FFMA2/FADD2 (sm_100 f32x2) ----
+// ---- generic-path arithmetic: float-domain pipeline on pixel PAIRS ----
 // (used by psd_score_kernel for strips the warp-specialised kernel cannot take: unaligned inputs, tails that
 // are not a multiple of 16 pixels, frames smaller than a strip; the fast path is hsv_half2.cuh.)
 // The table entries are regenerated with one MUFU.RCP each:
@@ -39,40 +39,31 @@ struct Px16 {  // 16 pixels, planar, 4 pixels per 32-bit word (pixel 4j+i in byt
 //       y = fma.rm(x, 2^-12, 1.5 * 2^23)      -> mantissa = 2^22 + floor(x / 4096)
 // |d * sdiv| < 2^28 and |h * hdiv| < 2^25, so the dropped bits are at most 2^4 resp. 2^1 wide and
 // 4096 k is always representable: floor(x/4096) is unchanged.  Pinned by the exhaustive test.
-typedef unsigned long long f32x2_t;
+// sm_90 has no packed FP32 instructions (f32x2 needs sm_100), so a pair is two scalar FP32 operations
+// with the same rounding mode per lane: the results are the same bits.
+struct f32x2_t {
+    float lo, hi;
+};
 
-__device__ __forceinline__ f32x2_t pack2(float lo, float hi) {
-    f32x2_t r;
-    asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
-    return r;
-}
+__device__ __forceinline__ f32x2_t pack2(float lo, float hi) { return {lo, hi}; }
 __device__ __forceinline__ void unpack2(f32x2_t v, float& lo, float& hi) {
-    asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
+    lo = v.lo;
+    hi = v.hi;
 }
 __device__ __forceinline__ f32x2_t add2(f32x2_t a, f32x2_t b) {
-    f32x2_t r;
-    asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-    return r;
+    return {__fadd_rn(a.lo, b.lo), __fadd_rn(a.hi, b.hi)};
 }
 __device__ __forceinline__ f32x2_t sub2(f32x2_t a, f32x2_t b) {
-    f32x2_t r;
-    asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-    return r;
+    return {__fsub_rn(a.lo, b.lo), __fsub_rn(a.hi, b.hi)};
 }
 __device__ __forceinline__ f32x2_t fma2_rn(f32x2_t a, f32x2_t b, f32x2_t c) {
-    f32x2_t r;
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c));
-    return r;
+    return {__fmaf_rn(a.lo, b.lo, c.lo), __fmaf_rn(a.hi, b.hi, c.hi)};
 }
 __device__ __forceinline__ f32x2_t fma2_rz(f32x2_t a, f32x2_t b, f32x2_t c) {
-    f32x2_t r;
-    asm("fma.rz.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c));
-    return r;
+    return {__fmaf_rz(a.lo, b.lo, c.lo), __fmaf_rz(a.hi, b.hi, c.hi)};
 }
 __device__ __forceinline__ f32x2_t fma2_rm(f32x2_t a, f32x2_t b, f32x2_t c) {
-    f32x2_t r;
-    asm("fma.rm.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c));
-    return r;
+    return {__fmaf_rd(a.lo, b.lo, c.lo), __fmaf_rd(a.hi, b.hi, c.hi)};
 }
 __device__ __forceinline__ float rcp_approx(float x) {
     float r;

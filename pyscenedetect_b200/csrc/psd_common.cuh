@@ -1,4 +1,4 @@
-// Shared helpers for the psd_b200 CUDA translation units (sm_100a only).
+// Shared helpers for the psd_b200 CUDA translation units (sm_90a only).
 #pragma once
 
 #include <cuda_runtime.h>

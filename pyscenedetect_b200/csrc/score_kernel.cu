@@ -282,7 +282,7 @@ __global__ void __launch_bounds__(Shape::kThreads, Shape::kMinBlocks) psd_score_
 // from one item into the next, so the producer is always kWsStages frames ahead - also across item
 // boundaries: there is no pipeline fill / drain per item, the LUT is built once per SM and no SM idles
 // between CTAs (the non-persistent form lost ~4 % of the SM time between CTAs and ~5 % of the warp time
-// waiting for the first frame of each CTA: profiles/r02a_*).
+// waiting for the first frame of each CTA).
 //
 // No CTA-wide barrier in the frame loop: consumers wait on the stage's FULL mbarrier (TMA complete_tx),
 // pull their 48 bytes, do the arithmetic, add their SADs to the stage's per-lane shared accumulators and
@@ -869,8 +869,11 @@ template <bool FAST>
 static int run_test_hsv(const uint8_t* d_bgr, int64_t groups, uint8_t* dh, uint8_t* ds, uint8_t* dv,
                         uint8_t* dy) {
     const int smem = FAST ? 65536 : 0;
+    int dev = 0, sm_count = 0;
+    PSD_CUDA(cudaGetDevice(&dev));
+    PSD_CUDA(cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, dev));
     PSD_CUDA(cudaFuncSetAttribute(psd_test_hsv_kernel<FAST>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    psd_test_hsv_kernel<FAST><<<148 * 2, 256, smem>>>(d_bgr, groups, dh, ds, dv, dy);
+    psd_test_hsv_kernel<FAST><<<sm_count * 2, 256, smem>>>(d_bgr, groups, dh, ds, dv, dy);
     PSD_CHECK_LAUNCH();
     return PSD_OK;
 }

@@ -1,7 +1,7 @@
 """Deterministic integer-only synthetic BGR24 frame sequences (SURVEY.md §8(d)).
 
-The reference's own fixtures are encoded videos (tests/resources/*.mp4, absent here and on
-the GPU box), so parity and benchmarks run on a seeded synthetic sequence instead: hard
+The reference's own fixtures are encoded videos (tests/resources/*.mp4, not shipped with
+the reference's source package), so parity and benchmarks run on a seeded synthetic sequence instead: hard
 cuts at known frames, slow in-scene drift, low-amplitude per-pixel noise, fades to black
 in every 3rd scene that is long enough (so ThresholdDetector's fade FSM fires) and a two-frame colour flash in
 every 7th scene (so FlashFilter's MERGE/SUPPRESS branches fire).  All arithmetic is

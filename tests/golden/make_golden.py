@@ -1,9 +1,9 @@
 #!/usr/bin/env python
 """Generate tests/golden/golden_v1.json by running the REAL reference (imported from
-/root/reference, PySceneDetect 0.7.1) on seeded synthetic sequences.
+a PySceneDetect 0.7.1 source checkout given as the first argument) on seeded synthetic sequences.
 
-Run in the build container only (`python tests/golden/make_golden.py`); the GPU box has no
-/root/reference, which is why the outputs are committed.  Metric values are stored as
+Run `python tests/golden/make_golden.py <reference checkout>`; the tests do not need the reference,
+which is why the outputs are committed.  Metric values are stored as
 `float.hex()` strings so they round-trip bit for bit.  Cases that go through the
 reference's own `SceneManager.detect_scenes` (decode thread, cv2.resize downscale,
 StatsManager CSV) use a synthetic `VideoStream`.
@@ -21,7 +21,7 @@ from fractions import Fraction
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
 sys.path.insert(0, ROOT)
-sys.path.insert(0, "/root/reference")
+sys.path.insert(0, os.path.abspath(sys.argv[1]))  # a PySceneDetect 0.7.1 source checkout
 
 import cv2  # noqa: E402
 import numpy as np  # noqa: E402

@@ -37,7 +37,7 @@ def test_binding_loads_and_reports_errors_without_gpu():
     from pyscenedetect_b200 import _capi
     lib = _capi.load()
     assert lib.psd_abi_version() == 1
-    assert b"sm_100a" in lib.psd_version()
+    assert b"sm_90a" in lib.psd_version()
     if lib.psd_device_count() == 0:
         # no CPU fallback: constructing an engine must fail loudly
         from pyscenedetect_b200.engine import F_HSV, Engine

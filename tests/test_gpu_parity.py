@@ -21,7 +21,7 @@ pytestmark = pytest.mark.gpu
 def lib():
     from pyscenedetect_b200 import _capi
     lib = _capi.load()
-    assert lib.psd_device_count() >= 1, "no CUDA device: GPU tests must run on the B200 box"
+    assert lib.psd_device_count() >= 1, "no CUDA device: GPU tests need an H100 (sm_90)"
     return lib
 
 

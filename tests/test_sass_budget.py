@@ -1,4 +1,4 @@
-"""Static checks on the compiled sm_100a code (no GPU needed): the fused pass really uses the
+"""Static checks on the compiled sm_90a code (no GPU needed): the fused pass really uses the
 instructions DESIGN.md says it does, nothing spills to local memory, and the two loops whose
 instruction count IS the performance (the kernel is issue-bound) stay within their budgets.  Runs on
 the in-tree libpsd_b200.so that __graft_entry__.build() produces; skipped without cuobjdump."""
