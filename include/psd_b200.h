@@ -41,10 +41,6 @@ extern "C" {
 #define PSD_F_HASH 16u  /* perceptual hash of every frame: hash_detector.py:124-158 */
 #define PSD_HASH_WORDS 4 /* a hash occupies 4 x uint64 (size * size <= 256 bits), bit u*size+v = D[u][v] > median */
 
-/* engine flags (psd_config.flags) */
-#define PSD_CFG_GENERIC_KERNEL 1u /* score every strip with the generic kernel instead of the persistent
-                                     warp-specialised one (same results; exists so tests can cross-check the two) */
-
 /* submit flags */
 #define PSD_SUBMIT_PINNED 1u /* host buffer is page-locked (psd_host_alloc): DMA straight from it,
                                 caller keeps it unchanged until psd_engine_sync() */
@@ -62,7 +58,7 @@ typedef struct psd_config {
     uint32_t features;        /* PSD_F_* */
     int32_t edge_kernel_size; /* dilate kernel k (odd >= 3); 0 = content_detector.py:39-46 estimate */
     int32_t max_batch;        /* max frames per submit call (staging is sized for it) */
-    uint32_t flags;           /* PSD_CFG_* */
+    uint32_t flags;           /* reserved: no flags are defined, must be 0 */
     int32_t hash_size;        /* PSD_F_HASH: HashDetector(size=...), 0 = 8 */
     int32_t hash_lowpass;     /* PSD_F_HASH: HashDetector(lowpass=...), 0 = 2 */
     int32_t reserved[4];
@@ -208,10 +204,9 @@ int psd_synth_frames(int device, void* d_out, const int32_t* params_host, int64_
                      int32_t height, int64_t frame_stride, void* stream);
 
 /* ---- test hooks ---- */
-/* device BGR (n pixels) -> H,S,V planes with the device functions the fused pass uses:
- * variant 7 = the warp-specialised kernel's arithmetic, 2 = the generic kernel's */
+/* device BGR (n pixels, a multiple of 16) -> H,S,V and Y planes with the device functions the fused pass uses */
 int psd_test_hsv(int device, const uint8_t* bgr_host, int64_t n_pixels, uint8_t* h_out, uint8_t* s_out,
-                 uint8_t* v_out, uint8_t* y_out, int variant);
+                 uint8_t* v_out, uint8_t* y_out);
 
 #ifdef __cplusplus
 }

@@ -28,7 +28,6 @@ F_EDGES = 8
 F_HASH = 16
 HASH_WORDS = 4
 SUBMIT_PINNED = 1
-CFG_GENERIC_KERNEL = 1
 
 
 class PsdConfig(C.Structure):
@@ -116,7 +115,7 @@ SIGNATURES = {
     "psd_engine_scan_hist_correl_host": (C.c_int, [_vp, _i64, _i64, _i32, _vp]),
     "psd_engine_scan_hash_dist_host": (C.c_int, [_vp, _i64, _i64, _vp]),
     "psd_synth_frames": (C.c_int, [C.c_int, _vp, _vp, _i64, _i32, _i32, _i64, _vp]),
-    "psd_test_hsv": (C.c_int, [C.c_int, _vp, _i64, _vp, _vp, _vp, _vp, C.c_int]),
+    "psd_test_hsv": (C.c_int, [C.c_int, _vp, _i64, _vp, _vp, _vp, _vp]),
 }
 
 _lib = None

@@ -26,9 +26,6 @@ namespace cg = cooperative_groups;
 // classify launch shape: 128 threads x 3 CTAs per SM = 163 registers, no spills (256 x 2 caps at 128 registers
 // and spills ~50 words; measured 3-4 % slower)
 constexpr int kClassifyBlock = 128;
-#ifndef PSD_HYST_STATS
-#define PSD_HYST_STATS 0
-#endif
 
 namespace psd {
 
@@ -271,14 +268,6 @@ __device__ __forceinline__ unsigned long long run_fill(unsigned long long t, uns
     return up | dn;
 }
 
-#if PSD_HYST_STATS   // alt build: per-round tile counts and times of the first launches
-__device__ unsigned long long g_hs_visit[512], g_hs_work[512], g_hs_change[512], g_hs_time[512], g_hs_iter[512];
-__device__ int g_hs_launch;
-#define HS_COUNT(arr, round) do { if (lane == 0 && (round) < 512) atomicAdd(&arr[round], 1ull); } while (0)
-#else
-#define HS_COUNT(arr, round) do { } while (0)
-#endif
-
 __global__ void __launch_bounds__(256, 5) psd_hyst_bits_kernel(uint32_t* __restrict__ edge_bits,
                                                             const uint32_t* __restrict__ cand_bits,
                                                             uint8_t* __restrict__ dirty /* [2][n_tiles] */,
@@ -315,7 +304,6 @@ __global__ void __launch_bounds__(256, 5) psd_hyst_bits_kernel(uint32_t* __restr
             while (todo) {
                 const int64_t t = base + __ffs(todo) - 1;
                 todo &= todo - 1;
-                HS_COUNT(g_hs_visit, round);
                 const int64_t f = t / per_frame_tiles;
                 const int tt = (int)(t - f * per_frame_tiles);
                 const int ty = tt / tiles_x, tx = tt - ty * tiles_x;
@@ -345,7 +333,6 @@ __global__ void __launch_bounds__(256, 5) psd_hyst_bits_kernel(uint32_t* __restr
                 unsigned long long e = (unsigned long long)e_lo | ((unsigned long long)e_hi << 32);
                 // weak pixels left in this tile?  (warp-uniform exit: nothing can change)
                 if (__ballot_sync(0xFFFFFFFFu, (c & ~e) != 0ull) == 0u) continue;
-                HS_COUNT(g_hs_work, round);
                 const uint32_t lbit = e_l >> 31, rbit = e_r & 1u;  // E left of column 0 / right of column 63, this row
                 const unsigned long long e_ring = (unsigned long long)g_lo | ((unsigned long long)g_hi << 32);
                 // the side columns do not change while the tile iterates: fold them into two seed bits per row
@@ -358,7 +345,6 @@ __global__ void __launch_bounds__(256, 5) psd_hyst_bits_kernel(uint32_t* __restr
                 if (ru | rbit | rd) side_seed |= 1ull << 63;
                 const unsigned long long e_in = e;
                 while (true) {
-                    HS_COUNT(g_hs_iter, round);
                     unsigned long long u = __shfl_up_sync(0xFFFFFFFFu, e, 1), d = __shfl_down_sync(0xFFFFFFFFu, e, 1);
                     if (lane == 0) u = e_ring;
                     if (lane == 31) d = e_ring;
@@ -374,7 +360,6 @@ __global__ void __launch_bounds__(256, 5) psd_hyst_bits_kernel(uint32_t* __restr
                 if (changed) reinterpret_cast<uint2*>(Et)[lane] = make_uint2((uint32_t)e, (uint32_t)(e >> 32));
                 if (__ballot_sync(0xFFFFFFFFu, changed) != 0u) {
                     warp_changed = true;
-                    HS_COUNT(g_hs_change, round);
                     // the ring of the 8 neighbours may have changed: they look again next round
                     if (lane < 9 && lane != 4) {
                         const int ny = ty + lane / 3 - 1, nx = tx + lane % 3 - 1;
@@ -387,29 +372,7 @@ __global__ void __launch_bounds__(256, 5) psd_hyst_bits_kernel(uint32_t* __restr
         if (warp_changed && lane == 0) atomicOr(&flags[round % 3], 1);
         __threadfence();
         grid.sync();
-#if PSD_HYST_STATS
-        if (blockIdx.x == 0 && threadIdx.x == 0 && round < 512) {
-            unsigned long long now;
-            asm volatile("mov.u64 %0, %globaltimer;" : "=l"(now));
-            g_hs_time[round] = now;
-        }
-#endif
-        if (*(volatile int32_t*)&flags[round % 3] == 0) {
-#if PSD_HYST_STATS
-            if (blockIdx.x == 0 && threadIdx.x == 0) {
-                const int l = atomicAdd(&g_hs_launch, 1);
-                if (l == 4 || l == 9) {   // a warm launch
-                    printf("hyst launch %d: %d rounds, %lld tiles, grid %d\n", l, round + 1, (long long)n_tiles, (int)gridDim.x);
-                    for (int r = 0; r <= round && r < 512; ++r)
-                        printf("  round %d: visited %llu worked %llu changed %llu iterations %llu  +%llu ns\n", r,
-                               g_hs_visit[r], g_hs_work[r], g_hs_change[r], g_hs_iter[r],
-                               r ? g_hs_time[r] - g_hs_time[r - 1] : 0ull);
-                }
-                for (int r = 0; r < 512; ++r) g_hs_visit[r] = g_hs_work[r] = g_hs_change[r] = g_hs_iter[r] = 0ull;
-            }
-#endif
-            break;
-        }
+        if (*(volatile int32_t*)&flags[round % 3] == 0) break;
     }
 }
 

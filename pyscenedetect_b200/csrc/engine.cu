@@ -53,7 +53,6 @@ struct psd_engine {
     uint32_t features = 0;
     int ksize = 0;
     int max_batch = 0;
-    bool generic_only = false;  // PSD_CFG_GENERIC_KERNEL: score with the generic kernel only (cross-check)
     cudaStream_t copy_stream = nullptr, compute_stream = nullptr;
     // staging (double buffered)
     uint8_t* pinned[2] = {nullptr, nullptr};
@@ -61,8 +60,10 @@ struct psd_engine {
     cudaEvent_t slot_free[2] = {nullptr, nullptr};
     cudaEvent_t h2d_done[2] = {nullptr, nullptr};
     int next_slot = 0;
-    // scored-size frames when resizing
+    // scored-size frames, small_stride apart (a multiple of 16 bytes, as the score pass needs): the resize
+    // output, or an aligned copy of a batch whose pointer or frame stride is not a multiple of 16
     uint8_t* small = nullptr;
+    int64_t small_stride = 0;
     int32_t* d_xofs = nullptr; int16_t* d_xa = nullptr; int32_t* d_yofs = nullptr; int16_t* d_ya = nullptr;
     // carry (predecessor of the next frame, scored size)
     uint8_t* carry = nullptr;
@@ -150,11 +151,17 @@ static int run_batch(psd_engine* e, const uint8_t* src, int64_t src_frame_stride
     int64_t scored_stride = src_frame_stride;
     if (e->resize) {
         ResizeTaps taps{e->d_xofs, e->d_xa, e->d_yofs, e->d_ya};
-        int rc = launch_resize(src, src_frame_stride, (int64_t)e->sw * 3, e->sw, e->sh, e->small, e->W,
-                               e->H, n, taps, st);
+        int rc = launch_resize(src, src_frame_stride, (int64_t)e->sw * 3, e->sw, e->sh, e->small, e->small_stride,
+                               e->W, e->H, n, taps, st);
         if (rc) return rc;
         scored = e->small;
-        scored_stride = e->frame_bytes;
+        scored_stride = e->small_stride;
+    } else if (((uintptr_t)src | (uintptr_t)src_frame_stride) & 15) {
+        if (!e->small) PSD_CUDA(cudaMalloc(&e->small, (size_t)e->small_stride * e->max_batch));
+        PSD_CUDA(cudaMemcpy2DAsync(e->small, (size_t)e->small_stride, src, (size_t)src_frame_stride,
+                                   (size_t)e->frame_bytes, (size_t)n, cudaMemcpyDeviceToDevice, st));
+        scored = e->small;
+        scored_stride = e->small_stride;
     }
     PSD_CUDA(cudaMemsetAsync(e->d_sums + slot0, 0, (size_t)n * sizeof(psd_frame_sums), st));
     if (e->features & PSD_F_YHIST)
@@ -167,7 +174,6 @@ static int run_batch(psd_engine* e, const uint8_t* src, int64_t src_frame_stride
     a.frame_stride = scored_stride;
     a.n_frames = (int32_t)n;
     a.n_pixels = (int32_t)e->P;
-    a.chunk_frames = 0;  // launch_score picks the time-chunk length
     a.sums = e->d_sums + slot0;
     a.yhist = (e->features & PSD_F_YHIST) ? e->d_yhist + slot0 * 256 : nullptr;
     a.vhist = (e->features & PSD_F_EDGES) ? e->eb.vhist : nullptr;
@@ -175,7 +181,7 @@ static int run_batch(psd_engine* e, const uint8_t* src, int64_t src_frame_stride
     PSD_CUDA(cudaEventRecord(k0, st));
     int rc = PSD_OK;
     if (e->features & 15u) {  // the fused pass (HSV / byte sum / Y histogram / edges)
-        rc = launch_score(a, e->features & 15u, e->generic_only, st);
+        rc = launch_score(a, e->features & 15u, st);
         if (rc) return rc;
     }
     if (e->features & PSD_F_HASH) {
@@ -306,6 +312,7 @@ int psd_engine_create(const psd_config* cfg, psd_engine** out) {
     PSD_REQUIRE(cfg->max_batch >= 1 && cfg->max_batch <= 4096, "max_batch must be in [1,4096]");
     PSD_REQUIRE(cfg->edge_kernel_size == 0 || (cfg->edge_kernel_size >= 3 && (cfg->edge_kernel_size & 1)),
                 "kernel_size must be odd integer >= 3");
+    PSD_REQUIRE(cfg->flags == 0, "psd_config.flags must be 0 (no flags are defined), got 0x%x", cfg->flags);
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
         cudaGetLastError();
@@ -329,10 +336,10 @@ int psd_engine_create(const psd_config* cfg, psd_engine** out) {
     e->resize = (e->sw != e->W) || (e->sh != e->H);
     e->P = (int64_t)e->W * e->H;
     e->frame_bytes = e->P * 3;
+    e->small_stride = (e->frame_bytes + 15) & ~(int64_t)15;
     e->src_frame_bytes = (int64_t)e->sw * e->sh * 3;
     e->features = cfg->features | ((cfg->features & PSD_F_EDGES) ? PSD_F_HSV : 0);
     e->max_batch = cfg->max_batch;
-    e->generic_only = (cfg->flags & PSD_CFG_GENERIC_KERNEL) != 0;
     if (e->features & PSD_F_EDGES) {
         int k = cfg->edge_kernel_size;
         if (k == 0) {  // content_detector.py:39-46; Python round() is half-to-even like nearbyint
@@ -357,8 +364,11 @@ int psd_engine_create(const psd_config* cfg, psd_engine** out) {
         ENG_CUDA(cudaEventCreateWithFlags(&e->h2d_done[s], cudaEventDisableTiming));
     }
     ENG_CUDA(cudaMalloc(&e->carry, (size_t)e->frame_bytes));
+    // without resizing, staged batches of a frame size that is not a multiple of 16 bytes are always copied
+    // (user device pointers that are not 16-byte aligned allocate it on first use, in run_batch)
+    if (e->resize || e->frame_bytes % 16 != 0)
+        ENG_CUDA(cudaMalloc(&e->small, (size_t)e->small_stride * e->max_batch));
     if (e->resize) {
-        ENG_CUDA(cudaMalloc(&e->small, (size_t)e->frame_bytes * e->max_batch));
         std::vector<int32_t> xo, yo; std::vector<int16_t> xa, ya;
         build_taps(e->sw, e->W, xo, xa);
         build_taps(e->sh, e->H, yo, ya);

@@ -1,5 +1,16 @@
-// The exact OpenCV BGR->HSV arithmetic of the warp-specialised fused pass (see hsv_math.cuh for the
-// formulas): the numerator stage runs on pixel PAIRS in packed 16-bit lanes, so most instructions serve
+// Per-pixel colour arithmetic of the fused score pass and the test hook.
+//
+// Exact restatement of OpenCV's 8-bit BGR->HSV (H in [0,180)) and BGR->YUV-Y, the arithmetic
+// behind content_detector.py:155 and histogram_detector.py:156 (see oracle/intmath.py, which is
+// pinned against cv2 over all 2^24 colours):
+//   V = max(B,G,R), d = V - min(B,G,R)
+//   S = (d * sdiv[V] + 2048) >> 12,           sdiv[i] = rint((255<<12) / i),     sdiv[0] = 0
+//   h = (V==R) ? G-B : (V==G) ? B-R+2d : R-G+4d
+//   H = (h * hdiv[d] + 2048) >> 12 (arithmetic), hdiv[i] = rint((180<<12) / (6 i)), hdiv[0] = 0
+//   H += 180 if H < 0
+//   Y = (R*4899 + G*9617 + B*1868 + 8192) >> 14
+//
+// HSV: the numerator stage runs on pixel PAIRS in packed 16-bit lanes, so most instructions serve
 // two pixels.  ("variant 7" in DESIGN.md's history of formulations.)
 //
 // The fused pass is issue-bound (one warp instruction per clock per sub-partition), so the lever is
@@ -20,16 +31,56 @@
 //     0..179 or 226..255, so a byte is negative iff its bits 7 and 6 are both set, and adding 180
 //     mod 256 equals subtracting 76 without a borrow.
 // Every step is an exact integer identity; pinned over all 2^24 colours by tests/test_gpu_parity.py
-// (psd_test_hsv, variant 7) and restated in numpy by tests/v7_model.py, which
+// (psd_test_hsv) and restated in numpy by tests/v7_model.py, which
 // tests/test_v7_model.py pins against the oracle over all 2^24 colours on the CPU.
 #pragma once
 
 #include <cuda_fp16.h>
 #include <stdint.h>
 
-#include "hsv_math.cuh"
-
 namespace psd {
+
+struct Px16 {  // 16 pixels, planar, 4 pixels per 32-bit word (pixel 4j+i in byte i of word j)
+    uint32_t h[4], s[4], v[4];
+};
+
+__device__ __forceinline__ uint32_t y_px(uint32_t b, uint32_t g, uint32_t r) {
+    return (r * 4899u + g * 9617u + b * 1868u + 8192u) >> 14;
+}
+
+// Y of pixel P straight from the packed words with IDP4A: the 14-bit coefficients are split into
+// (lo, hi) bytes, 1868 = 7*256+76, 9617 = 37*256+145, 4899 = 19*256+35, so
+// Y = (dp4a(w, lo) + 256 * dp4a(w, hi) + 8192) >> 14 with per-byte-position coefficient words.
+__host__ __device__ constexpr uint32_t y_coef_word(int word, int k0, int which) {
+    // which: 0 = lo bytes (76,145,35 for B,G,R), 1 = hi bytes (7,37,19)
+    uint32_t r = 0;
+    for (int b = 0; b < 4; ++b) {
+        const int g = 4 * word + b - k0;  // 0,1,2 -> B,G,R of this pixel
+        uint32_t c = 0;
+        if (g == 0) c = which ? 7u : 76u;
+        if (g == 1) c = which ? 37u : 145u;
+        if (g == 2) c = which ? 19u : 35u;
+        r |= c << (8 * b);
+    }
+    return r;
+}
+
+template <int P>
+__device__ __forceinline__ uint32_t y_of_pixel(const uint32_t (&w)[12]) {
+    constexpr int k0 = 3 * P, j0 = k0 >> 2, j1 = (k0 + 2) >> 2;
+    uint32_t lo = __dp4a(w[j0], y_coef_word(j0, k0, 0), 8192u);
+    uint32_t hi = __dp4a(w[j0], y_coef_word(j0, k0, 1), 0u);
+    if (j1 != j0) {
+        lo = __dp4a(w[j1], y_coef_word(j1, k0, 0), lo);
+        hi = __dp4a(w[j1], y_coef_word(j1, k0, 1), hi);
+    }
+    return (hi * 256u + lo) >> 14;
+}
+
+// byte k (0..47) of 12 packed words
+__device__ __forceinline__ uint32_t byte_of(const uint32_t (&w)[12], int k) {
+    return (w[k >> 2] >> ((k & 3) * 8)) & 0xFFu;
+}
 
 // The LUT is replicated per lane (32 copies of each of the 2 x 256 table values, 64 KB): rows of 128 B in two
 // tables (sdiv | hdiv), lane l reads word l of a row, so any 32 lookups hit 32 distinct banks.

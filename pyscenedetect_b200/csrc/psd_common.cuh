@@ -47,26 +47,21 @@ inline void count_launch(uint64_t n = 1) { g_launches.fetch_add(n, std::memory_o
 
 // ---- fused score pass (score_kernel.cu) ----
 struct ScoreArgs {
-    const uint8_t* frames;   // n frames, frame_stride apart, tightly packed rows (3*W bytes)
-    const uint8_t* prev;     // predecessor of frames[0] or nullptr
-    int64_t frame_stride;
+    const uint8_t* frames;   // n frames, frame_stride apart, tightly packed rows (3*W bytes); 16-byte aligned
+    const uint8_t* prev;     // predecessor of frames[0] or nullptr; 16-byte aligned
+    int64_t frame_stride;    // a multiple of 16
     int32_t n_frames;
     int32_t n_pixels;        // W*H
-    int32_t chunk_frames;    // frames per time chunk (generic kernel)
     int32_t n_chunks;        // time chunks (the persistent kernel splits the frames into n_chunks near-equal runs)
-    uint32_t features;       // PSD_F_* mask of the launch (device-side copy of the template argument)
+    uint32_t features;       // PSD_F_* mask of the launch (for the persistent kernel: a copy of the template argument)
     int32_t n_strips;
-    int32_t tma_ok;          // base pointers and stride 16-byte aligned
-    int32_t px_base;         // first pixel this launch covers (strips are relative to it)
-    int32_t write_has_prev;  // this launch owns the has_prev flags
     psd_frame_sums* sums;    // [n] (pre-zeroed)
     uint32_t* yhist;         // [n][256] (pre-zeroed) or nullptr
     uint32_t* vhist;         // [n][256] (pre-zeroed) or nullptr
     uint8_t* vplane;         // [n][n_pixels] or nullptr
     uint32_t shift24;        // 0x01000000, passed at run time: the kernel derives a zero the compiler cannot fold from it
 };
-int launch_score(const ScoreArgs& a, uint32_t features, bool generic_only, cudaStream_t stream);
-int score_kernel_smem_bytes();
+int launch_score(const ScoreArgs& a, uint32_t features, cudaStream_t stream);
 
 // ---- resize (resize_kernel.cu) ----
 struct ResizeTaps {  // device arrays built on the host exactly as OpenCV builds them
@@ -76,7 +71,8 @@ struct ResizeTaps {  // device arrays built on the host exactly as OpenCV builds
     const int16_t* ya;    // [dh][2]
 };
 int launch_resize(const uint8_t* src, int64_t src_frame_stride, int64_t src_row_pitch, int sw, int sh,
-                  uint8_t* dst, int dw, int dh, int64_t n, const ResizeTaps& taps, cudaStream_t stream);
+                  uint8_t* dst, int64_t dst_frame_stride, int dw, int dh, int64_t n, const ResizeTaps& taps,
+                  cudaStream_t stream);
 
 // ---- edge path (edge_kernels.cu) ----
 struct EdgeBuffers {

@@ -10,8 +10,8 @@ namespace psd {
 __global__ void __launch_bounds__(256) psd_resize_kernel(const uint8_t* __restrict__ src,
                                                          int64_t src_frame_stride,
                                                          int64_t src_row_pitch, int sw, int sh,
-                                                         uint8_t* __restrict__ dst, int dw, int dh,
-                                                         ResizeTaps taps) {
+                                                         uint8_t* __restrict__ dst, int64_t dst_frame_stride,
+                                                         int dw, ResizeTaps taps) {
     const int x = blockIdx.x * blockDim.x + threadIdx.x;
     const int y = blockIdx.y;
     const int64_t f = blockIdx.z;
@@ -24,7 +24,7 @@ __global__ void __launch_bounds__(256) psd_resize_kernel(const uint8_t* __restri
     const int b0 = taps.ya[2 * y], b1 = taps.ya[2 * y + 1];
     const uint8_t* r0 = src + f * src_frame_stride + (int64_t)sy0 * src_row_pitch;
     const uint8_t* r1 = src + f * src_frame_stride + (int64_t)sy1 * src_row_pitch;
-    uint8_t* o = dst + (f * dh + y) * (int64_t)dw * 3 + (int64_t)x * 3;
+    uint8_t* o = dst + f * dst_frame_stride + ((int64_t)y * dw + x) * 3;
 #pragma unroll
     for (int c = 0; c < 3; ++c) {
         const int h0 = r0[sx0 * 3 + c] * a0 + r0[sx1 * 3 + c] * a1;  // x2048
@@ -35,11 +35,12 @@ __global__ void __launch_bounds__(256) psd_resize_kernel(const uint8_t* __restri
 }
 
 int launch_resize(const uint8_t* src, int64_t src_frame_stride, int64_t src_row_pitch, int sw, int sh,
-                  uint8_t* dst, int dw, int dh, int64_t n, const ResizeTaps& taps, cudaStream_t stream) {
+                  uint8_t* dst, int64_t dst_frame_stride, int dw, int dh, int64_t n, const ResizeTaps& taps,
+                  cudaStream_t stream) {
     PSD_REQUIRE(n > 0 && n <= 65535, "resize batch out of range");
     dim3 grid((dw + 255) / 256, dh, (unsigned)n);
-    psd_resize_kernel<<<grid, 256, 0, stream>>>(src, src_frame_stride, src_row_pitch, sw, sh, dst, dw,
-                                                dh, taps);
+    psd_resize_kernel<<<grid, 256, 0, stream>>>(src, src_frame_stride, src_row_pitch, sw, sh, dst,
+                                                dst_frame_stride, dw, taps);
     PSD_CHECK_LAUNCH();
     count_launch();
     return PSD_OK;

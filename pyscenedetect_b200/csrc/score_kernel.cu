@@ -4,40 +4,17 @@
 //   * the 256-bin histogram of YUV-Y                          (histogram_detector.py:156-159)
 //   * (edge path) the V plane + its 256-bin histogram         (content_detector.py:231,238)
 //
-// Decomposition: spatial strip x time march.  A CTA owns STRIP_PX consecutive pixels of the
-// flattened frame and walks a chunk of consecutive frames; the previous frame's H,S,V for its
-// pixels stay in registers, so HBM traffic is one read of each BGR byte (+1 halo frame per
-// chunk).  Strips are streamed global->shared by 1-D bulk TMA (cp.async.bulk + mbarrier
-// complete_tx) into a STAGES-deep ring; each thread then pulls its 16 pixels (48 B) with three
-// conflict-free LDS.128.  Per-frame partial sums go warp-shuffle -> shared atomics -> one
-// red.global.add.u64 per CTA per frame per channel, so results are order-independent integers
-// and identical for any batching / sharding.
-#include "hsv_math.cuh"
+// The frames and the predecessor frame must be 16-byte aligned (base pointers and frame stride: the engine
+// copies any other input into an aligned buffer first).  The first P16 = P & ~15 pixels of every frame go
+// through the persistent warp-specialised kernel psd_score_ws_kernel<F>; the last P - P16 (< 16) pixels, if
+// any, through psd_score_tail_kernel with the same HSV device function.  Every partial sum reaches HBM as an
+// integer atomic, so the results are order-independent integers and identical for any batching / sharding.
 #include "hsv_half2.cuh"
 #include "psd_common.cuh"
 
 namespace psd {
 
 constexpr int kPxPerThread = 16;
-
-// generic kernel shape: table-free arithmetic, three 256-thread CTAs per SM
-struct Shape {
-    static constexpr int kThreads = 256;
-    static constexpr int kStages = 4;
-    static constexpr int kMinBlocks = 3;
-    static constexpr int kStripPx = kThreads * kPxPerThread;
-    static constexpr int kStripBytes = kStripPx * 3;
-};
-
-struct __align__(128) ScoreSmem {
-    uint8_t ring[Shape::kStages][Shape::kStripBytes];
-    unsigned long long full[Shape::kStages];
-    uint32_t acc[2][8];        // per-frame CTA partials: sadH, sadS, sadV, bgr (double-buffered)
-    uint32_t yhist[2][256];
-    uint32_t vhist[2][256];
-};
-
-int score_kernel_smem_bytes() { return (int)sizeof(ScoreSmem); }
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
     return (uint32_t)__cvta_generic_to_shared(p);
@@ -50,19 +27,6 @@ __device__ __forceinline__ void mbar_expect_tx(unsigned long long* bar, uint32_t
                  "r"(bytes)
                  : "memory");
 }
-__device__ __forceinline__ void mbar_wait(unsigned long long* bar, uint32_t parity) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "WAIT_%=:\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
-        "@p bra DONE_%=;\n\t"
-        "bra WAIT_%=;\n\t"
-        "DONE_%=:\n\t"
-        "}" ::"r"(smem_u32(bar)),
-        "r"(parity)
-        : "memory");
-}
 __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t bytes,
                                          unsigned long long* bar) {
     asm volatile(
@@ -72,212 +36,13 @@ __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t by
         : "memory");
 }
 
-// Cooperative fallback copy for partial strips / unaligned inputs (zero-fills the tail).
-template <int kThreads, int kStripBytes>
-__device__ __forceinline__ void coop_copy(uint8_t* dst, const uint8_t* src, int valid_bytes) {
-    const bool al = ((reinterpret_cast<uintptr_t>(src) & 15) == 0);
-    const int full16 = al ? (valid_bytes >> 4) : 0;
-    for (int i = threadIdx.x; i < kStripBytes / 16; i += kThreads) {
-        uint4 v = make_uint4(0, 0, 0, 0);
-        if (i < full16) {
-            v = *reinterpret_cast<const uint4*>(src + 16 * i);
-        } else {
-            uint32_t t[4] = {0, 0, 0, 0};
-            const int base = 16 * i;
-#pragma unroll
-            for (int k = 0; k < 16; ++k)
-                if (base + k < valid_bytes) t[k >> 2] |= (uint32_t)src[base + k] << ((k & 3) * 8);
-            v = make_uint4(t[0], t[1], t[2], t[3]);
-        }
-        *reinterpret_cast<uint4*>(dst + 16 * i) = v;
-    }
-}
-
-template <uint32_t F>
-__global__ void __launch_bounds__(Shape::kThreads, Shape::kMinBlocks) psd_score_kernel(const ScoreArgs a) {
-    constexpr int kThreads = Shape::kThreads, kStages = Shape::kStages;
-    constexpr int kStripPx = Shape::kStripPx, kStripBytes = Shape::kStripBytes;
-    extern __shared__ __align__(128) uint8_t smem_raw[];
-    ScoreSmem& sm = *reinterpret_cast<ScoreSmem*>(smem_raw);
-    constexpr bool kHSV = (F & PSD_F_HSV) != 0;
-    constexpr bool kSUM = (F & PSD_F_BGRSUM) != 0;
-    constexpr bool kYH = (F & PSD_F_YHIST) != 0;
-    constexpr bool kEDGE = (F & PSD_F_EDGES) != 0;
-
-    const int tid = threadIdx.x;
-    const int chunk = blockIdx.x % a.n_chunks;  // chunk-fastest: concurrent CTAs hit different frames
-    const int strip = blockIdx.x / a.n_chunks;
-    const int f0 = chunk * a.chunk_frames;
-    const int nf = min(a.chunk_frames, a.n_frames - f0);
-    const int px0 = a.px_base + strip * kStripPx;
-    const int valid_px = min(kStripPx, a.n_pixels - px0);
-    const int valid_bytes = valid_px * 3;
-    const bool use_tma = a.tma_ok && (valid_px == kStripPx);
-
-    // iteration `it` handles frame f0 - 1 + it; it == 0 is the halo (predecessor) frame
-    const bool have_halo = kHSV && (f0 > 0 || a.prev != nullptr);
-    const int it_begin = have_halo ? 0 : 1;
-    const int it_end = nf + 1;
-    const int64_t strip_off = (int64_t)px0 * 3;
-    auto frame_ptr = [&](int it) -> const uint8_t* {
-        const int fi = f0 - 1 + it;
-        return (fi < 0 ? a.prev : a.frames + (int64_t)fi * a.frame_stride) + strip_off;
-    };
-
-    for (int i = tid; i < 256; i += kThreads) {
-        sm.yhist[0][i] = sm.yhist[1][i] = 0;
-        sm.vhist[0][i] = sm.vhist[1][i] = 0;
-    }
-    if (tid < 16) sm.acc[tid >> 3][tid & 7] = 0;
-    if (tid == 0) {
-        for (int s = 0; s < kStages; ++s) mbar_init(&sm.full[s], 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncthreads();
-    if (use_tma && tid == 0) {
-        for (int s = 0; s < kStages && it_begin + s < it_end; ++s) {
-            mbar_expect_tx(&sm.full[s], kStripBytes);
-            bulk_g2s(sm.ring[s], frame_ptr(it_begin + s), kStripBytes, &sm.full[s]);
-        }
-    }
-
-    Px16 prev;
-#pragma unroll
-    for (int j = 0; j < 4; ++j) prev.h[j] = prev.s[j] = prev.v[j] = 0;
-    bool prev_valid = false;
-    const int lane = tid & 31;
-    const int my_px = px0 + tid * kPxPerThread;            // first pixel of this thread
-    const int my_valid = max(0, min(kPxPerThread, a.n_pixels - my_px));
-
-    for (int it = it_begin; it < it_end; ++it) {
-        const int k = it - it_begin;
-        const int stage = k % kStages;
-        if (use_tma) {
-            mbar_wait(&sm.full[stage], (uint32_t)((k / kStages) & 1));
-        } else {
-            coop_copy<kThreads, kStripBytes>(sm.ring[stage], frame_ptr(it), valid_bytes);
-            __syncthreads();
-        }
-        uint32_t w[12];
-        {
-            const uint4* p = reinterpret_cast<const uint4*>(sm.ring[stage] + tid * 48);
-            const uint4 q0 = p[0], q1 = p[1], q2 = p[2];
-            w[0] = q0.x; w[1] = q0.y; w[2] = q0.z; w[3] = q0.w;
-            w[4] = q1.x; w[5] = q1.y; w[6] = q1.z; w[7] = q1.w;
-            w[8] = q2.x; w[9] = q2.y; w[10] = q2.z; w[11] = q2.w;
-        }
-        __syncthreads();  // (A) every thread has drained this stage into registers
-        if (use_tma && tid == 0 && it + kStages < it_end) {
-            mbar_expect_tx(&sm.full[stage], kStripBytes);
-            bulk_g2s(sm.ring[stage], frame_ptr(it + kStages), kStripBytes, &sm.full[stage]);
-        }
-        // flush the previous iteration's CTA partials (complete: all warps added before (A))
-        const int fprev = f0 - 2 + it;  // frame index of iteration it-1
-        if (it > it_begin && fprev >= f0) {
-            const int slot = (it - 1) & 1;
-            if (tid < 4) {
-                const uint32_t v = sm.acc[slot][tid];
-                sm.acc[slot][tid] = 0;
-                if (v) atomicAdd(reinterpret_cast<unsigned long long*>(&a.sums[fprev]) + (tid < 3 ? tid : 4),
-                                 (unsigned long long)v);
-            }
-            if (kYH && tid < 256) {
-                const uint32_t v = sm.yhist[slot][tid];
-                sm.yhist[slot][tid] = 0;
-                if (v) atomicAdd(&a.yhist[(int64_t)fprev * 256 + tid], v);
-            }
-            if (kEDGE && tid < 256) {
-                const uint32_t v = sm.vhist[slot][tid];
-                sm.vhist[slot][tid] = 0;
-                if (v) atomicAdd(&a.vhist[(int64_t)fprev * 256 + tid], v);
-            }
-        }
-
-        const int fi = f0 - 1 + it;
-        const bool own = (it >= 1);  // not the halo: this CTA accounts for this frame's own sums
-        const int slot = it & 1;
-        uint32_t sad_h = 0, sad_s = 0, sad_v = 0, bsum = 0;
-        if (kHSV) {
-            Px16 cur;
-            hsv16_f32x2(w, cur);
-            if (prev_valid) {
-#pragma unroll
-                for (int j = 0; j < 4; ++j) {
-                    sad_h = __vsadu4(cur.h[j], prev.h[j]) + sad_h;
-                    sad_s = __vsadu4(cur.s[j], prev.s[j]) + sad_s;
-                    sad_v = __vsadu4(cur.v[j], prev.v[j]) + sad_v;
-                }
-            }
-            prev = cur;
-            prev_valid = true;
-            if (kEDGE && own) {
-                uint8_t* vp = a.vplane + (int64_t)fi * a.n_pixels + my_px;
-                if (my_valid == kPxPerThread && ((a.n_pixels & 15) == 0)) {
-                    *reinterpret_cast<uint4*>(vp) = make_uint4(cur.v[0], cur.v[1], cur.v[2], cur.v[3]);
-                } else {
-                    for (int p = 0; p < my_valid; ++p) vp[p] = (uint8_t)(cur.v[p >> 2] >> ((p & 3) * 8));
-                }
-                for (int p = 0; p < my_valid; ++p)
-                    atomicAdd(&sm.vhist[slot][(cur.v[p >> 2] >> ((p & 3) * 8)) & 0xFF], 1u);
-            }
-        }
-        if (own) {
-            if (kSUM) {
-#pragma unroll
-                for (int j = 0; j < 12; ++j) bsum = __dp4a(w[j], 0x01010101u, bsum);
-            }
-            if (kYH) {
-#pragma unroll
-                for (int p = 0; p < kPxPerThread; ++p) {
-                    if (p < my_valid) {
-                        const uint32_t y = y_px(byte_of(w, 3 * p), byte_of(w, 3 * p + 1), byte_of(w, 3 * p + 2));
-                        atomicAdd(&sm.yhist[slot][y], 1u);
-                    }
-                }
-            }
-            if (kHSV || kSUM) {
-                sad_h = __reduce_add_sync(0xFFFFFFFFu, sad_h);
-                sad_s = __reduce_add_sync(0xFFFFFFFFu, sad_s);
-                sad_v = __reduce_add_sync(0xFFFFFFFFu, sad_v);
-                bsum = __reduce_add_sync(0xFFFFFFFFu, bsum);
-                if (lane == 0) {
-                    if (kHSV) {
-                        atomicAdd(&sm.acc[slot][0], sad_h);
-                        atomicAdd(&sm.acc[slot][1], sad_s);
-                        atomicAdd(&sm.acc[slot][2], sad_v);
-                    }
-                    if (kSUM) atomicAdd(&sm.acc[slot][3], bsum);
-                }
-            }
-            if (a.write_has_prev && strip == 0 && tid == 0) a.sums[fi].has_prev = (fi > 0 || a.prev != nullptr) ? 1ull : 0ull;
-        }
-    }
-    __syncthreads();
-    {   // flush the last frame
-        const int fprev = f0 + nf - 1;
-        const int slot = (it_end - 1) & 1;
-        if (tid < 4) {
-            const uint32_t v = sm.acc[slot][tid];
-            if (v) atomicAdd(reinterpret_cast<unsigned long long*>(&a.sums[fprev]) + (tid < 3 ? tid : 4),
-                             (unsigned long long)v);
-        }
-        if (kYH && tid < 256) {
-            const uint32_t v = sm.yhist[slot][tid];
-            if (v) atomicAdd(&a.yhist[(int64_t)fprev * 256 + tid], v);
-        }
-        if (kEDGE && tid < 256) {
-            const uint32_t v = sm.vhist[slot][tid];
-            if (v) atomicAdd(&a.vhist[(int64_t)fprev * 256 + tid], v);
-        }
-    }
-}
-
-
 // ---------------------------------------------------------------------------------------------
-// Warp-specialised, persistent form of the same pass (full, 16-byte aligned strips only).
+// Warp-specialised, persistent kernel (the first P16 pixels of every frame).
 //
 // One CTA per SM for the whole launch: 24 consumer warps + 1 producer warp.  The work is cut into items
 // (strip of 12288 pixels x chunk of consecutive frames); CTA b walks items b, b + grid, b + 2 grid, ...
+// Within an item the previous frame's H,S,V of a thread's 16 pixels stay in registers, so HBM traffic is
+// one read of each BGR byte (+1 halo frame per item).
 // Frames travel global->shared by 1-D bulk TMA into a 4-stage ring whose stage sequence simply continues
 // from one item into the next, so the producer is always kWsStages frames ahead - also across item
 // boundaries: there is no pipeline fill / drain per item, the LUT is built once per SM and no SM idles
@@ -296,29 +61,13 @@ __global__ void __launch_bounds__(Shape::kThreads, Shape::kMinBlocks) psd_score_
 // the body is an immediate.
 // ---------------------------------------------------------------------------------------------
 // 24 consumer warps = 6 per sub-partition (25 was measured 4.5 % slower: 7/6/6/6 is unbalanced).
-// A last, partial strip is handled in the same kernel when it is a whole number of 16-pixel
-// thread slices (1080p: 168 full strips + one of 9216 px); other remainders go to the generic kernel.
-#ifndef PSD_WS_WARPS
-#define PSD_WS_WARPS 24
-#endif
-#ifndef PSD_WS_STAGES
-#define PSD_WS_STAGES 4
-#endif
-#ifndef PSD_WS_UNROLL
-#define PSD_WS_UNROLL 4  // frames per consumer loop body: 2 (stage pair toggles) or 4 (all stage offsets immediate)
-#endif
-#ifndef PSD_WS_SYNCWARP
-// 0: no __syncwarp() in front of lane 0's EMPTY arrival.  The warp is converged there (every branch of the
-// step is closed by the compiler's BSSY/BSYNC pair), its lanes' LDS results were consumed by the arithmetic
-// above and its shared REDs entered the same in-order shared-memory pipe before the arrival does; the
-// convergence check costs UMOV + BRA.DIV + NOP + three register copies per frame.
-#define PSD_WS_SYNCWARP 0
-#endif
-constexpr int kWsConsumerWarps = PSD_WS_WARPS;
+// The last strip may be partial: it holds the rest of the first P16 pixels, a whole number of 16-pixel
+// thread slices (1080p: 168 full strips + one of 9216 px).
+constexpr int kWsConsumerWarps = 24;
 constexpr int kWsConsumers = kWsConsumerWarps * 32;  // 768
 constexpr int kWsThreads = kWsConsumers + 32;        // + producer warp
-constexpr int kWsStages = PSD_WS_STAGES;
-constexpr int kWsUnroll = PSD_WS_UNROLL;
+constexpr int kWsStages = 4;
+constexpr int kWsUnroll = 4;                         // frames per consumer loop body: all stage offsets immediate
 constexpr int kWsStripPx = kWsConsumers * kPxPerThread;  // 12288 pixels
 constexpr int kWsStripBytes = kWsStripPx * 3;            // 36864 bytes
 static_assert(kWsStages % kWsUnroll == 0, "the stage ring must be a whole number of loop bodies");
@@ -344,17 +93,10 @@ __device__ __forceinline__ uint32_t sad4_acc(uint32_t a, uint32_t b, uint32_t c)
     asm volatile("vabsdiff4.u32.u32.u32.add %0, %1, %2, %3;" : "=r"(r) : "r"(a), "r"(b), "r"(c));
     return r;
 }
-#ifndef PSD_WS_WAITMODE
-#define PSD_WS_WAITMODE 0  // 0: try_wait with a suspend-time hint, 1: plain try_wait, 2: test_wait first, then try_wait
-#endif
-#ifndef PSD_WS_PAIRWAIT
-#define PSD_WS_PAIRWAIT 1  // 1: the consumer checks the FULL barriers of two consecutive frames back to back
-#endif
 // try_wait with a long suspend-time hint: the waiting warp sleeps in hardware until the phase
 // completes instead of burning issue slots of its sub-partition in a poll loop
 template <int OFF>
 __device__ __forceinline__ void mbar_wait_hint_off(uint32_t bar, uint32_t parity) {
-#if PSD_WS_WAITMODE == 0
     asm volatile(
         "{\n\t"
         ".reg .pred p;\n\t"
@@ -366,33 +108,6 @@ __device__ __forceinline__ void mbar_wait_hint_off(uint32_t bar, uint32_t parity
         "}" ::"r"(bar),
         "r"(parity), "r"(20000u), "n"(OFF)
         : "memory");
-#elif PSD_WS_WAITMODE == 1
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "WAIT_%=:\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0+%2], %1;\n\t"
-        "@p bra DONE_%=;\n\t"
-        "bra WAIT_%=;\n\t"
-        "DONE_%=:\n\t"
-        "}" ::"r"(bar),
-        "r"(parity), "n"(OFF)
-        : "memory");
-#else
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "mbarrier.test_wait.parity.shared::cta.b64 p, [%0+%3], %1;\n\t"
-        "@p bra DONE_%=;\n\t"
-        "WAIT_%=:\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0+%3], %1, %2;\n\t"
-        "@p bra DONE_%=;\n\t"
-        "bra WAIT_%=;\n\t"
-        "DONE_%=:\n\t"
-        "}" ::"r"(bar),
-        "r"(parity), "r"(20000u), "n"(OFF)
-        : "memory");
-#endif
 }
 __device__ __forceinline__ void mbar_wait_hint(unsigned long long* bar, uint32_t parity) {
     mbar_wait_hint_off<0>(smem_u32(bar), parity);
@@ -408,9 +123,6 @@ __device__ __forceinline__ void red_shared_add_off(uint32_t addr, uint32_t v) {
 template <int OFF>
 __device__ __forceinline__ void mbar_arrive_off(uint32_t bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0+%1];" ::"r"(bar), "n"(OFF) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(unsigned long long* bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
 
 // ---- work decomposition shared by host, producer and consumers ----
@@ -432,7 +144,7 @@ __device__ __forceinline__ WsItem ws_item(const ScoreArgs& a, int item) {
     w.f0 = chunk_first(chunk, a.n_frames, a.n_chunks);
     w.nf = chunk_first(chunk + 1, a.n_frames, a.n_chunks) - w.f0;
     w.px0 = strip * kWsStripPx;
-    w.valid_px = min(kWsStripPx, a.n_pixels - w.px0);
+    w.valid_px = min(kWsStripPx, a.n_pixels - w.px0) & ~15;  // the tail kernel takes the last P mod 16 pixels
     const bool have_halo = (a.features & PSD_F_HSV) && (w.f0 > 0 || a.prev != nullptr);
     w.it_begin = have_halo ? 0 : 1;
     w.walked = w.nf + 1 - w.it_begin;
@@ -456,7 +168,6 @@ __device__ __forceinline__ void ws_step(const ScoreArgs& a, WsSmem& sm, const Ws
     constexpr bool kSUM = (F & PSD_F_BGRSUM) != 0;
     constexpr bool kYH = (F & PSD_F_YHIST) != 0;
     constexpr bool kEDGE = (F & PSD_F_EDGES) != 0;
-#if PSD_WS_PAIRWAIT
     // HSV pass (issue-bound), even frame of a body: check this frame's and the next frame's barrier back to back,
     // so the latency of the second check hides behind the first; the odd frame then finds its data without asking
     // again.  The byte-sum and histogram passes are bandwidth-bound: waiting for two stages before touching the
@@ -470,9 +181,6 @@ __device__ __forceinline__ void ws_step(const ScoreArgs& a, WsSmem& sm, const Ws
     } else {
         mbar_wait_hint_off<J * 8>(ad.full, parity);
     }
-#else
-    mbar_wait_hint_off<J * 8>(ad.full, parity);
-#endif
     uint32_t w[12];
     // idle threads of a partial last strip read stale ring bytes; they never contribute (sink / mine)
     lds128_off<J * kWsStripBytes>(ad.ring, w[0], w[1], w[2], w[3]);
@@ -524,9 +232,9 @@ __device__ __forceinline__ void ws_step(const ScoreArgs& a, WsSmem& sm, const Ws
 #undef PSD_YH
         }
     }
-#if PSD_WS_SYNCWARP
-    __syncwarp();  // all lanes' shared atomics / ring reads precede the arrival
-#endif
+    // no __syncwarp() in front of lane 0's EMPTY arrival: the warp is converged here (every branch of the step
+    // is closed by the compiler's BSSY/BSYNC pair), its lanes' LDS results were consumed by the arithmetic above
+    // and its shared REDs entered the same in-order shared-memory pipe before the arrival does
     if (lane == 0) mbar_arrive_off<kWsStages * 8 + J * 8>(ad.full);
 }
 
@@ -590,7 +298,7 @@ __global__ void __launch_bounds__(kWsThreads, 1) psd_score_ws_kernel(const Score
                 mbar_expect_tx(&sm.full[stage], bytes);
                 bulk_g2s(sm.ring[stage], src, bytes, &sm.full[stage]);
             } else {
-                mbar_arrive(&sm.full[stage]);  // padding slot: complete the phase without a copy
+                mbar_arrive_off<0>(smem_u32(&sm.full[stage]));  // padding slot: complete the phase without a copy
             }
         };
         Cursor iss{(int)blockIdx.x, 0, {}}, ret{(int)blockIdx.x, 0, {}};
@@ -631,7 +339,7 @@ __global__ void __launch_bounds__(kWsThreads, 1) psd_score_ws_kernel(const Score
                         if (v) { sm.vhist[stage][b] = 0; atomicAdd(&a.vhist[(int64_t)fi * 256 + b], v); }
                     }
                 }
-                if (a.write_has_prev && ret.w.px0 == 0 && lane == 0)
+                if (ret.item < a.n_chunks && lane == 0)  // an item of strip 0
                     a.sums[fi].has_prev = (fi > 0 || a.prev != nullptr) ? 1ull : 0ull;
             }
             __syncwarp();  // the histogram zeroing above is ordered before lane 0 re-arms the stage
@@ -698,10 +406,8 @@ __global__ void __launch_bounds__(kWsThreads, 1) psd_score_ws_kernel(const Score
             const bool first_mine = active && (wi.it_begin + k >= 1);
             ws_step<F, 0>(a, sm, ad, parity, stage0, acc_first, first_mine, fbase + k, my_px, lane, zero, lut7, P0, P1);
             ws_step<F, 1>(a, sm, ad, parity, stage0, ad.acc, active, fbase + k + 1, my_px, lane, zero, lut7, P1, P0);
-            if (U == 4) {
-                ws_step<F, 2 % U>(a, sm, ad, parity, stage0, ad.acc, active, fbase + k + 2, my_px, lane, zero, lut7, P0, P1);
-                ws_step<F, 3 % U>(a, sm, ad, parity, stage0, ad.acc, active, fbase + k + 3, my_px, lane, zero, lut7, P1, P0);
-            }
+            ws_step<F, 2>(a, sm, ad, parity, stage0, ad.acc, active, fbase + k + 2, my_px, lane, zero, lut7, P0, P1);
+            ws_step<F, 3>(a, sm, ad, parity, stage0, ad.acc, active, fbase + k + 3, my_px, lane, zero, lut7, P1, P0);
             next_body(acc0);
             acc_first = ad.acc;
         }
@@ -709,15 +415,11 @@ __global__ void __launch_bounds__(kWsThreads, 1) psd_score_ws_kernel(const Score
             const int r = n - k;  // 1 .. U-1
             ws_step<F, 0>(a, sm, ad, parity, stage0, acc_first, active && (wi.it_begin + k >= 1), fbase + k, my_px,
                               lane, zero, lut7, P0, P1);
-            if (U == 4) {
-                if (r > 1) ws_step<F, 1>(a, sm, ad, parity, stage0, ad.acc, active, fbase + k + 1, my_px, lane, zero, lut7, P1, P0);
-                else ws_null_step<1>(ad, parity, lane);
-                if (r > 2) ws_step<F, 2 % U>(a, sm, ad, parity, stage0, ad.acc, active, fbase + k + 2, my_px, lane, zero, lut7, P0, P1);
-                else ws_null_step<2 % U>(ad, parity, lane);
-                ws_null_step<3 % U>(ad, parity, lane);
-            } else {
-                ws_null_step<1>(ad, parity, lane);
-            }
+            if (r > 1) ws_step<F, 1>(a, sm, ad, parity, stage0, ad.acc, active, fbase + k + 1, my_px, lane, zero, lut7, P1, P0);
+            else ws_null_step<1>(ad, parity, lane);
+            if (r > 2) ws_step<F, 2>(a, sm, ad, parity, stage0, ad.acc, active, fbase + k + 2, my_px, lane, zero, lut7, P0, P1);
+            else ws_null_step<2>(ad, parity, lane);
+            ws_null_step<3>(ad, parity, lane);
             next_body(acc0);
         }
     }
@@ -752,7 +454,7 @@ static int launch_ws(ScoreArgs a, int n_ws_strips, cudaStream_t stream) {
     a.shift24 = 0x01000000u;
     a.features = F;
     a.n_strips = n_ws_strips;
-    if (a.n_chunks <= 0) a.n_chunks = pick_chunks(a.n_frames, n_ws_strips, sm_count);
+    a.n_chunks = pick_chunks(a.n_frames, n_ws_strips, sm_count);
     if (a.n_chunks > a.n_frames) a.n_chunks = a.n_frames;
     const int64_t items = (int64_t)a.n_chunks * n_ws_strips;
     PSD_REQUIRE(items > 0 && items < 2147483647LL, "score work items out of range (%lld)", (long long)items);
@@ -775,75 +477,108 @@ static int dispatch_ws(const ScoreArgs& a, uint32_t f, int n_ws_strips, cudaStre
     }
 }
 
-template <uint32_t F>
-static int launch_one(ScoreArgs a, cudaStream_t stream) {
-    const int smem = (int)sizeof(ScoreSmem);
-    PSD_CUDA(cudaFuncSetAttribute(psd_score_kernel<F>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    a.n_strips = (a.n_pixels - a.px_base + Shape::kStripPx - 1) / Shape::kStripPx;
-    const int64_t grid = (int64_t)a.n_chunks * a.n_strips;
-    PSD_REQUIRE(grid > 0 && grid < 2147483647LL, "score grid out of range (%lld)", (long long)grid);
-    psd_score_kernel<F><<<(unsigned)grid, Shape::kThreads, smem, stream>>>(a);
+// ---------------------------------------------------------------------------------------------
+// Tail kernel: the last P - P16 (1 .. 15) pixels of every frame, one thread per frame.  The thread loads
+// this frame's and the predecessor's tail bytes into zero-filled words and runs the warp-specialised kernel's
+// HSV arithmetic on them; the zero padding is black in both frames, so the padded pixels add nothing to the
+// SADs or the byte sum, and the histograms and the V plane only take the valid pixels.
+// ---------------------------------------------------------------------------------------------
+constexpr int kTailThreads = 128;
+constexpr int kLutBytes = 256 * 64 * 4;
+
+__device__ __forceinline__ void load_tail(const uint8_t* src, int n_bytes, uint32_t (&w)[12]) {
+#pragma unroll
+    for (int j = 0; j < 12; ++j) w[j] = 0;
+#pragma unroll
+    for (int k = 0; k < 48; ++k)
+        if (k < n_bytes) w[k >> 2] |= (uint32_t)src[k] << ((k & 3) * 8);
+}
+
+__global__ void __launch_bounds__(kTailThreads) psd_score_tail_kernel(const ScoreArgs a) {
+    extern __shared__ __align__(128) float lut[];
+    const bool hsv = (a.features & PSD_F_HSV) != 0;
+    if (hsv) lut_fill7(lut, threadIdx.x, blockDim.x);
+    __syncthreads();
+    const int fi = blockIdx.x * blockDim.x + threadIdx.x;
+    if (fi >= a.n_frames) return;
+    const int p16 = a.n_pixels & ~15, n = a.n_pixels - p16;
+    const uint8_t* prev = fi > 0 ? a.frames + (int64_t)(fi - 1) * a.frame_stride : a.prev;
+    uint32_t w[12];
+    load_tail(a.frames + (int64_t)fi * a.frame_stride + (int64_t)p16 * 3, 3 * n, w);
+    unsigned long long* sums = reinterpret_cast<unsigned long long*>(&a.sums[fi]);
+    if (hsv) {
+        const LutView7 lut7 = make_lut7(smem_u32(lut), threadIdx.x & 31);
+        Px16 cur;
+        hsv16_v7(w, cur, lut7);
+        if (prev) {
+            uint32_t wp[12];
+            load_tail(prev + (int64_t)p16 * 3, 3 * n, wp);
+            Px16 pre;
+            hsv16_v7(wp, pre, lut7);
+            uint32_t sad_h = 0, sad_s = 0, sad_v = 0;
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                sad_h = __vsadu4(cur.h[j], pre.h[j]) + sad_h;
+                sad_s = __vsadu4(cur.s[j], pre.s[j]) + sad_s;
+                sad_v = __vsadu4(cur.v[j], pre.v[j]) + sad_v;
+            }
+            atomicAdd(sums + 0, (unsigned long long)sad_h);
+            atomicAdd(sums + 1, (unsigned long long)sad_s);
+            atomicAdd(sums + 2, (unsigned long long)sad_v);
+        }
+        if (a.features & PSD_F_EDGES) {
+            uint8_t* vp = a.vplane + (int64_t)fi * a.n_pixels + p16;
+            for (int p = 0; p < n; ++p) {
+                const uint32_t v = (cur.v[p >> 2] >> ((p & 3) * 8)) & 0xFFu;
+                vp[p] = (uint8_t)v;
+                atomicAdd(&a.vhist[(int64_t)fi * 256 + v], 1u);
+            }
+        }
+    }
+    if (a.features & PSD_F_BGRSUM) {
+        uint32_t bsum = 0;
+#pragma unroll
+        for (int j = 0; j < 12; ++j) bsum = __dp4a(w[j], 0x01010101u, bsum);
+        atomicAdd(sums + 4, (unsigned long long)bsum);
+    }
+    if (a.features & PSD_F_YHIST) {
+        for (int p = 0; p < n; ++p)
+            atomicAdd(&a.yhist[(int64_t)fi * 256 + y_px(byte_of(w, 3 * p), byte_of(w, 3 * p + 1), byte_of(w, 3 * p + 2))],
+                      1u);
+    }
+    if (p16 == 0) a.sums[fi].has_prev = (fi > 0 || a.prev != nullptr) ? 1ull : 0ull;  // else the ws kernel writes it
+}
+
+static int launch_tail(ScoreArgs a, uint32_t features, cudaStream_t stream) {
+    PSD_CUDA(cudaFuncSetAttribute(psd_score_tail_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kLutBytes));
+    a.features = features;
+    const int grid = (a.n_frames + kTailThreads - 1) / kTailThreads;
+    psd_score_tail_kernel<<<grid, kTailThreads, (features & PSD_F_HSV) ? kLutBytes : 0, stream>>>(a);
     PSD_CHECK_LAUNCH();
     count_launch();
     return PSD_OK;
 }
 
-static int dispatch(const ScoreArgs& a, uint32_t f, cudaStream_t s) {
-    switch (f & 15u) {
-#define CASE(F) case F: return launch_one<F>(a, s);
-        CASE(1) CASE(2) CASE(3) CASE(4) CASE(5) CASE(6) CASE(7)
-        CASE(9) CASE(11) CASE(13) CASE(15)
-#undef CASE
-        default:
-            set_error("unsupported feature mask 0x%x", f);
-            return PSD_ERR_INVALID;
-    }
-}
-
-int launch_score(const ScoreArgs& a_in, uint32_t features, bool generic_only, cudaStream_t stream) {
-    ScoreArgs a = a_in;
+int launch_score(const ScoreArgs& a, uint32_t features, cudaStream_t stream) {
     if (features & PSD_F_EDGES) features |= PSD_F_HSV;
     PSD_REQUIRE(a.n_frames > 0 && a.n_pixels > 0, "empty score launch");
     const uintptr_t al = reinterpret_cast<uintptr_t>(a.frames) | (uintptr_t)a.frame_stride |
                          reinterpret_cast<uintptr_t>(a.prev);
-    a.tma_ok = ((al & 15) == 0) ? 1 : 0;
-    a.px_base = 0;
-    a.write_has_prev = 1;
-    // generic kernel: fixed-length time chunks (one CTA per strip x chunk)
-    auto generic_chunks = [&](int frames_per_chunk) {
-        a.chunk_frames = frames_per_chunk;
-        a.n_chunks = (a.n_frames + a.chunk_frames - 1) / a.chunk_frames;
-    };
-    // persistent warp-specialised kernel on the 12288-pixel strips, generic kernel on the remainder; an
-    // unaligned input (or PSD_CFG_GENERIC_KERNEL, the cross-check switch) goes entirely through the generic kernel
-    int n_ws = (a.tma_ok && !generic_only) ? a.n_pixels / kWsStripPx : 0;
-    int covered = n_ws * kWsStripPx;
-    const int tail = a.n_pixels - covered;
-    if (n_ws > 0 && tail > 0 && (tail % 16) == 0) {  // partial last strip stays in the same kernel
-        n_ws += 1;
-        covered = a.n_pixels;
-    }
-    if (n_ws > 0) {
-        a.n_chunks = 0;  // launch_ws balances the time chunks over the SMs
-        int rc = dispatch_ws(a, features, n_ws, stream);
+    PSD_REQUIRE((al & 15) == 0, "score pass input is not 16-byte aligned");
+    const int p16 = a.n_pixels & ~15;
+    if (p16 > 0) {
+        const int rc = dispatch_ws(a, features, (p16 + kWsStripPx - 1) / kWsStripPx, stream);
         if (rc) return rc;
-        a.px_base = covered;
-        a.write_has_prev = 0;
-        if (a.px_base >= a.n_pixels) return PSD_OK;
-        generic_chunks(16);  // the remainder is a sliver of the frame: short time chunks give it enough CTAs
-    } else {
-        generic_chunks(64);
     }
-    return dispatch(a, features, stream);
+    if (p16 < a.n_pixels) return launch_tail(a, features, stream);
+    return PSD_OK;
 }
 
-// ---- test hook: the same device functions on a flat pixel array ----
-// FAST = the warp-specialised kernel's arithmetic (hsv_half2.cuh), else the generic kernel's (hsv_math.cuh)
-template <bool FAST>
+// ---- test hook: the fused pass's device functions on a flat pixel array ----
 __global__ void psd_test_hsv_kernel(const uint8_t* bgr, int64_t n_groups, uint8_t* h, uint8_t* s,
                                     uint8_t* v, uint8_t* y) {
     extern __shared__ __align__(128) float lutmem[];
-    if (FAST) lut_fill7(lutmem, threadIdx.x, blockDim.x);
+    lut_fill7(lutmem, threadIdx.x, blockDim.x);
     const LutView7 lut7 = make_lut7(smem_u32(lutmem), threadIdx.x & 31);
     __syncthreads();
     for (int64_t g = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; g < n_groups;
@@ -855,8 +590,7 @@ __global__ void psd_test_hsv_kernel(const uint8_t* bgr, int64_t n_groups, uint8_
         w[4] = q1.x; w[5] = q1.y; w[6] = q1.z; w[7] = q1.w;
         w[8] = q2.x; w[9] = q2.y; w[10] = q2.z; w[11] = q2.w;
         Px16 o;
-        if (FAST) hsv16_v7(w, o, lut7);
-        else hsv16_f32x2(w, o);
+        hsv16_v7(w, o, lut7);
         *reinterpret_cast<uint4*>(h + g * 16) = make_uint4(o.h[0], o.h[1], o.h[2], o.h[3]);
         *reinterpret_cast<uint4*>(s + g * 16) = make_uint4(o.s[0], o.s[1], o.s[2], o.s[3]);
         *reinterpret_cast<uint4*>(v + g * 16) = make_uint4(o.v[0], o.v[1], o.v[2], o.v[3]);
@@ -865,28 +599,15 @@ __global__ void psd_test_hsv_kernel(const uint8_t* bgr, int64_t n_groups, uint8_
     }
 }
 
-template <bool FAST>
-static int run_test_hsv(const uint8_t* d_bgr, int64_t groups, uint8_t* dh, uint8_t* ds, uint8_t* dv,
-                        uint8_t* dy) {
-    const int smem = FAST ? 65536 : 0;
-    int dev = 0, sm_count = 0;
-    PSD_CUDA(cudaGetDevice(&dev));
-    PSD_CUDA(cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, dev));
-    PSD_CUDA(cudaFuncSetAttribute(psd_test_hsv_kernel<FAST>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    psd_test_hsv_kernel<FAST><<<sm_count * 2, 256, smem>>>(d_bgr, groups, dh, ds, dv, dy);
-    PSD_CHECK_LAUNCH();
-    return PSD_OK;
-}
-
 }  // namespace psd
 
 extern "C" int psd_test_hsv(int device, const uint8_t* bgr_host, int64_t n_pixels, uint8_t* h_out,
-                            uint8_t* s_out, uint8_t* v_out, uint8_t* y_out, int variant) {
+                            uint8_t* s_out, uint8_t* v_out, uint8_t* y_out) {
     using namespace psd;
     PSD_REQUIRE(n_pixels > 0 && (n_pixels % 16) == 0, "n_pixels must be a positive multiple of 16");
-    PSD_REQUIRE(variant == 2 || variant == 7,
-                "unknown hsv arithmetic %d (2 = generic kernel, 7 = warp-specialised kernel)", variant);
     PSD_CUDA(cudaSetDevice(device));
+    int sm_count = 0;
+    PSD_CUDA(cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, device));
     uint8_t *d_bgr = nullptr, *d_out = nullptr;
     PSD_CUDA(cudaMalloc(&d_bgr, (size_t)n_pixels * 3));
     PSD_CUDA(cudaMalloc(&d_out, (size_t)n_pixels * 4));
@@ -895,9 +616,9 @@ extern "C" int psd_test_hsv(int device, const uint8_t* bgr_host, int64_t n_pixel
     uint8_t* ds = d_out + n_pixels;
     uint8_t* dv = d_out + 2 * n_pixels;
     uint8_t* dy = d_out + 3 * n_pixels;
-    int rc = variant == 7 ? run_test_hsv<true>(d_bgr, n_pixels / 16, dh, ds, dv, dy)
-                          : run_test_hsv<false>(d_bgr, n_pixels / 16, dh, ds, dv, dy);
-    if (rc) return rc;
+    PSD_CUDA(cudaFuncSetAttribute(psd_test_hsv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kLutBytes));
+    psd_test_hsv_kernel<<<sm_count * 2, 256, kLutBytes>>>(d_bgr, n_pixels / 16, dh, ds, dv, dy);
+    PSD_CHECK_LAUNCH();
     count_launch();
     PSD_CUDA(cudaDeviceSynchronize());
     PSD_CUDA(cudaMemcpy(h_out, dh, (size_t)n_pixels, cudaMemcpyDeviceToHost));

@@ -75,8 +75,7 @@ class Engine:
 
     def __init__(self, src_width: int, src_height: int, features: int, width: int | None = None,
                  height: int | None = None, device: int = 0, max_batch: int = 64,
-                 edge_kernel_size: int = 0, generic_kernel: bool = False, hash_size: int = 8,
-                 hash_lowpass: int = 2):
+                 edge_kernel_size: int = 0, hash_size: int = 8, hash_lowpass: int = 2):
         self._lib = _capi.load()
         cfg = _capi.PsdConfig()
         cfg.struct_size = C.sizeof(_capi.PsdConfig)
@@ -87,7 +86,6 @@ class Engine:
         cfg.features = int(features)
         cfg.edge_kernel_size = int(edge_kernel_size)
         cfg.max_batch = int(max_batch)
-        cfg.flags = _capi.CFG_GENERIC_KERNEL if generic_kernel else 0  # cross-check switch (tests)
         cfg.hash_size, cfg.hash_lowpass = int(hash_size), int(hash_lowpass)
         self.hash_size = int(hash_size)
         h = C.c_void_p()

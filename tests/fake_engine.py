@@ -14,7 +14,7 @@ from pyscenedetect_b200._capi import F_BGRSUM, F_EDGES, F_HASH, F_HSV, F_YHIST, 
 
 class OracleEngine:
     def __init__(self, src_width, src_height, features, width=None, height=None, device=0,
-                 max_batch=64, edge_kernel_size=0, generic_kernel=False, hash_size=8, hash_lowpass=2):
+                 max_batch=64, edge_kernel_size=0, hash_size=8, hash_lowpass=2):
         self.src_width, self.src_height = src_width, src_height
         self.width = width if width is not None else src_width
         self.height = height if height is not None else src_height

@@ -133,7 +133,7 @@ CASES = [
          kw=dict(weights=(0.5, 0.25, 1.0, 2.0), kernel_size=3), mode="direct", stats=True,
          fps=30.0),
     # width not a multiple of 32 / 16 / 4: the bit-packed dilation has padding bits in every row's last
-    # word and the fused pass takes its generic (unaligned) path
+    # word, and the fused pass scores an aligned copy and sends the last pixels of each frame to its tail kernel
     dict(name="content_edges_odd_size", gen=(140, 131, 97, 12, 20, 50, 30), det="content",
          kw=dict(weights=(1.0, 1.0, 1.0, 1.0), threshold=28.0), mode="direct", stats=True, fps=30.0),
     dict(name="content_luma_only", gen=(200, 160, 90, 7, 20, 60, 30), det="content",

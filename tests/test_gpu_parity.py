@@ -3,6 +3,7 @@ golden fixtures recorded from the real reference.  Integer-derived metrics are c
 bit-exactly; `hist_diff` (cv2's SIMD summation order is not reproduced) to 1e-9, far inside
 the 1e-4 tolerance BASELINE.json states."""
 
+import ctypes as C
 import hashlib
 import io
 
@@ -122,8 +123,7 @@ def test_batched_scene_manager_matches_reference_golden(lib, name, batch):
         _check_stats(case, stats, frames.shape[0])
 
 
-@pytest.mark.parametrize("variant", [2, 7])  # 2 = generic kernel arithmetic, 7 = warp-specialised kernel arithmetic
-def test_hsv_and_y_exhaustive_2_24(lib, variant):
+def test_hsv_and_y_exhaustive_2_24(lib):
     """Every BGR colour through the device functions of the fused kernel vs cv2."""
     v = np.arange(1 << 24, dtype=np.uint32)
     img = np.stack([(v & 255), (v >> 8) & 255, (v >> 16) & 255], axis=-1).astype(np.uint8)
@@ -131,7 +131,7 @@ def test_hsv_and_y_exhaustive_2_24(lib, variant):
     h, s, val, y = (np.empty(n, np.uint8) for _ in range(4))
     from pyscenedetect_b200 import _capi
     _capi.check(lib.psd_test_hsv(0, img.ctypes.data, n, h.ctypes.data, s.ctypes.data,
-                                 val.ctypes.data, y.ctypes.data, variant))
+                                 val.ctypes.data, y.ctypes.data))
     want = cv2.cvtColor(img.reshape(4096, 4096, 3), cv2.COLOR_BGR2HSV).reshape(-1, 3)
     assert np.array_equal(h, want[:, 0])
     assert np.array_equal(s, want[:, 1])
@@ -155,8 +155,9 @@ def test_device_generator_matches_numpy(lib):
 
 @pytest.mark.parametrize("shape", [(160, 90), (131, 97), (17, 5), (1, 1), (4096, 3), (640, 360)])
 def test_integer_sums_any_shape(lib, shape):
-    """Raw integer outputs vs the oracle for aligned, unaligned, tiny and partial-strip sizes."""
-    from pyscenedetect_b200.engine import F_BGRSUM, F_HSV, F_YHIST, Engine
+    """Raw integer outputs vs the oracle for aligned, unaligned, tiny and partial-strip sizes; the same frames
+    submitted from device memory at a base pointer that is not 16-byte aligned give the same bytes."""
+    from pyscenedetect_b200.engine import F_BGRSUM, F_HSV, F_YHIST, DeviceBuffer, Engine
     w, h = shape
     rng = np.random.default_rng(w * 1000 + h)
     frames = rng.integers(0, 256, size=(9, h, w, 3), dtype=np.uint8)
@@ -164,6 +165,14 @@ def test_integer_sums_any_shape(lib, shape):
     eng.submit(frames)
     sums = eng.read_sums()
     hist = eng.read_yhist()
+    buf = DeviceBuffer(frames.nbytes + 16)
+    buf.upload(frames, offset=1)
+    dev = Engine(w, h, F_HSV | F_BGRSUM | F_YHIST, max_batch=4)
+    dev.submit_device(buf.ptr + 1, frames.shape[0])
+    assert dev.read_sums().tobytes() == sums.tobytes()
+    assert np.array_equal(dev.read_yhist(), hist)
+    dev.close()
+    buf.close()
     prev = None
     for i, f in enumerate(frames):
         hsv = M.bgr_to_hsv(f)
@@ -203,32 +212,34 @@ def test_strided_crop_view_and_batch_invariance(lib):
 
 
 def test_halo_shards_equal_serial(lib):
-    """Contiguous time shards with a one-frame halo reproduce the serial run exactly."""
+    """Contiguous time shards with a one-frame halo reproduce the serial run exactly.  (131x97: a frame of
+    12707 pixels, whose last 3 go through the tail kernel, staged at a stride that is not 16-byte aligned.)"""
     from pyscenedetect_b200.engine import F_BGRSUM, F_EDGES, F_HSV, F_YHIST, Engine
     from pyscenedetect_b200.synth import ScenePlan, render_frames
-    frames = render_frames(ScenePlan(60, seed=2, min_len=10, max_len=25).params, 192, 108)
-    feats = F_HSV | F_BGRSUM | F_YHIST | F_EDGES
-    serial = Engine(192, 108, feats)
-    serial.submit(frames)
-    want_s, want_h = serial.read_sums(), serial.read_yhist()
-    want_c = serial.scan_hist_correl(256)
-    for shards in (2, 3, 4):
-        bounds = [round(i * 60 / shards) for i in range(shards + 1)]
-        got_s, got_h, got_c = [], [], []
-        for r in range(shards):
-            eng = Engine(192, 108, feats)
-            if r > 0:
-                eng.set_halo(frames[bounds[r] - 1])
-            eng.submit(frames[bounds[r]:bounds[r + 1]])
-            got_s.append(eng.read_sums())
-            got_h.append(eng.read_yhist())
-            got_c.append(eng.scan_hist_correl(256))
-            eng.close()
-        assert np.concatenate(got_s).tobytes() == want_s.tobytes()
-        assert np.array_equal(np.concatenate(got_h), want_h)
-        c = np.concatenate(got_c)
-        assert np.array_equal(c[1:], want_c[1:]) and np.isnan(c[0]) and np.isnan(want_c[0])
-    serial.close()
+    for w, h in ((192, 108), (131, 97)):
+        frames = render_frames(ScenePlan(60, seed=2, min_len=10, max_len=25).params, w, h)
+        feats = F_HSV | F_BGRSUM | F_YHIST | F_EDGES
+        serial = Engine(w, h, feats)
+        serial.submit(frames)
+        want_s, want_h = serial.read_sums(), serial.read_yhist()
+        want_c = serial.scan_hist_correl(256)
+        for shards in (2, 3, 4):
+            bounds = [round(i * 60 / shards) for i in range(shards + 1)]
+            got_s, got_h, got_c = [], [], []
+            for r in range(shards):
+                eng = Engine(w, h, feats)
+                if r > 0:
+                    eng.set_halo(frames[bounds[r] - 1])
+                eng.submit(frames[bounds[r]:bounds[r + 1]])
+                got_s.append(eng.read_sums())
+                got_h.append(eng.read_yhist())
+                got_c.append(eng.scan_hist_correl(256))
+                eng.close()
+            assert np.concatenate(got_s).tobytes() == want_s.tobytes(), (w, h, shards)
+            assert np.array_equal(np.concatenate(got_h), want_h)
+            c = np.concatenate(got_c)
+            assert np.array_equal(c[1:], want_c[1:]) and np.isnan(c[0]) and np.isnan(want_c[0])
+        serial.close()
 
 
 @pytest.mark.parametrize("src,dst", [((640, 360), (256, 144)), ((1920, 1080), (256, 144)),
@@ -422,39 +433,43 @@ def test_errors_are_loud(lib):
     eng.close()
     with pytest.raises(ValueError):
         Engine(16, 9, 0)
+    from pyscenedetect_b200 import _capi
+    cfg = _capi.PsdConfig(struct_size=C.sizeof(_capi.PsdConfig), src_width=16, src_height=9, width=16, height=9,
+                          features=F_HSV, max_batch=1, flags=1)
+    h = C.c_void_p()
+    assert lib.psd_engine_create(C.byref(cfg), C.byref(h)) == _capi.PSD_ERR_INVALID  # no flags are defined
+    assert not h.value
 
 
 @pytest.mark.parametrize("shape", [(1920, 1080), (640, 360), (3840, 2160), (1000, 37)])
-def test_kernel_variants_agree_at_full_size(lib, shape):
-    """The persistent warp-specialised kernel (+ generic remainder) and the generic kernel alone produce
-    the same integer sums/histograms on full-size frames; the first frames are also checked against
-    the integer oracle.  (1920x1080 and 3840x2160 exercise the warp-specialised strips, 1000x37 the
-    partial strip + remainder split.)"""
-    from pyscenedetect_b200.engine import F_BGRSUM, F_EDGES, F_HSV, F_YHIST, DeviceBuffer, Engine, synth_frames_device
+def test_score_pass_matches_oracle_at_full_size(lib, shape):
+    """Every frame's integer sums and Y histogram from a device-resident sequence vs the integer oracle.
+    (1920x1080 and 3840x2160 exercise the full and partial warp-specialised strips; 1000x37, submitted at
+    its tight, not 16-byte aligned frame stride, the aligned copy and the tail kernel for the last 8 pixels.)"""
+    from pyscenedetect_b200.engine import F_BGRSUM, F_HSV, F_YHIST, DeviceBuffer, Engine, synth_frames_device
     from pyscenedetect_b200.synth import ScenePlan
     w, h = shape
     n = 70 if w * h < 3000000 else 12   # > one 64-frame chunk where memory allows
     plan = ScenePlan(n, seed=9, min_len=5, max_len=12, noise_shift=29)
     buf = DeviceBuffer(n * w * h * 3)
     synth_frames_device(buf.ptr, plan.params, w, h)
-    ref = None
-    for variant in ("fused", "generic"):
-        eng = Engine(w, h, F_HSV | F_BGRSUM | F_YHIST, max_batch=128, generic_kernel=(variant == "generic"))
-        eng.submit_device(buf.ptr, n)
-        got = (eng.read_sums().tobytes(), eng.read_yhist().tobytes())
-        if ref is None:
-            ref = got
-            first = buf.download(3 * w * h * 3).reshape(3, h, w, 3)
-            sums = eng.read_sums()
-            hsv = [M.bgr_to_hsv(f) for f in first]
-            for i in (1, 2):
-                assert int(sums["sad_hue"][i]) == M.sad(hsv[i][0], hsv[i - 1][0])
-                assert int(sums["sad_sat"][i]) == M.sad(hsv[i][1], hsv[i - 1][1])
-                assert int(sums["sad_lum"][i]) == M.sad(hsv[i][2], hsv[i - 1][2])
-                assert int(sums["bgr_sum"][i]) == int(first[i].astype(np.int64).sum())
-        assert got == ref, f"variant {variant} differs"
-        eng.close()
+    eng = Engine(w, h, F_HSV | F_BGRSUM | F_YHIST, max_batch=128)
+    eng.submit_device(buf.ptr, n)
+    sums, hist = eng.read_sums(), eng.read_yhist()
+    eng.close()
+    frames = buf.download(n * w * h * 3).reshape(n, h, w, 3)
     buf.close()
+    prev = None
+    for i, f in enumerate(frames):
+        hsv = M.bgr_to_hsv(f)
+        want = [M.sad(hsv[c], prev[c]) for c in range(3)] if prev is not None else [0, 0, 0]
+        got = [int(sums[k][i]) for k in ("sad_hue", "sad_sat", "sad_lum")]
+        assert got == want, (i, got, want)
+        assert int(sums["sad_edges"][i]) == 0
+        assert int(sums["bgr_sum"][i]) == int(f.astype(np.int64).sum()), i
+        assert int(sums["has_prev"][i]) == (1 if i else 0)
+        assert np.array_equal(hist[i], np.bincount(M.bgr_to_y(f).ravel(), minlength=256)), i
+        prev = hsv
 
 
 def test_full_size_properties_1080p(lib):
