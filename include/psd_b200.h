@@ -187,6 +187,50 @@ int psd_cuts_threshold(const double* average, int64_t n, int64_t first_frame, do
                        int32_t method_ceiling, double fade_bias, int64_t min_frames, int32_t add_final_scene,
                        int64_t* cuts, int32_t* count, int32_t cap, void* stream);
 
+/* ---- parameter sweep: every cell of a detector-parameter grid over one scored video ---- */
+/* cell kinds: which automaton a cell runs, over which metric array(s) */
+#define PSD_SWEEP_CONTENT 0   /* FlashFilter over content_val >= threshold (content_detector.py:210, detector.py:160-224) */
+#define PSD_SWEEP_ADAPTIVE 1  /* adaptive_detector.py:134-143: metric = ratio, metric2 = content_val */
+#define PSD_SWEEP_THRESHOLD 2 /* threshold_detector.py:113-191: metric = average_rgb */
+#define PSD_SWEEP_HISTOGRAM 3 /* histogram_detector.py:87-112: metric = hist correl, threshold = 1 - t clamped */
+#define PSD_SWEEP_HASH 4      /* hash_detector.py:79-109: metric = hash_dist (NaN = no predecessor) */
+#define PSD_SWEEP_MAX_TOLERANCES 8
+/* One grid cell (64 bytes): the arguments the matching psd_cuts_* call takes.  Metric arrays are DEVICE
+ * pointers of n doubles (the psd_scan_* outputs); cells that share an array should be adjacent so that
+ * the 32 cells of a warp read each frame's value with one broadcast load. */
+typedef struct psd_sweep_cell {
+    int32_t kind;             /* PSD_SWEEP_* */
+    int32_t mode;             /* CONTENT: 0 = MERGE, 1 = SUPPRESS; THRESHOLD: 1 = Method.CEILING; else 0 */
+    const double* metric;     /* see the kinds */
+    const double* metric2;    /* ADAPTIVE: content_val; else NULL */
+    double threshold;         /* CONTENT / THRESHOLD / HISTOGRAM / HASH threshold, ADAPTIVE adaptive_threshold */
+    double min_content_val;   /* ADAPTIVE */
+    double fade_bias;         /* THRESHOLD */
+    int64_t min_frames;       /* min_scene_len in frames, as for psd_cuts_* */
+    int32_t window;           /* ADAPTIVE window_width (>= 1) */
+    int32_t add_final_scene;  /* THRESHOLD */
+} psd_sweep_cell;
+/* benchmark/sweep.py:142-187 runs one SceneManager + detector per cell; here one thread per cell walks
+ * the metric arrays with the automaton psd_cuts_* runs.  cells is a HOST array (validated, then copied
+ * on `stream`); cuts[n_cells][cap] and count[n_cells] are DEVICE arrays: cell k's cut frames
+ * (first_frame + index, in emission order) and how many it found (may exceed cap: only cap are stored). */
+int psd_sweep_cuts(const psd_sweep_cell* cells, int32_t n_cells, int64_t n, int64_t first_frame, int64_t* cuts,
+                   int32_t* count, int32_t cap, void* stream);
+/* benchmark/evaluator.py:227-331 (score_video) for every (cell, tolerance), on the cells' cut lists from
+ * psd_sweep_cuts.  Each cell's list is first turned, in place, into the predicted list of
+ * benchmark/sweep.py:169 (`scene[1]` of SceneManager.get_scene_list()): sorted unique cuts followed by
+ * end_frame, or nothing when the cell has no cut; out_n_pred[cell] is its length (-1: count > cap, the
+ * cell overflowed and is not scored).  Fade intervals ([n_fades][2], inclusive) match first-hit in the
+ * order given; the remaining predictions match the strictly increasing gt_cuts greedily by distance.
+ * out_hard[n_cells][n_tol][5] = matched, false_positives, missed, offset_sum, offset_count;
+ * out_fades[n_cells][3] = matched, false_positives, missed.  tolerances is a HOST array (n_tol <=
+ * PSD_SWEEP_MAX_TOLERANCES); every other pointer is a DEVICE pointer.  workspace holds the matching
+ * bitmaps: n_cells * n_tol * 4 * (ceil((cap + 1) / 32) + ceil(n_gt / 32) + ceil(n_fades / 32)) bytes. */
+int psd_sweep_eval(int64_t* cuts, const int32_t* count, int32_t n_cells, int32_t cap, int64_t end_frame,
+                   const int64_t* gt_cuts, int32_t n_gt, const int64_t* fades, int32_t n_fades,
+                   const int32_t* tolerances, int32_t n_tol, void* workspace, size_t workspace_bytes,
+                   int32_t* out_n_pred, int64_t* out_hard, int64_t* out_fades, void* stream);
+
 /* host-convenience wrappers: engine-owned sums -> host arrays (numpy), implies sync */
 int psd_engine_scan_content_host(psd_engine* e, int64_t first, int64_t n, const double weights[4],
                                  double weight_abs_sum, double* out_components,

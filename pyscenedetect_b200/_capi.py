@@ -48,6 +48,33 @@ class PsdConfig(C.Structure):
     ]
 
 
+SWEEP_CONTENT = 0
+SWEEP_ADAPTIVE = 1
+SWEEP_THRESHOLD = 2
+SWEEP_HISTOGRAM = 3
+SWEEP_HASH = 4
+SWEEP_MAX_TOLERANCES = 8
+
+
+class PsdSweepCell(C.Structure):
+    """psd_sweep_cell: one grid cell of psd_sweep_cuts (64 bytes)."""
+    _fields_ = [
+        ("kind", C.c_int32),
+        ("mode", C.c_int32),
+        ("metric", C.c_void_p),
+        ("metric2", C.c_void_p),
+        ("threshold", C.c_double),
+        ("min_content_val", C.c_double),
+        ("fade_bias", C.c_double),
+        ("min_frames", C.c_int64),
+        ("window", C.c_int32),
+        ("add_final_scene", C.c_int32),
+    ]
+
+
+assert C.sizeof(PsdSweepCell) == 64
+
+
 # numpy view of psd_frame_sums (64 bytes)
 SUMS_DTYPE = np.dtype([
     ("sad_hue", "<u8"), ("sad_sat", "<u8"), ("sad_lum", "<u8"), ("sad_edges", "<u8"),
@@ -109,6 +136,9 @@ SIGNATURES = {
     "psd_cuts_histogram": (C.c_int, [_vp, _i64, _i64, _dbl, _i64, _vp, _vp, _i32, _vp]),
     "psd_cuts_hash": (C.c_int, [_vp, _i64, _i64, _dbl, _i64, _vp, _vp, _i32, _vp]),
     "psd_cuts_threshold": (C.c_int, [_vp, _i64, _i64, _dbl, _i32, _dbl, _i64, _i32, _vp, _vp, _i32, _vp]),
+    "psd_sweep_cuts": (C.c_int, [_vp, _i32, _i64, _i64, _vp, _vp, _i32, _vp]),
+    "psd_sweep_eval": (C.c_int, [_vp, _vp, _i32, _i32, _i64, _vp, _i32, _vp, _i32, _vp, _i32, _vp, C.c_size_t,
+                                 _vp, _vp, _vp, _vp]),
     "psd_engine_scan_content_host": (C.c_int, [_vp, _i64, _i64, _dp, _dbl, _vp, _vp]),
     "psd_engine_scan_adaptive_host": (C.c_int, [_vp, _vp, _i64, _i32, _dbl, _vp]),
     "psd_engine_scan_average_host": (C.c_int, [_vp, _i64, _i64, _vp]),

@@ -3,63 +3,24 @@
 // every `min_scene_len` form into a frame count with FrameTimecode's own rounding rule,
 // common.py:480-486,627-638).  One thread walks the sequence: these are strictly sequential
 // automata over a few bytes per frame; at 100k frames they take ~1 ms and keep the cut list on the
-// device next to the scores.
+// device next to the scores.  The automata themselves are the device functions of cut_automata.cuh,
+// which psd_sweep_cuts (sweep_kernels.cu) runs once per grid cell.
 //   psd_cuts_flash_filter   detector.py:160-224   (FlashFilter MERGE / SUPPRESS over score >= threshold)
 //   psd_cuts_adaptive       adaptive_detector.py:134-143
 //   psd_cuts_histogram      histogram_detector.py:87-112
 //   psd_cuts_hash           hash_detector.py:79-109
 //   psd_cuts_threshold      threshold_detector.py:113-168, 170-191
-#include "psd_common.cuh"
+#include "cut_automata.cuh"
 
 namespace psd {
-
-__device__ __forceinline__ void push_cut(int64_t* cuts, int32_t* count, int32_t cap, int64_t frame) {
-    const int32_t i = *count;
-    if (i < cap) cuts[i] = frame;
-    *count = i + 1;
-}
 
 __global__ void psd_cuts_flash_filter_kernel(const uint8_t* __restrict__ above, int64_t n, int64_t first_frame,
                                              int64_t min_frames, int mode, int64_t* cuts, int32_t* count,
                                              int32_t cap) {
     if (blockIdx.x != 0 || threadIdx.x != 0) return;
-    *count = 0;
-    if (min_frames <= 0) {  // filter disabled: every above-threshold frame is a cut (detector.py:161-162)
-        for (int64_t i = 0; i < n; ++i)
-            if (above[i]) push_cut(cuts, count, cap, first_frame + i);
-        return;
-    }
-    int64_t last_above = first_frame;  // initialised to the first frame seen (detector.py:163-164)
-    bool merge_enabled = false, merge_triggered = false;
-    int64_t merge_start = 0;
-    for (int64_t i = 0; i < n; ++i) {
-        const int64_t t = first_frame + i;
-        const bool a = above[i] != 0;
-        const bool met = (t - last_above) >= min_frames;
-        if (mode == 1) {  // SUPPRESS (detector.py:171-187)
-            if (a && met) {
-                last_above = t;
-                push_cut(cuts, count, cap, t);
-            }
-            continue;
-        }
-        if (a) last_above = t;  // MERGE (detector.py:189-224)
-        if (merge_triggered) {
-            if (met && !a && (last_above - merge_start) >= min_frames) {
-                merge_triggered = false;
-                push_cut(cuts, count, cap, last_above);
-            }
-            continue;
-        }
-        if (!a) continue;
-        if (met) {
-            merge_enabled = true;
-            push_cut(cuts, count, cap, t);
-        } else if (merge_enabled) {
-            merge_triggered = true;
-            merge_start = t;
-        }
-    }
+    CutSink out{cuts, cap, 0};
+    flash_filter_cuts([&](int64_t i) { return above[i] != 0; }, n, first_frame, min_frames, mode, out);
+    *count = out.n;
 }
 
 __global__ void psd_cuts_adaptive_kernel(const double* __restrict__ ratio, const double* __restrict__ score,
@@ -67,48 +28,27 @@ __global__ void psd_cuts_adaptive_kernel(const double* __restrict__ ratio, const
                                          double min_content_val, int64_t min_frames, int64_t* cuts,
                                          int32_t* count, int32_t cap) {
     if (blockIdx.x != 0 || threadIdx.x != 0) return;
-    *count = 0;
-    int64_t last_cut = first_frame;  // adaptive_detector.py:108-109
-    for (int64_t i = window; i + window < n; ++i) {  // target i is decided when frame i+w arrives
-        const bool met = ratio[i] >= adaptive_threshold && score[i] >= min_content_val;
-        const int64_t current = first_frame + i + window;
-        if (met && (current - last_cut) >= min_frames) {
-            last_cut = first_frame + i;
-            push_cut(cuts, count, cap, first_frame + i);
-        }
-    }
+    CutSink out{cuts, cap, 0};
+    adaptive_cuts(ratio, score, n, first_frame, window, adaptive_threshold, min_content_val, min_frames, out);
+    *count = out.n;
 }
 
 __global__ void psd_cuts_histogram_kernel(const double* __restrict__ correl, int64_t n, int64_t first_frame,
                                           double threshold, int64_t min_frames, int64_t* cuts, int32_t* count,
                                           int32_t cap) {
     if (blockIdx.x != 0 || threadIdx.x != 0) return;
-    *count = 0;
-    int64_t last_cut = first_frame;  // histogram_detector.py:87-88 (a FrameTimecode is always truthy)
-    for (int64_t i = 1; i < n; ++i) {    // frame 0 has nothing to compare with
-        const int64_t t = first_frame + i;
-        if (correl[i] <= threshold && (t - last_cut) >= min_frames) {
-            push_cut(cuts, count, cap, t);
-            last_cut = t;
-        }
-    }
+    CutSink out{cuts, cap, 0};
+    histogram_cuts(correl, n, first_frame, threshold, min_frames, out);
+    *count = out.n;
 }
 
 __global__ void psd_cuts_hash_kernel(const double* __restrict__ dist, int64_t n, int64_t first_frame,
                                      double threshold, int64_t min_frames, int64_t* cuts, int32_t* count,
                                      int32_t cap) {
     if (blockIdx.x != 0 || threadIdx.x != 0) return;
-    *count = 0;
-    int64_t last_cut = first_frame;  // hash_detector.py:79-80
-    for (int64_t i = 0; i < n; ++i) {
-        const double d = dist[i];
-        if (d != d) continue;         // NaN: no predecessor frame (hash_detector.py:83)
-        const int64_t t = first_frame + i;
-        if (d >= threshold && (t - last_cut) >= min_frames) {
-            push_cut(cuts, count, cap, t);
-            last_cut = t;
-        }
-    }
+    CutSink out{cuts, cap, 0};
+    hash_cuts(dist, n, first_frame, threshold, min_frames, out);
+    *count = out.n;
 }
 
 __global__ void psd_cuts_threshold_kernel(const double* __restrict__ avg, int64_t n, int64_t first_frame,
@@ -116,30 +56,9 @@ __global__ void psd_cuts_threshold_kernel(const double* __restrict__ avg, int64_
                                           int64_t min_frames, int add_final_scene, int64_t* cuts,
                                           int32_t* count, int32_t cap) {
     if (blockIdx.x != 0 || threadIdx.x != 0) return;
-    *count = 0;
-    if (n <= 0) return;
-    int64_t last_scene_cut = first_frame, fade_frame = first_frame;
-    bool fade_in = !(avg[0] < threshold);  // first frame: 'out' iff avg < threshold (any method)
-    for (int64_t i = 1; i < n; ++i) {
-        const int64_t t = first_frame + i;
-        const double v = avg[i];
-        const bool below = method_ceiling ? (v >= threshold) : (v < threshold);  // "faded out" condition
-        if (fade_in && below) {
-            fade_in = false;
-            fade_frame = t;
-        } else if (!fade_in && !below) {
-            if ((t - last_scene_cut) >= min_frames) {
-                const double half = __dmul_rn((double)(t - fade_frame), __dadd_rn(1.0, fade_bias)) / 2.0;
-                push_cut(cuts, count, cap, fade_frame + (int64_t)rint(half));  // Python round(): half to even
-                last_scene_cut = t;
-            }
-            fade_in = true;
-            fade_frame = t;
-        }
-    }
-    // post_process (threshold_detector.py:170-191) with timecode = last frame
-    const int64_t last = first_frame + n - 1;
-    if (!fade_in && add_final_scene && (last - last_scene_cut) >= min_frames) push_cut(cuts, count, cap, fade_frame);
+    CutSink out{cuts, cap, 0};
+    threshold_cuts(avg, n, first_frame, threshold, method_ceiling, fade_bias, min_frames, add_final_scene, out);
+    *count = out.n;
 }
 
 }  // namespace psd

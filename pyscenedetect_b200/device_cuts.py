@@ -114,7 +114,7 @@ class DeviceCuts:
         _, hist = self._e.device_results()
         corr = self._tmp(n)
         check(self._lib.psd_scan_hist_correl(hist, n, int(bins), None, corr.ptr, self._stream))
-        check(self._lib.psd_cuts_histogram(corr.ptr, n, first_frame, max(0.0, min(1.0, 1.0 - threshold)),
+        check(self._lib.psd_cuts_histogram(corr.ptr, n, first_frame, histogram_threshold(threshold),
                                            min_len_frames(min_scene_len, fps), self._cuts.ptr, self._count.ptr,
                                            self._cap, self._stream), "psd_cuts_histogram")
         return self._fetch()
@@ -141,25 +141,42 @@ class DeviceCuts:
         return self._fetch()
 
 
-def cuts_for_detector(dc: DeviceCuts, detector, fps, first_frame: int = 0) -> list[int]:
-    """Run the device automaton that corresponds to a (fresh) detector object of this package with the
-    detector's own parameters: the cut list its per-frame `process_frame` + `post_process` would produce."""
+def histogram_threshold(threshold) -> float:
+    """The correlation bound psd_cuts_histogram compares with: 1 - threshold, clamped (histogram_detector.py:44)."""
+    return max(0.0, min(1.0, 1.0 - threshold))
+
+
+def automaton_args(detector) -> tuple[str, dict]:
+    """The device automaton that corresponds to a (fresh) detector object of this package, as the name of the
+    `DeviceCuts` method that runs it and that method's keyword arguments, taken from the detector's own
+    parameters (`fps` and `first_frame` excepted).  `cuts_for_detector` and `sweep.ParameterSweep` both map
+    detectors to automata through this one function."""
     from .compat import FlashFilter
     from .detectors import AdaptiveDetector, ContentDetector, HashDetector, HistogramDetector, ThresholdDetector
     if isinstance(detector, HashDetector):
-        return dc.hash(detector._threshold, detector._min_scene_len, fps, first_frame)
+        return "hash", dict(threshold=detector._threshold, min_scene_len=detector._min_scene_len)
     if isinstance(detector, AdaptiveDetector):
-        return dc.adaptive(tuple(detector._weights), detector.adaptive_threshold, detector.min_scene_len,
-                           detector.window_width, detector.min_content_val, fps, first_frame)
+        return "adaptive", dict(weights=tuple(detector._weights), adaptive_threshold=detector.adaptive_threshold,
+                                min_scene_len=detector.min_scene_len, window_width=detector.window_width,
+                                min_content_val=detector.min_content_val)
     if isinstance(detector, ContentDetector):
         ff = detector._flash_filter
         length = ff._filter_secs if ff._filter_secs is not None else ff._filter_length
-        return dc.content(tuple(detector._weights), detector._threshold, length, fps,
-                          suppress=ff._mode == FlashFilter.Mode.SUPPRESS, first_frame=first_frame)
+        return "content", dict(weights=tuple(detector._weights), threshold=detector._threshold, min_scene_len=length,
+                               suppress=ff._mode == FlashFilter.Mode.SUPPRESS)
     if isinstance(detector, HistogramDetector):
         # the constructor stored 1 - threshold (clamped); DeviceCuts.histogram applies the same map
-        return dc.histogram(1.0 - detector._threshold, detector._bins, detector._min_scene_len, fps, first_frame)
+        return "histogram", dict(threshold=1.0 - detector._threshold, bins=detector._bins,
+                                 min_scene_len=detector._min_scene_len)
     if isinstance(detector, ThresholdDetector):
-        return dc.threshold(detector.threshold, detector.min_scene_len, detector.fade_bias, detector.add_final_scene,
-                            detector.method == ThresholdDetector.Method.CEILING, fps, first_frame)
+        return "threshold", dict(threshold=detector.threshold, min_scene_len=detector.min_scene_len,
+                                 fade_bias=detector.fade_bias, add_final_scene=detector.add_final_scene,
+                                 ceiling=detector.method == ThresholdDetector.Method.CEILING)
     raise TypeError(f"no device automaton for {type(detector).__name__}")
+
+
+def cuts_for_detector(dc: DeviceCuts, detector, fps, first_frame: int = 0) -> list[int]:
+    """Run the device automaton that corresponds to a (fresh) detector object of this package with the
+    detector's own parameters: the cut list its per-frame `process_frame` + `post_process` would produce."""
+    method, kwargs = automaton_args(detector)
+    return getattr(dc, method)(**kwargs, fps=fps, first_frame=first_frame)

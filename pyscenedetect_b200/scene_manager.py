@@ -55,6 +55,84 @@ def get_scenes_from_cuts(cut_list, start_pos, end_pos):
     return scene_list
 
 
+class FrameBatches:
+    """The frame-gathering half of the detection loop (scene_manager.py:650-689): reads `video` in batches of
+    up to `batch_size` frames, cropped to `box` = (x0, y0, x1, y1) of size `size` = (w, h).  A stream with
+    `read_batch` and no crop / frame skip is read zero-copy; otherwise frames are copied into one of two
+    page-locked buffers, so that a batch can be gathered while the GPU scores the previous one.
+
+    `next()` returns (timecodes, frames, pinned) or None at the end.  The frames of a batch stay valid until
+    the batch after the next one is gathered: the caller must have synchronised the engines that read a batch
+    before asking for the batch two after it.  `close()` frees the buffers, after the last batch is done."""
+
+    def __init__(self, video, box, size, batch_size: int, cropped: bool = False, frame_skip: int = 0,
+                 end_frame: int | None = None):
+        self._video = video
+        self._box, self._size = box, size
+        self._batch_size = int(batch_size)
+        self._frame_skip = frame_skip
+        self._end_frame = end_frame
+        self._zero_copy = hasattr(video, "read_batch") and not cropped and frame_skip == 0
+        self._pinned = [None, None]
+        self._which = 0
+        self._done = False
+        self._processed = 0
+
+    def next(self):
+        if self._done:
+            return None
+        video, end_frame, zero_copy = self._video, self._end_frame, self._zero_copy
+        x0, y0, x1, y1 = self._box
+        w, h = self._size
+        fps = video.frame_rate
+        tcs, batch = [], None
+        want = self._batch_size
+        if end_frame is not None and zero_copy:
+            # the frame at position p is processed, then the loop stops unless p + 1 < end; the first
+            # frame is always processed (the check follows the put, scene_manager.py:680-689)
+            want = min(want, max(end_frame - video.frame_number, 1 if self._processed == 0 else 0))
+        if want > 0:
+            if zero_copy:
+                pos0 = video.frame_number
+                view = video.read_batch(want)
+                if view is not None:
+                    batch = view
+                    tcs = [FrameTimecode(pos0 + i, fps) for i in range(view.shape[0])]
+            else:
+                which = self._which
+                if self._pinned[which] is None:
+                    self._pinned[which] = PinnedBuffer(self._batch_size * w * h * 3)
+                buf = self._pinned[which].array.reshape(self._batch_size, h, w, 3)
+                k = 0
+                while k < want:
+                    frame = video.read()
+                    if frame is False:
+                        self._done = True
+                        break
+                    np.copyto(buf[k], frame[y0:y1, x0:x1])
+                    tcs.append(video.position)
+                    k += 1
+                    for _ in range(self._frame_skip):  # scene_manager.py:682-685
+                        if not video.read(decode=False):
+                            break
+                    if end_frame is not None and not (video.position.frame_num + 1) < end_frame:
+                        self._done = True
+                        break
+                batch = buf[:k] if k else None
+        if batch is None:
+            self._done = True
+            return None
+        self._processed += len(tcs)
+        self._which ^= 1
+        return tcs, batch, (not zero_copy) or bool(getattr(video, "is_pinned", False))
+
+    def close(self) -> None:
+        for p in self._pinned:
+            if p is not None:
+                p.close()
+        self._pinned = [None, None]
+
+
 class SceneManager:
     def __init__(self, stats_manager: StatsManager | None = None, device: int = 0,
                  batch_size: int = 64):
@@ -223,62 +301,21 @@ class SceneManager:
             end_frame = (self._base_timecode + end_time).frame_num
         elif duration is not None:
             end_frame = ((self._base_timecode + duration) + start_frame_num).frame_num
-        zero_copy = hasattr(video, "read_batch") and self._crop is None and frame_skip == 0
-        pinned = [None, None]
+        gather = FrameBatches(video, (x0, y0, x1, y1), (w, h), self._batch_size, cropped=self._crop is not None,
+                              frame_skip=frame_skip, end_frame=end_frame)
         pending = None  # (timecodes, frames_view, first engine index)
-        which = 0
-        done = False
-        processed = 0
         while True:
             # 1. gather the next batch while the GPU works on the previous one
-            tcs, batch = [], None
-            if not done:
-                want = self._batch_size
-                if end_frame is not None and zero_copy:
-                    # the frame at position p is processed, then the loop stops unless p + 1 < end; the first
-                    # frame is always processed (the check follows the put, scene_manager.py:680-689)
-                    want = min(want, max(end_frame - video.frame_number, 1 if processed == 0 else 0))
-                if want > 0:
-                    if zero_copy:
-                        pos0 = video.frame_number
-                        view = video.read_batch(want)
-                        if view is not None:
-                            batch = view
-                            tcs = [FrameTimecode(pos0 + i, fps) for i in range(view.shape[0])]
-                    else:
-                        if pinned[which] is None:
-                            pinned[which] = PinnedBuffer(self._batch_size * w * h * 3)
-                        buf = pinned[which].array.reshape(self._batch_size, h, w, 3)
-                        k = 0
-                        while k < want:
-                            frame = video.read()
-                            if frame is False:
-                                done = True
-                                break
-                            np.copyto(buf[k], frame[y0:y1, x0:x1])
-                            tcs.append(video.position)
-                            k += 1
-                            for _ in range(frame_skip):  # scene_manager.py:682-685
-                                if not video.read(decode=False):
-                                    break
-                            if end_frame is not None and not (video.position.frame_num + 1) < end_frame:
-                                done = True
-                                break
-                        batch = buf[:k] if k else None
-                if batch is None:
-                    done = True
+            tcs, batch, use_pinned = gather.next() or ([], None, False)
             # 2. launch the fused pass on the new batch (its H2D overlaps step 3's host work)
             nxt = None
             if batch is not None:
-                use_pinned = (not zero_copy) or bool(getattr(video, "is_pinned", False))
                 first = self._engine.frame_count
                 self._engine.submit(batch, pinned=use_pinned)
                 if self._start_pos is None:
                     self._start_pos = tcs[0]
                 self._last_pos = tcs[-1]
-                processed += len(tcs)
                 nxt = (tcs, batch, first)
-                which ^= 1
             # 3. retire the previous batch (device scans + per-frame state machines)
             if pending is not None:
                 self._consume(*pending, callback)
@@ -291,9 +328,7 @@ class SceneManager:
             self._last_pos = video.position
             for d in self._detector_list:
                 self._cutting_list += d.post_process(self._last_pos)
-        for p in pinned:
-            if p is not None:
-                p.close()
+        gather.close()
         return video.frame_number - start_frame_num
 
     def _consume(self, timecodes, frames, first, callback) -> None:
