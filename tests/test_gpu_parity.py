@@ -153,22 +153,29 @@ def test_device_generator_matches_numpy(lib):
         buf.close()
 
 
-@pytest.mark.parametrize("shape", [(160, 90), (131, 97), (17, 5), (1, 1), (4096, 3), (640, 360)])
+@pytest.mark.parametrize("shape", [(160, 90), (131, 97), (17, 5), (1, 1), (4096, 3), (640, 360), (64, 36)])
 def test_integer_sums_any_shape(lib, shape):
     """Raw integer outputs vs the oracle for aligned, unaligned, tiny and partial-strip sizes; the same frames
-    submitted from device memory at a base pointer that is not 16-byte aligned give the same bytes."""
+    submitted from device memory at a base pointer that is not 16-byte aligned give the same bytes.  64x36 submits
+    9 000 frames in calls of 1 000 (batches of 256), so the engine's result slots grow from 4 096 to 8 192 with
+    4 000 frames' results in place and to 16 384 with 8 000; the frames right after each growth read the
+    previous frame carried across it."""
     from pyscenedetect_b200.engine import F_BGRSUM, F_HSV, F_YHIST, DeviceBuffer, Engine
     w, h = shape
+    n, batch, chunk = (9000, 256, 1000) if shape == (64, 36) else (9, 4, 9)
     rng = np.random.default_rng(w * 1000 + h)
-    frames = rng.integers(0, 256, size=(9, h, w, 3), dtype=np.uint8)
-    eng = Engine(w, h, F_HSV | F_BGRSUM | F_YHIST, max_batch=4)
-    eng.submit(frames)
+    frames = rng.integers(0, 256, size=(n, h, w, 3), dtype=np.uint8)
+    eng = Engine(w, h, F_HSV | F_BGRSUM | F_YHIST, max_batch=batch)
+    for i in range(0, n, chunk):
+        eng.submit(frames[i:i + chunk])
     sums = eng.read_sums()
     hist = eng.read_yhist()
     buf = DeviceBuffer(frames.nbytes + 16)
     buf.upload(frames, offset=1)
-    dev = Engine(w, h, F_HSV | F_BGRSUM | F_YHIST, max_batch=4)
-    dev.submit_device(buf.ptr + 1, frames.shape[0])
+    dev = Engine(w, h, F_HSV | F_BGRSUM | F_YHIST, max_batch=batch)
+    for i in range(0, n, chunk):
+        dev.submit_device(buf.ptr + 1 + i * frames[0].nbytes, min(chunk, n - i))
+    assert dev.frame_count == n
     assert dev.read_sums().tobytes() == sums.tobytes()
     assert np.array_equal(dev.read_yhist(), hist)
     dev.close()
