@@ -39,7 +39,11 @@ extern "C" {
 #define PSD_F_YHIST 4u  /* 256-bin histogram of YUV-Y: histogram_detector.py:156-159 */
 #define PSD_F_EDGES 8u  /* Canny+dilate edge-map SAD: content_detector.py:213-239 (implies HSV) */
 #define PSD_F_HASH 16u  /* perceptual hash of every frame: hash_detector.py:124-158 */
-#define PSD_HASH_WORDS 4 /* a hash occupies 4 x uint64 (size * size <= 256 bits), bit u*size+v = D[u][v] > median */
+#define PSD_HASH_WORDS 4 /* the hash stride for size <= 16: 4 x uint64 (size * size <= 256 bits) */
+/* Per-frame stride (uint64 words) of every hash array of an engine or scan with HashDetector(size=...):
+ * max(4, ceil(size * size / 64)), so 4 for size <= 16.  Bit u*size+v (word (u*size+v)/64, bit (u*size+v)%64) is
+ * D[u][v] > median; the bits past size * size are 0. */
+#define PSD_HASH_WORDS_FOR(size) ((size) * (size) <= 256 ? PSD_HASH_WORDS : ((size) * (size) + 63) / 64)
 
 /* submit flags */
 #define PSD_SUBMIT_PINNED 1u /* host buffer is page-locked (psd_host_alloc): DMA straight from it,
@@ -59,8 +63,9 @@ typedef struct psd_config {
     int32_t edge_kernel_size; /* dilate kernel k (odd >= 3); 0 = content_detector.py:39-46 estimate */
     int32_t max_batch;        /* max frames per submit call (staging is sized for it) */
     uint32_t flags;           /* reserved: no flags are defined, must be 0 */
-    int32_t hash_size;        /* PSD_F_HASH: HashDetector(size=...), 0 = 8 */
-    int32_t hash_lowpass;     /* PSD_F_HASH: HashDetector(lowpass=...), 0 = 2 */
+    int32_t hash_size;        /* PSD_F_HASH: HashDetector(size=...) >= 1, 0 = 8 */
+    int32_t hash_lowpass;     /* PSD_F_HASH: HashDetector(lowpass=...) >= 1, 0 = 2; the scored frame must be at
+                                 least (size*lowpass) x (size*lowpass) */
     int32_t reserved[4];
 } psd_config;
 
@@ -123,11 +128,13 @@ int64_t psd_engine_frame_count(const psd_engine* e);
 /* copy results for frames [first, first+n) to host (implies sync) */
 int psd_engine_read_sums(psd_engine* e, int64_t first, int64_t n, psd_frame_sums* out);
 int psd_engine_read_yhist(psd_engine* e, int64_t first, int64_t n, uint32_t* out /*[n][256]*/);
-int psd_engine_read_hash(psd_engine* e, int64_t first, int64_t n, uint64_t* out /*[n][PSD_HASH_WORDS]*/);
+int psd_engine_read_hash(psd_engine* e, int64_t first, int64_t n,
+                         uint64_t* out /*[n][PSD_HASH_WORDS_FOR(hash_size)]*/);
 /* device pointers of the engine-owned result arrays (valid until destroy/reset) */
 int psd_engine_device_results(psd_engine* e, const psd_frame_sums** sums, const uint32_t** yhist);
-int psd_engine_device_hash(psd_engine* e, const uint64_t** hashes /* stream frame i at hashes + i*PSD_HASH_WORDS;
-                                                                      the halo frame's hash sits one entry before */);
+int psd_engine_device_hash(psd_engine* e, const uint64_t** hashes /* stream frame i at hashes + i*PSD_HASH_WORDS_FOR(
+                                                                      hash_size); the halo frame's hash sits one
+                                                                      stride before */);
 /* CUDA-event time (ms) spent in the engine's kernels between the first launch after the last
  * psd_engine_timing_reset() and the last launch (on the engine's compute stream). */
 int psd_engine_timing_reset(psd_engine* e);
@@ -159,7 +166,7 @@ int psd_scan_average(const psd_frame_sums* sums, int64_t n, int64_t n_values, do
 int psd_scan_hist_correl(const uint32_t* yhist, int64_t n, int32_t bins, const uint32_t* prev_hist,
                          double* out_correl, void* stream);
 /* hash_detector.py:95-99: hash_dist = popcount(hash_t xor hash_{t-1}) / (size*size); out[0] uses prev_hash if
- * non-NULL else is NaN */
+ * non-NULL else is NaN.  hashes and prev_hash have the stride PSD_HASH_WORDS_FOR(hash_size) */
 int psd_scan_hash_dist(const uint64_t* hashes, int64_t n, int32_t hash_size, const uint64_t* prev_hash,
                        double* out_dist, void* stream);
 /* >= / <= compare producing u8 flags (content_detector.py:210, histogram_detector.py:108) */

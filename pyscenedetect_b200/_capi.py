@@ -30,6 +30,11 @@ HASH_WORDS = 4
 SUBMIT_PINNED = 1
 
 
+def hash_words(size: int) -> int:
+    """PSD_HASH_WORDS_FOR(size): uint64 words per frame of every hash array, max(4, ceil(size * size / 64))."""
+    return max(HASH_WORDS, (int(size) * int(size) + 63) // 64)
+
+
 class PsdConfig(C.Structure):
     _fields_ = [
         ("struct_size", C.c_int32),

@@ -71,7 +71,7 @@ struct psd_engine {
     // results: slot 0 = halo frame, stream frame i at slot i+1
     psd_frame_sums* d_sums = nullptr;
     uint32_t* d_yhist = nullptr;
-    uint64_t* d_hash = nullptr;   // [capacity][PSD_HASH_WORDS]
+    uint64_t* d_hash = nullptr;   // [capacity][hash.words]
     HashPlan hash{};
     int64_t capacity = 0;
     int64_t n_frames = 0;
@@ -116,10 +116,10 @@ static int ensure_capacity(psd_engine* e, int64_t need_slots) {
     }
     if (e->features & PSD_F_HASH) {
         uint64_t* nh = nullptr;
-        PSD_CUDA(cudaMalloc(&nh, (size_t)cap * PSD_HASH_WORDS * sizeof(uint64_t)));
-        PSD_CUDA(cudaMemsetAsync(nh, 0, (size_t)cap * PSD_HASH_WORDS * sizeof(uint64_t), e->compute_stream));
+        PSD_CUDA(cudaMalloc(&nh, (size_t)cap * e->hash.words * sizeof(uint64_t)));
+        PSD_CUDA(cudaMemsetAsync(nh, 0, (size_t)cap * e->hash.words * sizeof(uint64_t), e->compute_stream));
         if (e->d_hash) {
-            PSD_CUDA(cudaMemcpyAsync(nh, e->d_hash, (size_t)(e->n_frames + 1) * PSD_HASH_WORDS * sizeof(uint64_t),
+            PSD_CUDA(cudaMemcpyAsync(nh, e->d_hash, (size_t)(e->n_frames + 1) * e->hash.words * sizeof(uint64_t),
                                      cudaMemcpyDeviceToDevice, e->compute_stream));
             PSD_CUDA(cudaStreamSynchronize(e->compute_stream));
             cudaFree(e->d_hash);
@@ -185,7 +185,7 @@ static int run_batch(psd_engine* e, const uint8_t* src, int64_t src_frame_stride
         if (rc) return rc;
     }
     if (e->features & PSD_F_HASH) {
-        rc = launch_hash(e->hash, scored, scored_stride, (int)n, e->W, e->H, e->d_hash + slot0 * PSD_HASH_WORDS, st);
+        rc = launch_hash(e->hash, scored, scored_stride, (int)n, e->W, e->H, e->d_hash + slot0 * e->hash.words, st);
         if (rc) return rc;
     }
     PSD_CUDA(cudaEventRecord(k1, st));
@@ -583,13 +583,13 @@ int psd_engine_read_hash(psd_engine* e, int64_t first, int64_t n, uint64_t* out)
     PSD_REQUIRE(first >= -1 && n >= 0 && first + n <= e->n_frames, "frame range out of bounds");
     int rc = psd_engine_sync(e);
     if (rc) return rc;
-    if (n) PSD_CUDA(cudaMemcpy(out, e->d_hash + (first + 1) * PSD_HASH_WORDS, (size_t)n * PSD_HASH_WORDS * 8, cudaMemcpyDeviceToHost));
+    if (n) PSD_CUDA(cudaMemcpy(out, e->d_hash + (first + 1) * e->hash.words, (size_t)n * e->hash.words * 8, cudaMemcpyDeviceToHost));
     return PSD_OK;
 }
 
 int psd_engine_device_hash(psd_engine* e, const uint64_t** hashes) {
     PSD_REQUIRE(e && hashes, "psd_engine_device_hash: null argument");
-    *hashes = e->d_hash ? e->d_hash + PSD_HASH_WORDS : nullptr;
+    *hashes = e->d_hash ? e->d_hash + e->hash.words : nullptr;
     return PSD_OK;
 }
 
@@ -718,7 +718,7 @@ int psd_engine_scan_hist_correl_host(psd_engine* e, int64_t first, int64_t n, in
 
 int psd_scan_hash_dist(const uint64_t* hashes, int64_t n, int32_t hash_size, const uint64_t* prev_hash, double* out,
                        void* stream) {
-    PSD_REQUIRE(hashes && out && n >= 0 && hash_size >= 1 && hash_size <= 16, "psd_scan_hash_dist: bad arguments");
+    PSD_REQUIRE(hashes && out && n >= 0 && hash_size >= 1 && hash_size <= 32768, "psd_scan_hash_dist: bad arguments");
     return launch_hash_dist(hashes, n, hash_size, prev_hash, out, (cudaStream_t)stream);
 }
 
@@ -731,8 +731,8 @@ int psd_engine_scan_hash_dist_host(psd_engine* e, int64_t first, int64_t n, doub
     double* tmp = nullptr;
     PSD_CUDA(cudaMalloc(&tmp, (size_t)n * sizeof(double)));
     // slot `first` (= stream frame first-1, or the halo slot) precedes slot first+1
-    const uint64_t* prev = (first > 0 || e->halo_scored) ? e->d_hash + first * PSD_HASH_WORDS : nullptr;
-    int rc = psd_scan_hash_dist(e->d_hash + (first + 1) * PSD_HASH_WORDS, n, e->hash.size, prev, tmp, e->compute_stream);
+    const uint64_t* prev = (first > 0 || e->halo_scored) ? e->d_hash + first * e->hash.words : nullptr;
+    int rc = psd_scan_hash_dist(e->d_hash + (first + 1) * e->hash.words, n, e->hash.size, prev, tmp, e->compute_stream);
     if (!rc) rc = scan_to_host(e, tmp, out, (size_t)n);
     cudaFree(tmp);
     return rc;

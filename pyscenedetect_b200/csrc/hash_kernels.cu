@@ -30,13 +30,14 @@ __device__ __forceinline__ uint32_t gray_word(uint32_t px) {
 // byte -> float32 without the conversion unit: 0x4B000000 | g is 2^23 + g
 __device__ __forceinline__ float byte_to_float(uint32_t g) { return __fadd_rn(__uint_as_float(0x4B000000u | g), -8388608.0f); }
 
-// The horizontal pass.  A CTA takes a block of consecutive source rows of one frame (256 / n of them):
+// The horizontal pass.  A CTA takes a block of consecutive source rows of one frame (max(1, 256 / n) of them):
 //   1. all threads pull the block - it is contiguous in memory - 16 pixels (three 16-byte loads) at a time,
 //      convert to gray and park the gray bytes in shared memory (row pitch W rounded up + 4: two rows of a
 //      1920-wide frame would otherwise sit in the same banks);
 //   2. thread (row, destination column) walks its taps in shared memory: the integer block sum if both scale
 //      factors are integers, else OpenCV's float32 `buf += S * alpha` in source order (separate multiply and
-//      add: the order and the roundings decide the last bit, so this chain stays sequential).
+//      add: the order and the roundings decide the last bit, so this chain stays sequential).  For n <= 256
+//      every thread has at most one (row, column); for n > 256 the CTA owns one row and loops over columns.
 // (The first version had one thread per (row, column) read its 3 x 120 bytes straight from global memory, 32
 // lanes 360 bytes apart: 0.085 of the HBM roofline.)
 __global__ void __launch_bounds__(256) psd_hash_rows_kernel(const uint8_t* __restrict__ frames, int64_t frame_stride,
@@ -79,30 +80,31 @@ __global__ void __launch_bounds__(256) psd_hash_rows_kernel(const uint8_t* __res
         }
     }
     __syncthreads();
-    // ---- 2. one thread per (row, destination column) ----
-    const int r = tid / n, dx = tid - r * n;
-    if (r >= rows) return;
-    const uint8_t* srow = sgray + r * pitch;
-    float* out = rowbuf + (f * H + sy0 + r) * (int64_t)n + dx;
-    if (fast) {  // integer scale: exact integer sum of the block's columns
-        const int sxw = W / n;
-        uint32_t s = 0;
-        for (int x = dx * sxw; x < (dx + 1) * sxw; ++x) s += srow[x];
-        *out = __uint_as_float(s);
-    } else {
-        // first (partial) tap, the run of whole pixels, last (partial) tap - in source order
-        float buf = 0.0f;
-        const int k0 = xstart[dx], k1 = xstart[dx + 1];
-        const int km = xmid[2 * dx], nm = xmid[2 * dx + 1];
-        for (int k = k0; k < km; ++k) buf = __fadd_rn(buf, __fmul_rn(byte_to_float(srow[xsi[k]]), xalpha[k]));
-        if (nm > 0) {
-            const uint8_t* sp = srow + xsi[km];
-            const float am = xalpha[km];
+    // ---- 2. (row, destination column) pairs ----
+    for (int c = tid; c < rows * n; c += 256) {
+        const int r = c / n, dx = c - r * n;
+        const uint8_t* srow = sgray + r * pitch;
+        float* out = rowbuf + (f * H + sy0 + r) * (int64_t)n + dx;
+        if (fast) {  // integer scale: exact integer sum of the block's columns
+            const int sxw = W / n;
+            uint32_t s = 0;
+            for (int x = dx * sxw; x < (dx + 1) * sxw; ++x) s += srow[x];
+            *out = __uint_as_float(s);
+        } else {
+            // first (partial) tap, the run of whole pixels, last (partial) tap - in source order
+            float buf = 0.0f;
+            const int k0 = xstart[dx], k1 = xstart[dx + 1];
+            const int km = xmid[2 * dx], nm = xmid[2 * dx + 1];
+            for (int k = k0; k < km; ++k) buf = __fadd_rn(buf, __fmul_rn(byte_to_float(srow[xsi[k]]), xalpha[k]));
+            if (nm > 0) {
+                const uint8_t* sp = srow + xsi[km];
+                const float am = xalpha[km];
 #pragma unroll 8
-            for (int i = 0; i < nm; ++i) buf = __fadd_rn(buf, __fmul_rn(byte_to_float(sp[i]), am));
+                for (int i = 0; i < nm; ++i) buf = __fadd_rn(buf, __fmul_rn(byte_to_float(sp[i]), am));
+            }
+            for (int k = km + nm; k < k1; ++k) buf = __fadd_rn(buf, __fmul_rn(byte_to_float(srow[xsi[k]]), xalpha[k]));
+            *out = buf;
         }
-        for (int k = km + nm; k < k1; ++k) buf = __fadd_rn(buf, __fmul_rn(byte_to_float(srow[xsi[k]]), xalpha[k]));
-        *out = buf;
     }
 }
 
@@ -138,31 +140,82 @@ __device__ __forceinline__ double fold_coef(const double* v0, int stride0, const
     return acc;
 }
 
-// one CTA per frame: vertical pass, normalisation, DCT low band, median, bits
-constexpr int kHashMaxN = 64, kHashMaxSize = 16;
-__global__ void __launch_bounds__(256) psd_hash_finish_kernel(const float* __restrict__ rowbuf, int H, int n, int size,
+// Order-preserving keys of float32: key(a) < key(b) exactly when a < b (-0.0 sorts just below +0.0, which
+// compare equal, so the selected value compares like numpy's).
+__device__ __forceinline__ uint32_t float_key(float a) {
+    const uint32_t b = __float_as_uint(a);
+    return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
+}
+__device__ __forceinline__ float key_float(uint32_t k) {
+    return __uint_as_float((k & 0x80000000u) ? (k & 0x7FFFFFFFu) : ~k);
+}
+
+// The k-th smallest (0-based) of v[0..m) by a CTA of 256 threads: a radix select over the keys, 8 bits a pass from
+// the top.  Each pass histograms the digit of the keys that share the prefix found so far; warp 0 scans the 256
+// counts (8 per lane) and picks the bin that holds rank k.  hist[256] and sel[2] are shared scratch.
+__device__ float cta_select(const float* v, int m, int k, uint32_t* hist, uint32_t* sel) {
+    const int tid = threadIdx.x;
+    uint32_t prefix = 0, mask = 0;
+    for (int shift = 24; shift >= 0; shift -= 8) {
+        hist[tid] = 0;
+        __syncthreads();
+        for (int c = tid; c < m; c += 256) {
+            const uint32_t key = float_key(v[c]);
+            if ((key & mask) == prefix) atomicAdd(&hist[(key >> shift) & 255u], 1u);
+        }
+        __syncthreads();
+        if (tid < 32) {
+            uint32_t s = 0;
+#pragma unroll
+            for (int b = 0; b < 8; ++b) s += hist[tid * 8 + b];
+            uint32_t incl = s;
+#pragma unroll
+            for (int d = 1; d < 32; d <<= 1) {
+                const uint32_t y = __shfl_up_sync(0xFFFFFFFFu, incl, d);
+                if (tid >= d) incl += y;
+            }
+            uint32_t below = incl - s;
+            if (below <= (uint32_t)k && (uint32_t)k < incl) {
+                int b = tid * 8;
+                while (below + hist[b] <= (uint32_t)k) below += hist[b++];
+                sel[0] = (uint32_t)b;
+                sel[1] = below;
+            }
+        }
+        __syncthreads();
+        prefix |= sel[0] << shift;
+        mask |= 255u << shift;
+        k -= (int)sel[1];
+        __syncthreads();
+    }
+    return key_float(prefix);
+}
+
+// One CTA per frame: vertical pass, normalisation, DCT low band, median, bits.  The working set (image, folded
+// levels, low band) sits in dynamic shared memory, or for large hash images (kGlobal) in the frame's slice of a
+// global workspace - the same code on the same values either way.
+template <bool kGlobal>
+__global__ void __launch_bounds__(256, 2) psd_hash_finish_kernel(const float* __restrict__ rowbuf, int H, int n, int size,
                                                               int fast, int area_w, int area_h,
                                                               const int32_t* __restrict__ ystart,
                                                               const int32_t* __restrict__ ysi,
                                                               const float* __restrict__ ybeta,
                                                               const double* __restrict__ costab /* [4n] cos(pi k / 2n) */,
-                                                              FoldPlan fp,
-                                                              uint64_t* __restrict__ hashes /* [frames][PSD_HASH_WORDS] */) {
+                                                              FoldPlan fp, double* __restrict__ ws, int64_t ws_doubles,
+                                                              int words,
+                                                              uint64_t* __restrict__ hashes /* [frames][words] */) {
     extern __shared__ __align__(16) double dsm[];
-    double* x = dsm;                    // [n][n] normalised image (row i, column j)
+    const int64_t f = blockIdx.x;
+    double* x = kGlobal ? ws + f * ws_doubles : dsm;   // [n][n] normalised image (row i, column j)
     double* lev = x + n * n;            // [n][n]: folded levels of every column j (element e of column j at lev[e*n + j])
     double* t = lev + n * n;            // [size][n]: vertical transform, t[u][j]
     double* lev2 = t + size * n;        // [n][size]: folded levels of every t[u][.] (element e of row u at lev2[e*size + u])
-    __shared__ float low[kHashMaxSize * kHashMaxSize];
+    float* low = reinterpret_cast<float*>(lev2 + (int64_t)n * size);   // [size][size] low band
     __shared__ uint32_t mx;
-    __shared__ float med;
-    __shared__ float mid[2];
-    __shared__ unsigned long long bits[PSD_HASH_WORDS];
+    __shared__ uint32_t hist[256], sel[2];
     const int tid = threadIdx.x;
-    const int64_t f = blockIdx.x;
     const float* rb = rowbuf + f * (int64_t)H * n;
     if (tid == 0) mx = 0;
-    if (tid < PSD_HASH_WORDS) bits[tid] = 0ull;
     __syncthreads();
     uint32_t my_max = 0;
     for (int c = tid; c < n * n; c += 256) {
@@ -226,35 +279,33 @@ __global__ void __launch_bounds__(256) psd_hash_finish_kernel(const float* __res
         low[c] = (float)__dmul_rn(__dmul_rn(acc, u ? s1 : s0), v ? s1 : s0);
     }
     __syncthreads();
-    // numpy.median: rank every element (ties broken by index), pick the middle one / the float32 mean of the two
-    for (int c = tid; c < m; c += 256) {
-        const float a = low[c];
-        int rank = 0;
-        for (int k = 0; k < m; ++k) rank += (low[k] < a) || (low[k] == a && k < c);
-        if (m & 1) { if (rank == m / 2) mid[0] = mid[1] = a; }
-        else { if (rank == m / 2 - 1) mid[0] = a; if (rank == m / 2) mid[1] = a; }
+    // numpy.median: the middle value, or the float32 mean of the two middle values
+    float med = cta_select(low, m, m / 2, hist, sel);
+    if ((m & 1) == 0) med = __fmul_rn(__fadd_rn(cta_select(low, m, m / 2 - 1, hist, sel), med), 0.5f);
+    // bit c = low[c] > med; word w holds bits 64 w .. 64 w + 63 (words past the low band stay 0)
+    const int warp = tid >> 5, lane = tid & 31;
+    for (int w = warp; w < words; w += 8) {
+        const int c0 = w * 64 + lane, c1 = c0 + 32;
+        const uint32_t lo = __ballot_sync(0xFFFFFFFFu, c0 < m && low[c0] > med);
+        const uint32_t hi = __ballot_sync(0xFFFFFFFFu, c1 < m && low[c1] > med);
+        if (lane == 0) hashes[f * words + w] = ((uint64_t)hi << 32) | lo;
     }
-    __syncthreads();
-    if (tid == 0) med = (m & 1) ? mid[0] : __fmul_rn(__fadd_rn(mid[0], mid[1]), 0.5f);
-    __syncthreads();
-    for (int c = tid; c < m; c += 256)
-        if (low[c] > med) atomicOr(&bits[c >> 6], 1ull << (c & 63));
-    __syncthreads();
-    if (tid < PSD_HASH_WORDS) hashes[f * PSD_HASH_WORDS + tid] = bits[tid];
 }
 
-// hash_detector.py:95-99: Hamming distance to the previous frame's hash, divided by size * size
-__global__ void psd_scan_hash_dist_kernel(const uint64_t* __restrict__ hashes, int64_t n, double size_sq,
+// hash_detector.py:95-99: Hamming distance to the previous frame's hash, divided by size * size.  One warp per
+// frame; hashes are `words` apart.
+__global__ void psd_scan_hash_dist_kernel(const uint64_t* __restrict__ hashes, int64_t n, int words, double size_sq,
                                           const uint64_t* __restrict__ prev_hash, double* __restrict__ out) {
-    const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+    const int64_t i = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5;
+    const int lane = threadIdx.x & 31;
     if (i >= n) return;
-    const uint64_t* cur = hashes + i * PSD_HASH_WORDS;
-    const uint64_t* prv = (i > 0) ? cur - PSD_HASH_WORDS : prev_hash;
-    if (prv == nullptr) { out[i] = __longlong_as_double(0x7FF8000000000000LL); return; }
+    const uint64_t* cur = hashes + i * words;
+    const uint64_t* prv = (i > 0) ? cur - words : prev_hash;
+    if (prv == nullptr) { if (lane == 0) out[i] = __longlong_as_double(0x7FF8000000000000LL); return; }
     int cnt = 0;
-#pragma unroll
-    for (int w = 0; w < PSD_HASH_WORDS; ++w) cnt += __popcll(cur[w] ^ prv[w]);
-    out[i] = __ddiv_rn((double)cnt, size_sq);
+    for (int w = lane; w < words; w += 32) cnt += __popcll(cur[w] ^ prv[w]);
+    cnt = __reduce_add_sync(0xFFFFFFFFu, cnt);
+    if (lane == 0) out[i] = __ddiv_rn((double)cnt, size_sq);
 }
 
 // ---- host side: OpenCV's computeResizeAreaTab, the cosine table ----
@@ -283,12 +334,17 @@ static int upload(const std::vector<T>& v, T** out) {
     return PSD_OK;
 }
 
+constexpr int kHashStaticSmem = 2048;                       // the finish kernel's static shared memory, rounded up
+constexpr int64_t kHashWorkspaceBytes = (int64_t)512 << 20;  // row buffer + finish workspace of one sub-batch
+
 int hash_plan_create(HashPlan* p, int W, int H, int size, int lowpass, int max_batch) {
-    PSD_REQUIRE(size >= 1 && size <= kHashMaxSize && lowpass >= 1 && size * lowpass <= kHashMaxN,
-                "HashDetector on the GPU needs size <= %d and size * lowpass <= %d", kHashMaxSize, kHashMaxN);
-    const int n = size * lowpass;
-    PSD_REQUIRE(W >= n && H >= n, "frames smaller than the %dx%d hash image are not supported", n, n);
+    PSD_REQUIRE(size >= 1 && lowpass >= 1, "HashDetector needs size >= 1 and lowpass >= 1");
+    const int64_t n64 = (int64_t)size * lowpass;
+    PSD_REQUIRE(W >= n64 && H >= n64, "frames smaller than the %lldx%lld hash image are not supported",
+                (long long)n64, (long long)n64);
+    const int n = (int)n64;
     p->n = n; p->size = size;
+    p->words = PSD_HASH_WORDS_FOR(size);
     p->fast = (W % n == 0 && H % n == 0) ? 1 : 0;
     p->area_w = W / n; p->area_h = H / n;
     std::vector<int32_t> st, si; std::vector<float> al;
@@ -326,44 +382,71 @@ int hash_plan_create(HashPlan* p, int W, int H, int size, int lowpass, int max_b
         off += p->len[p->levels];
         p->levels += 1;
     }
-    PSD_CUDA(cudaMalloc(&p->rowbuf, (size_t)max_batch * H * n * sizeof(float)));
+    // the finish kernel's working set per frame: image and column levels (2 n^2), t and its levels (2 size n),
+    // the low band (size^2 floats); in shared memory while it fits, else in a global workspace
+    const int64_t m = (int64_t)size * size;
+    p->ws_doubles = ((2 * n64 * n64 + 2 * (int64_t)size * n64 + (m + 1) / 2) + 1) & ~(int64_t)1;
+    int dev = 0, smem_optin = 0;
+    PSD_CUDA(cudaGetDevice(&dev));
+    PSD_CUDA(cudaDeviceGetAttribute(&smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+    p->global_ws = (size_t)p->ws_doubles * sizeof(double) > (size_t)smem_optin - kHashStaticSmem;
+    // frames per sub-batch: the row buffer and the workspace together stay within kHashWorkspaceBytes
+    // (or one frame's worth, if that is larger)
+    const int64_t per_frame = (int64_t)H * n * (int64_t)sizeof(float) +
+                              (p->global_ws ? p->ws_doubles * (int64_t)sizeof(double) : 0);
+    p->batch = (int)std::max<int64_t>(1, std::min<int64_t>(max_batch, kHashWorkspaceBytes / per_frame));
+    PSD_CUDA(cudaMalloc(&p->rowbuf, (size_t)p->batch * H * n * sizeof(float)));
+    if (p->global_ws) PSD_CUDA(cudaMalloc(&p->ws, (size_t)p->batch * p->ws_doubles * sizeof(double)));
     return PSD_OK;
 }
 
 void hash_plan_destroy(HashPlan* p) {
     cudaFree(p->xstart); cudaFree(p->xsi); cudaFree(p->xmid); cudaFree(p->xalpha); cudaFree(p->ystart); cudaFree(p->ysi);
-    cudaFree(p->ybeta); cudaFree(p->cosn); cudaFree(p->rowbuf);
+    cudaFree(p->ybeta); cudaFree(p->cosn); cudaFree(p->rowbuf); cudaFree(p->ws);
     *p = HashPlan{};
 }
 
 int launch_hash(const HashPlan& p, const uint8_t* frames, int64_t frame_stride, int n_frames, int W, int H,
                 uint64_t* hashes, cudaStream_t stream) {
-    // rows kernel: 256 / n source rows per CTA, their gray bytes in shared memory
-    const int rows_per_cta = 256 / p.n;
+    // rows kernel: max(1, 256 / n) source rows per CTA, their gray bytes in shared memory
+    const int rows_per_cta = std::max(1, 256 / p.n);
     const int pitch = ((W + 3) & ~3) + 4;
     const size_t smem_rows = (size_t)rows_per_cta * pitch;
     PSD_REQUIRE(smem_rows <= 200 * 1024, "frame too wide for the hash rows kernel (%d columns)", W);
     PSD_CUDA(cudaFuncSetAttribute(psd_hash_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_rows));
-    dim3 rgrid((unsigned)((H + rows_per_cta - 1) / rows_per_cta), (unsigned)n_frames);
-    psd_hash_rows_kernel<<<rgrid, 256, smem_rows, stream>>>(frames, frame_stride, W, H, p.n, rows_per_cta, pitch, p.fast,
-                                                            p.xstart, p.xsi, p.xalpha, p.xmid, p.rowbuf);
-    PSD_CHECK_LAUNCH();
     FoldPlan fp{};
     fp.levels = p.levels;
     for (int k = 0; k < 8; ++k) { fp.len[k] = p.len[k]; fp.off[k] = p.off[k]; }
-    const size_t smem = ((size_t)2 * p.n * p.n + (size_t)p.size * p.n + (size_t)p.n * p.size) * sizeof(double);
-    PSD_CUDA(cudaFuncSetAttribute(psd_hash_finish_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    psd_hash_finish_kernel<<<(unsigned)n_frames, 256, smem, stream>>>(p.rowbuf, H, p.n, p.size, p.fast, p.area_w, p.area_h,
-                                                                     p.ystart, p.ysi, p.ybeta, p.cosn, fp, hashes);
-    PSD_CHECK_LAUNCH();
-    count_launch(2);
+    const size_t smem = p.global_ws ? 0 : (size_t)p.ws_doubles * sizeof(double);
+    if (!p.global_ws)
+        PSD_CUDA(cudaFuncSetAttribute(psd_hash_finish_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    for (int f0 = 0; f0 < n_frames; f0 += p.batch) {   // sub-batches share the row buffer and the workspace
+        const int nb = std::min(p.batch, n_frames - f0);
+        dim3 rgrid((unsigned)((H + rows_per_cta - 1) / rows_per_cta), (unsigned)nb);
+        psd_hash_rows_kernel<<<rgrid, 256, smem_rows, stream>>>(frames + f0 * frame_stride, frame_stride, W, H, p.n,
+                                                                rows_per_cta, pitch, p.fast, p.xstart, p.xsi, p.xalpha,
+                                                                p.xmid, p.rowbuf);
+        PSD_CHECK_LAUNCH();
+        uint64_t* out = hashes + (int64_t)f0 * p.words;
+        if (p.global_ws)
+            psd_hash_finish_kernel<true><<<(unsigned)nb, 256, 0, stream>>>(
+                p.rowbuf, H, p.n, p.size, p.fast, p.area_w, p.area_h, p.ystart, p.ysi, p.ybeta, p.cosn, fp, p.ws,
+                p.ws_doubles, p.words, out);
+        else
+            psd_hash_finish_kernel<false><<<(unsigned)nb, 256, smem, stream>>>(
+                p.rowbuf, H, p.n, p.size, p.fast, p.area_w, p.area_h, p.ystart, p.ysi, p.ybeta, p.cosn, fp, nullptr, 0,
+                p.words, out);
+        PSD_CHECK_LAUNCH();
+        count_launch(2);
+    }
     return PSD_OK;
 }
 
 int launch_hash_dist(const uint64_t* hashes, int64_t n, int size, const uint64_t* prev_hash, double* out,
                      cudaStream_t stream) {
     if (n <= 0) return PSD_OK;
-    psd_scan_hash_dist_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(hashes, n, (double)(size * size), prev_hash, out);
+    psd_scan_hash_dist_kernel<<<(unsigned)((n + 7) / 8), 256, 0, stream>>>(hashes, n, PSD_HASH_WORDS_FOR(size),
+                                                                          (double)size * size, prev_hash, out);
     PSD_CHECK_LAUNCH();
     count_launch();
     return PSD_OK;

@@ -103,7 +103,12 @@ struct HashPlan {        // per-engine tables for one (frame size, hash size, lo
     float *xalpha = nullptr, *ybeta = nullptr;
     double* cosn = nullptr;   // [4n] cos(pi k / 2n)
     int levels = 1, len[8] = {0}, off[8] = {0};  // folded levels of a length-n vector (hash_kernels.cu:FoldPlan)
-    float* rowbuf = nullptr;  // [max_batch][H][n] horizontal pass
+    int words = PSD_HASH_WORDS;  // per-frame stride of the hash arrays: PSD_HASH_WORDS_FOR(size)
+    int batch = 0;               // frames per sub-batch of the hash pass
+    bool global_ws = false;      // the finish kernel's working set lives in `ws`, not in shared memory
+    int64_t ws_doubles = 0;      // finish working set per frame (doubles)
+    float* rowbuf = nullptr;  // [batch][H][n] horizontal pass
+    double* ws = nullptr;     // [batch][ws_doubles] finish workspace (global_ws only)
 };
 int hash_plan_create(HashPlan* p, int W, int H, int size, int lowpass, int max_batch);
 void hash_plan_destroy(HashPlan* p);

@@ -19,8 +19,8 @@ class HashDetector(EngineDetector):
 
     def __init__(self, threshold: float = 0.35, size: int = 8, lowpass: int = 2, min_scene_len=15):
         super().__init__()
-        if not (1 <= int(size) <= 16 and int(lowpass) >= 1 and int(size) * int(lowpass) <= 64):
-            raise ValueError("the GPU HashDetector supports size <= 16 and size * lowpass <= 64")
+        if not (int(size) >= 1 and int(lowpass) >= 1):
+            raise ValueError("HashDetector needs size >= 1 and lowpass >= 1")
         self._threshold = threshold
         self._min_scene_len = min_scene_len
         self._size = size

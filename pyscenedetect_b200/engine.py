@@ -8,7 +8,7 @@ import ctypes as C
 import numpy as np
 
 from . import _capi
-from ._capi import F_BGRSUM, F_EDGES, F_HASH, F_HSV, F_YHIST, HASH_WORDS, SUMS_DTYPE, check
+from ._capi import F_BGRSUM, F_EDGES, F_HASH, F_HSV, F_YHIST, SUMS_DTYPE, check, hash_words
 
 
 class PinnedBuffer:
@@ -182,9 +182,10 @@ class Engine:
         return out
 
     def read_hash(self, first: int = 0, n: int | None = None) -> np.ndarray:
-        """-> (n, 4) uint64: bit u*size+v of the 256-bit word = DCT[u][v] > median (hash_detector.py:156)."""
+        """-> (n, hash_words(size)) uint64: bit u*size+v of the row (word k // 64, bit k % 64) = DCT[u][v] > median
+        (hash_detector.py:156); 4 words for size <= 16."""
         n = self.frame_count - first if n is None else n
-        out = np.zeros((n, HASH_WORDS), dtype=np.uint64)
+        out = np.zeros((n, hash_words(self.hash_size)), dtype=np.uint64)
         check(self._lib.psd_engine_read_hash(self._h, first, n, out.ctypes.data), "psd_engine_read_hash")
         return out
 

@@ -15,7 +15,7 @@ from __future__ import annotations
 
 import numpy as np
 
-from ._capi import F_HASH, F_YHIST, HASH_WORDS, SUMS_DTYPE
+from ._capi import F_HASH, F_YHIST, SUMS_DTYPE, hash_words
 
 
 def shard_bounds(n_frames: int, world: int) -> list[int]:
@@ -159,8 +159,9 @@ class GatheredResults:
     def scan_hash_dist(self, first: int = 0, n: int | None = None) -> np.ndarray:
         n = self._n - first if n is None else n
         out = self._out(n)
-        prev = self._hashes.ptr + (first - 1) * 8 * HASH_WORDS if first > 0 else None
-        self._capi.check(self._lib.psd_scan_hash_dist(self._hashes.ptr + first * 8 * HASH_WORDS, n, self.hash_size,
+        row = 8 * hash_words(self.hash_size)   # bytes per frame: the PSD_HASH_WORDS_FOR(size) stride
+        prev = self._hashes.ptr + (first - 1) * row if first > 0 else None
+        self._capi.check(self._lib.psd_scan_hash_dist(self._hashes.ptr + first * row, n, self.hash_size,
                                                       prev, out.ptr, None), "psd_scan_hash_dist")
         return self._fetch(out, n)
 
