@@ -13,7 +13,8 @@
 //   -> classify: Sobel / L1 magnitude / NMS / double threshold straight into two bit planes,
 //      E = strong pixels, C = candidates (weak or strong), both tile-major      [1 launch]
 //   -> hysteresis: E grows inside C until nothing changes, bit-parallel          [1 cooperative launch]
-//   -> k x k max on the bits in one pass, popcount SAD against the previous frame [2 launches]
+//   -> k x k max on the bits in one pass (k <= 17) or two separable passes (k >= 19),
+//      popcount SAD against the previous frame                                   [2 - 3 launches]
 // (the first version kept a byte class map, 4-byte union-find labels per pixel and 12 launches per
 // batch).
 #include <cooperative_groups.h>
@@ -382,42 +383,6 @@ __device__ __forceinline__ uint32_t tiled_word(const uint32_t* __restrict__ plan
     return plane[((int64_t)(y >> 5) * tiles_x + (wq >> 1)) * kTileWords + ((y & 31) << 1) + (wq & 1)];
 }
 
-// one row of one word column, horizontally dilated: OR over |dx| <= r of the row shifted by dx (funnel shifts
-// across word boundaries); columns >= W of the last word stay 0 (the SAD counts whole words)
-template <int R>
-__device__ __forceinline__ uint32_t hdil_word(const uint32_t* __restrict__ plane, int tiles_x, int Wq, int y, int wq,
-                                              int r, uint32_t keep) {
-    const uint32_t cur = tiled_word(plane, tiles_x, y, wq);
-    const uint32_t prv = (wq > 0) ? tiled_word(plane, tiles_x, y, wq - 1) : 0u;
-    const uint32_t nxt = (wq + 1 < Wq) ? tiled_word(plane, tiles_x, y, wq + 1) : 0u;
-    uint32_t o = cur;
-    if (R > 0) {
-#pragma unroll
-        for (int s = 1; s <= R; ++s) o |= __funnelshift_r(cur, nxt, s) | __funnelshift_l(prv, cur, s);
-    } else {
-        for (int s = 1; s <= r; ++s) o |= __funnelshift_r(cur, nxt, s) | __funnelshift_l(prv, cur, s);
-    }
-    return o & keep;
-}
-
-// any kernel size: one thread per output word, (2 r + 1) x 3 loads
-__global__ void __launch_bounds__(256) psd_edge_dilate_any_bits_kernel(const uint32_t* __restrict__ in,
-                                                                       uint32_t* __restrict__ dil, int H, int Wq,
-                                                                       int tiles_x, int64_t tile_words_per_frame,
-                                                                       int r, uint32_t last_word_mask) {
-    const int64_t per_frame = (int64_t)H * Wq;
-    const int64_t f = blockIdx.y;
-    const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
-    if (i >= per_frame) return;
-    const int y = (int)(i / Wq), wq = (int)(i - (int64_t)y * Wq);
-    const uint32_t* src = in + f * tile_words_per_frame;
-    const uint32_t keep = (wq == Wq - 1) ? last_word_mask : 0xFFFFFFFFu;
-    uint32_t o = 0;
-    const int ya = max(y - r, 0), yb = min(y + r, H - 1);
-    for (int yy = ya; yy <= yb; ++yy) o |= hdil_word<0>(src, tiles_x, Wq, yy, wq, r, keep);
-    dil[f * per_frame + i] = o;
-}
-
 // the usual kernel sizes (k = 2 R + 1 <= 17): a thread owns one word column of a band of kDilBand rows and
 // marches down it with the last 2 R + 1 horizontally dilated rows in registers (the row loop is unrolled
 // 2 R + 1 times so the ring slots are register names).  Consecutive lanes own consecutive word columns of the
@@ -477,6 +442,156 @@ __global__ void __launch_bounds__(256) psd_edge_dilate_bits_kernel(const uint32_
             }
         }
     }
+}
+
+// every larger kernel size (r >= kLargeMinR): the k x k box is separable, a horizontal window-OR of radius r into
+// the row-major plane `hdil`, then a vertical one into the dilated plane.  Neither pass does work that grows with k
+// beyond log2 k per word.  Radii are clamped to W - 1 / H - 1 first: a window that covers the whole row or column
+// from every pixel is saturated, and taps outside the image contribute nothing (cv2.dilate's default border).
+// (It replaced a one-thread-per-word kernel for k = 19 .. 63 that ORed (2 r + 1) rows x (2 r + 1) shifts per word:
+// on an H100 at 1980 MHz that took 6.3 - 34 us per 1080p frame against 1.0 - 1.2 us for the two passes, and
+// 27 - 137 us per 4K frame against 3.8 - 5.1 us; bench_dilate.py.)
+constexpr int kLargeMinR = 9;    // k >= 19
+constexpr int kHdilRows = 8;     // rows per CTA of the horizontal pass (a warp per row), fewer for very wide rows
+
+// 32 bits of a shared-memory row starting at bit `bit` (>= 0); words at or past `len` read as 0
+__device__ __forceinline__ uint32_t row_bits(const uint32_t* row, int len, int bit) {
+    const int w = bit >> 5;
+    const uint32_t lo = w < len ? row[w] : 0u;
+    const uint32_t hi = w + 1 < len ? row[w + 1] : 0u;
+    return __funnelshift_r(lo, hi, bit & 31);
+}
+
+// Horizontal pass.  A CTA takes `rows` consecutive rows of one frame (they lie in one tile row, and each tile holds
+// them as 2 x rows consecutive words, so the load is contiguous per tile) into shared memory, each behind `pad`
+// zero words that stand for bit positions -32 pad .. -1.  A warp then doubles windows on its row,
+// W_2l(x) = W_l(x) | W_l(x + l) with W_1 = the row, up to the largest power of two L <= k = 2 r + 1, and writes
+// out(x) = W_L(x - r) | W_L(x + r - L + 1): two windows of length L that together cover exactly [x - r, x + r]
+// (pad = ceil(r / 32) keeps every position read >= -32 pad).  Columns >= W of the last word stay 0.
+__global__ void __launch_bounds__(32 * kHdilRows) psd_edge_hdil_rows_kernel(
+    const uint32_t* __restrict__ in, uint32_t* __restrict__ hdil, int H, int Wq, int tiles_x,
+    int64_t tile_words_per_frame, int rows, int pad, int r, int L, uint32_t last_word_mask) {
+    extern __shared__ uint32_t srow[];
+    const int len = pad + 2 * tiles_x;   // words of one row buffer
+    const int64_t f = blockIdx.y;
+    const int y0 = blockIdx.x * rows;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const uint32_t* src = in + f * tile_words_per_frame + (int64_t)(y0 >> 5) * tiles_x * kTileWords + 2 * (y0 & 31);
+    const int per_tile = 2 * rows;
+    for (int i = threadIdx.x; i < per_tile * tiles_x; i += blockDim.x) {
+        const int tx = i / per_tile, j = i - tx * per_tile;   // word j of this tile's slice: row j / 2, word j % 2
+        srow[(j >> 1) * 2 * len + pad + 2 * tx + (j & 1)] = src[(int64_t)tx * kTileWords + j];
+    }
+    for (int i = threadIdx.x; i < rows * pad; i += blockDim.x) srow[(i / pad) * 2 * len + i % pad] = 0u;
+    __syncthreads();
+    const int y = y0 + warp;
+    if (y >= H) return;
+    uint32_t* a = srow + warp * 2 * len;
+    uint32_t* b = a + len;
+    for (int l = 1; l < L; l <<= 1) {
+        for (int w = lane; w < len; w += 32) b[w] = a[w] | row_bits(a, len, 32 * w + l);
+        __syncwarp();   // b complete; every read of a is done before the next step overwrites it
+        uint32_t* t = a; a = b; b = t;
+    }
+    uint32_t* dst = hdil + (f * H + y) * (int64_t)Wq;
+    for (int w = lane; w < Wq; w += 32) {
+        const int x = 32 * (pad + w);
+        uint32_t o = row_bits(a, len, x - r) | row_bits(a, len, x + r - L + 1);
+        if (w == Wq - 1) o &= last_word_mask;
+        dst[w] = o;
+    }
+}
+
+// Vertical pass: van Herk / Gil-Werman.  Pad the column with r zero rows on either side; output row y then ORs the
+// padded rows y .. y + k - 1.  Cut the padded column into blocks of k rows: that window is the suffix of block
+// b = y / k from row y on and the prefix of block b + 1 up to row y + k - 1.  A thread owns one word column of one
+// block of output rows: it marches up block b storing the suffix ORs, then down block b + 1 ORing the running
+// prefix in - 3 ORs and 5 accesses per word whatever k is.
+__global__ void __launch_bounds__(256) psd_edge_vdil_cols_kernel(const uint32_t* __restrict__ hdil,
+                                                                 uint32_t* __restrict__ out, int H, int Wq, int r,
+                                                                 int blocks, int64_t n_threads) {
+    const int64_t gid = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+    if (gid >= n_threads) return;
+    const int wq = (int)(gid % Wq);
+    const int b = (int)((gid / Wq) % blocks);
+    const int64_t f = gid / ((int64_t)Wq * blocks);
+    const int k = 2 * r + 1;
+    const uint32_t* src = hdil + f * H * (int64_t)Wq + wq;   // padded row q is image row q - r
+    uint32_t* dst = out + f * H * (int64_t)Wq + wq;
+    const int q0 = b * k, y_end = min(q0 + k, H);
+    uint32_t acc = 0;
+#pragma unroll 4
+    for (int q = min(q0 + k - 1, r + H - 1); q >= q0; --q) {   // padded rows >= r + H are 0
+        if (q >= r) acc |= src[(int64_t)(q - r) * Wq];
+        if (q < H) dst[(int64_t)q * Wq] = acc;
+    }
+    acc = 0;
+#pragma unroll 4
+    for (int y = q0; y < y_end; ++y) {   // padded row y + k of block b + 1 (> r always)
+        if (y > q0) dst[(int64_t)y * Wq] |= acc;
+        if (y + k < r + H) acc |= src[(int64_t)(y + k - r) * Wq];
+    }
+}
+
+static int hdil_smem_bytes(int rows, int pad, int tiles_x) { return rows * 2 * (pad + 2 * tiles_x) * 4; }
+
+static int max_smem_optin() {
+    static int optin = 0;
+    if (optin == 0) {
+        int dev = 0;
+        if (cudaGetDevice(&dev) != cudaSuccess ||
+            cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev) != cudaSuccess)
+            optin = 48 * 1024;
+    }
+    return optin;
+}
+
+// rows per CTA of the horizontal pass for a frame width and kernel size, 0 if one row does not fit
+static int hdil_rows(int W, int ksize) {
+    const int Wq = (W + 31) / 32, tiles_x = (Wq + 1) / 2;
+    const int r = min(ksize / 2, W - 1), pad = (r + 31) / 32;
+    int rows = kHdilRows;
+    while (rows > 0 && hdil_smem_bytes(rows, pad, tiles_x) > max_smem_optin()) rows >>= 1;
+    return rows;
+}
+
+bool edge_dilate_separable(int ksize) { return ksize / 2 >= kLargeMinR; }
+
+int edge_dilate_check(int W, int ksize) {
+    if (!edge_dilate_separable(ksize)) return PSD_OK;
+    PSD_REQUIRE(hdil_rows(W, ksize) > 0, "frame width %d is too wide for the kernel size %d dilation (one row and "
+                "its padding must fit in %d bytes of shared memory)", W, ksize, max_smem_optin());
+    return PSD_OK;
+}
+
+static int launch_dilate_separable(const uint32_t* in, uint32_t* hdil, uint32_t* out, int n, int W, int H, int ksize,
+                                   uint32_t mask, cudaStream_t stream) {
+    const int Wq = (W + 31) / 32, tiles_x = (Wq + 1) / 2;
+    const int rh = min(ksize / 2, W - 1), rv = min(ksize / 2, H - 1);
+    const int pad = (rh + 31) / 32;
+    int L = 1;
+    while (2 * L <= 2 * rh + 1) L *= 2;
+    const int rows = hdil_rows(W, ksize);
+    PSD_REQUIRE(rows > 0, "frame width %d is too wide for the kernel size %d dilation", W, ksize);
+    const int smem = hdil_smem_bytes(rows, pad, tiles_x);
+    if (smem > 48 * 1024) {
+        static int raised = 0;   // the attribute is a ceiling, not a reservation: raise it once to the device limit
+        if (!raised) {
+            PSD_CUDA(cudaFuncSetAttribute(psd_edge_hdil_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                          max_smem_optin()));
+            raised = 1;
+        }
+    }
+    // rows per CTA divide 32, so a CTA never straddles two tile rows; rows past H load the planes' zero padding
+    dim3 hg((unsigned)((H + rows - 1) / rows), (unsigned)n);
+    psd_edge_hdil_rows_kernel<<<hg, 32 * rows, smem, stream>>>(in, hdil, H, Wq, tiles_x, edge_tile_words(W, H), rows,
+                                                             pad, rh, L, mask);
+    PSD_CHECK_LAUNCH();
+    const int k = 2 * rv + 1, blocks = (H + k - 1) / k;
+    const int64_t n_threads = (int64_t)Wq * blocks * n;
+    psd_edge_vdil_cols_kernel<<<(unsigned)((n_threads + 255) / 256), 256, 0, stream>>>(hdil, out, H, Wq, rv, blocks,
+                                                                                      n_threads);
+    return PSD_OK;
 }
 
 template <int R>
@@ -588,7 +703,11 @@ int launch_edges(const EdgeBuffers& b, int n, int W, int H, int ksize, bool have
     count_launch(3);
     const int r = ksize / 2;
     const uint32_t last_mask = (W & 31) ? ((1u << (W & 31)) - 1u) : 0xFFFFFFFFu;
-    switch (r) {
+    if (edge_dilate_separable(ksize)) {   // k >= 19
+        const int rc = launch_dilate_separable(b.bits_in, b.bits_hdil, b.bits_dil, n, W, H, ksize, last_mask, stream);
+        if (rc) return rc;
+        count_launch(1);   // the second pass
+    } else switch (r) {
         case 1: launch_dilate<1>(b.bits_in, b.bits_dil, n, H, Wq, last_mask, stream); break;
         case 2: launch_dilate<2>(b.bits_in, b.bits_dil, n, H, Wq, last_mask, stream); break;
         case 3: launch_dilate<3>(b.bits_in, b.bits_dil, n, H, Wq, last_mask, stream); break;
@@ -597,11 +716,7 @@ int launch_edges(const EdgeBuffers& b, int n, int W, int H, int ksize, bool have
         case 6: launch_dilate<6>(b.bits_in, b.bits_dil, n, H, Wq, last_mask, stream); break;
         case 7: launch_dilate<7>(b.bits_in, b.bits_dil, n, H, Wq, last_mask, stream); break;
         case 8: launch_dilate<8>(b.bits_in, b.bits_dil, n, H, Wq, last_mask, stream); break;
-        default: {   // any other kernel size
-            dim3 cgd((unsigned)((per_frame + 255) / 256), (unsigned)n);
-            psd_edge_dilate_any_bits_kernel<<<cgd, 256, 0, stream>>>(b.bits_in, b.bits_dil, H, Wq, (Wq + 1) / 2,
-                                                                     edge_tile_words(W, H), r, last_mask);
-        }
+        default: PSD_REQUIRE(false, "edge kernel size %d has no dilation kernel", ksize);
     }
     PSD_CHECK_LAUNCH();
     dim3 sg((unsigned)min((int64_t)64, (per_frame + 255) / 256), (unsigned)n);

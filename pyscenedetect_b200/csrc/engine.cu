@@ -283,7 +283,7 @@ void psd_engine_destroy(psd_engine* e) {
     cudaFree(e->carry); cudaFree(e->d_sums); cudaFree(e->d_yhist); cudaFree(e->d_hash);
     hash_plan_destroy(&e->hash);
     cudaFree(e->eb.vplane); cudaFree(e->eb.vhist); cudaFree(e->eb.thresholds); cudaFree(e->eb.cand);
-    cudaFree(e->eb.tmp); cudaFree(e->eb.bits_in); cudaFree(e->eb.bits_dil);
+    cudaFree(e->eb.tmp); cudaFree(e->eb.bits_in); cudaFree(e->eb.bits_dil); cudaFree(e->eb.bits_hdil);
     cudaFree(e->eb.carry_bits); cudaFree(e->eb.dirty); cudaFree(e->eb.hyst_flags);
     for (cudaEvent_t ev : e->ev_pool) cudaEventDestroy(ev);
     if (e->copy_stream) cudaStreamDestroy(e->copy_stream);
@@ -346,9 +346,9 @@ int psd_engine_create(const psd_config* cfg, psd_engine** out) {
             k = 4 + (int)nearbyint(sqrt((double)e->W * (double)e->H) / 192.0);
             if ((k & 1) == 0) k += 1;
         }
-        if (k > 63) {  // the bit-plane dilation shifts words by at most 31 bits
+        if (edge_dilate_check(e->W, k) != PSD_OK) {
             psd_engine_destroy(e);
-            PSD_REQUIRE(false, "edge kernel size %d is not supported (odd sizes 3 .. 63)", k);
+            return PSD_ERR_INVALID;
         }
         e->ksize = k;
     }
@@ -392,6 +392,7 @@ int psd_engine_create(const psd_config* cfg, psd_engine** out) {
         ENG_CUDA(cudaMemset(e->eb.bits_in, 0, tiled));
         ENG_CUDA(cudaMalloc(&e->eb.tmp, (size_t)e->P));
         ENG_CUDA(cudaMalloc(&e->eb.bits_dil, words * 4 * e->max_batch));
+        if (edge_dilate_separable(e->ksize)) ENG_CUDA(cudaMalloc(&e->eb.bits_hdil, words * 4 * e->max_batch));
         ENG_CUDA(cudaMalloc(&e->eb.carry_bits, words * 4));
         ENG_CUDA(cudaMalloc(&e->eb.vhist, (size_t)e->max_batch * 256 * 4));
         ENG_CUDA(cudaMalloc(&e->eb.thresholds, (size_t)e->max_batch * 2 * 4));

@@ -83,6 +83,7 @@ struct EdgeBuffers {
                         // tile (ty, tx) = 32 rows x 64 columns = 64 consecutive words, row r at words 2r, 2r+1
     uint32_t* bits_in;  // same layout: strong pixels after classify, the Canny map after hysteresis
     uint32_t* bits_dil; // [n][H][Wq] dilated edges, row-major
+    uint32_t* bits_hdil;// [n][H][Wq] horizontal pass of the separable dilation (kernel sizes >= 19 only, else null)
     uint32_t* carry_bits; // [H][Wq] dilated edges of the predecessor frame
     uint8_t* tmp;       // [P] scratch for debug taps
     uint8_t* dirty;     // [2][n][tiles] hysteresis: tiles to revisit (double-buffered by round parity)
@@ -92,6 +93,8 @@ int launch_edges(const EdgeBuffers& b, int n, int width, int height, int ksize, 
                  psd_frame_sums* sums, cudaStream_t stream);
 int edge_unpack(const uint32_t* bits, uint8_t* out, int W, int H, bool tile_major, cudaStream_t stream);
 int64_t edge_tile_words(int W, int H);   // words per frame of a tile-major bit plane
+bool edge_dilate_separable(int ksize);  // this kernel size dilates in two passes through EdgeBuffers::bits_hdil
+int edge_dilate_check(int W, int ksize); // PSD_OK, or PSD_ERR_INVALID if a row of the separable pass is too wide
 
 // ---- perceptual hash (hash_kernels.cu) ----
 struct HashPlan {        // per-engine tables for one (frame size, hash size, lowpass)
