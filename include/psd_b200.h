@@ -61,7 +61,8 @@ typedef struct psd_config {
     int32_t width, height;
     uint32_t features;        /* PSD_F_* */
     int32_t edge_kernel_size; /* dilate kernel k (odd >= 3); 0 = content_detector.py:39-46 estimate */
-    int32_t max_batch;        /* max frames per submit call (staging is sized for it) */
+    int32_t max_batch;        /* frames per batch (staging and per-batch scratch are sized for it); an aligned
+                                 device submission without resize, edges or hashes is scored in one batch */
     uint32_t flags;           /* reserved: no flags are defined, must be 0 */
     int32_t hash_size;        /* PSD_F_HASH: HashDetector(size=...) >= 1, 0 = 8 */
     int32_t hash_lowpass;     /* PSD_F_HASH: HashDetector(lowpass=...) >= 1, 0 = 2; the scored frame must be at

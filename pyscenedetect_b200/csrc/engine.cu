@@ -508,9 +508,16 @@ int psd_engine_submit_device(psd_engine* e, const void* dptr, int64_t n, int64_t
     int rc = ensure_capacity(e, e->n_frames + n + 1);
     if (rc) return rc;
     const uint8_t* p = (const uint8_t*)dptr;
+    // Frames the fused pass can read where they are (no resize, no edge or hash scratch, 16-byte aligned) are
+    // scored in one launch: max_batch only sizes staging and those per-batch buffers, and every launch costs a
+    // pipeline fill and drain and a work split whose busiest SM sets the launch's time.  Only the kernels'
+    // int32 frame counts limit such a batch (2^30 keeps their grid arithmetic clear of overflow too).
+    const bool in_place = !e->resize && !(e->features & (PSD_F_EDGES | PSD_F_HASH)) &&
+                          (((uintptr_t)p | (uintptr_t)frame_stride) & 15) == 0;
+    const int64_t batch = in_place ? ((int64_t)1 << 30) : (int64_t)e->max_batch;
     int64_t done = 0;
     while (done < n) {
-        const int64_t b = (n - done < e->max_batch) ? (n - done) : e->max_batch;
+        const int64_t b = (n - done < batch) ? (n - done) : batch;
         rc = run_batch(e, p + done * frame_stride, frame_stride, b, e->n_frames + 1, false);
         if (rc) return rc;
         e->n_frames += b;

@@ -39,7 +39,7 @@ __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t by
 // ---------------------------------------------------------------------------------------------
 // Warp-specialised, persistent kernel (the first P16 pixels of every frame).
 //
-// One CTA per SM for the whole launch: 24 consumer warps + 1 producer warp.  The work is cut into items
+// One CTA per SM for the whole launch: 24 consumer warps + 4 side warps.  The work is cut into items
 // (strip of 12288 pixels x chunk of consecutive frames); CTA b walks items b, b + grid, b + 2 grid, ...
 // Within an item the previous frame's H,S,V of a thread's 16 pixels stay in registers, so HBM traffic is
 // one read of each BGR byte (+1 halo frame per item).
@@ -51,9 +51,12 @@ __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t by
 //
 // No CTA-wide barrier in the frame loop: consumers wait on the stage's FULL mbarrier (TMA complete_tx),
 // pull their 48 bytes, do the arithmetic, add their SADs to the stage's per-lane shared accumulators and
-// arrive on the stage's EMPTY mbarrier; the producer warp waits for the 24 arrivals, reads the stage's
-// totals, re-arms the stage with the frame kWsStages slots ahead and then flushes the totals / histogram
-// bins of the retired frame to HBM with integer atomics.
+// arrive on the stage's EMPTY mbarrier.  Side warp s (warp 24 + s, so one per SM sub-partition) owns
+// stage s: it waits for the 24 arrivals, takes and zeroes the stage's totals and histogram bins, re-arms
+// the stage with the frame kWsStages slots ahead (one lane issues the copy) and then flushes what it took
+// to HBM with integer atomics.  EMPTY phases complete in slot order, so the copies are still issued in
+// slot order.  The stages advance only as fast as their slowest sub-partition, so the per-frame
+// bookkeeping is dealt out to all four instead of adding to the issue load of sub-partition 0.
 //
 // An item whose frame count is not a multiple of the consumer loop's unroll factor is padded with null
 // slots (the producer completes the FULL barrier without a copy, the consumers only arrive), so a loop
@@ -65,8 +68,10 @@ __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t by
 // thread slices (1080p: 168 full strips + one of 9216 px).
 constexpr int kWsConsumerWarps = 24;
 constexpr int kWsConsumers = kWsConsumerWarps * 32;  // 768
-constexpr int kWsThreads = kWsConsumers + 32;        // + producer warp
 constexpr int kWsStages = 4;
+constexpr int kWsSideWarps = kWsStages;              // side warp s retires and re-arms stage s
+constexpr int kWsThreads = kWsConsumers + kWsSideWarps * 32;  // 28 warps x 72 registers fit the 64 K register file
+static_assert(kWsSideWarps == 4 && kWsConsumerWarps % 4 == 0, "one side warp per SM sub-partition");
 constexpr int kWsUnroll = 4;                         // frames per consumer loop body: all stage offsets immediate
 constexpr int kWsStripPx = kWsConsumers * kPxPerThread;  // 12288 pixels
 constexpr int kWsStripBytes = kWsStripPx * 3;            // 36864 bytes
@@ -77,12 +82,10 @@ struct __align__(128) WsSmem {
     float lut[256 * 64];
     unsigned long long full[kWsStages];
     unsigned long long empty[kWsStages];   // must follow `full` (addressed as full + kWsStages * 8)
-    // per-lane running totals of sadH, sadS, sadV, bgr: every consumer thread adds its partial to the
-    // word of ITS lane (32 distinct banks: one conflict-free red.shared per channel per thread, no
-    // warp reduction, no election).  Never zeroed: the producer keeps the totals it saw last and
-    // flushes the difference, so its bookkeeping needs no ordering against the consumers' adds.
+    // per-lane totals of sadH, sadS, sadV, bgr: every consumer thread adds its partial to the word of ITS
+    // lane (32 distinct banks: one conflict-free red.shared per channel per thread, no warp reduction, no
+    // election).  The side warp that retires the stage zeroes them before it hands the stage back.
     uint32_t accl[kWsStages][4][32];
-    uint32_t accl_seen[kWsStages][4][32];
     uint32_t accl_sink[kWsStages][4][32];  // where threads without pixels / without a predecessor frame add
     uint32_t yhist[kWsStages][256];
     uint32_t vhist[kWsStages][256];
@@ -265,7 +268,6 @@ __global__ void __launch_bounds__(kWsThreads, 1) psd_score_ws_kernel(const Score
     }
     for (int i = tid; i < kWsStages * 4 * 32; i += kWsThreads) {
         (&sm.accl[0][0][0])[i] = 0;
-        (&sm.accl_seen[0][0][0])[i] = 0;
         (&sm.accl_sink[0][0][0])[i] = 0;
     }
     if (kHSV) lut_fill7(sm.lut, tid, kWsThreads);
@@ -279,88 +281,90 @@ __global__ void __launch_bounds__(kWsThreads, 1) psd_score_ws_kernel(const Score
     __syncthreads();
 
     if (tid >= kWsConsumers) {
-        // ===================== producer warp =====================
-        // Two cursors over the same slot sequence (items of this CTA, slots of each item): `iss` is the slot
-        // whose copy is issued next, `ret` the slot retired next; iss runs kWsStages slots ahead of ret.
+        // ===================== side warps =====================
+        // Cursors over this CTA's slot sequence (items of this CTA, slots of each item).  Every item has a
+        // multiple of kWsStages slots, so slot k of an item always sits in stage k mod kWsStages: side warp
+        // `rs` owns slots rs, rs + kWsStages, ... of every item.  It retires them (`ret`) and re-arms its
+        // stage with the slot kWsStages further on (`iss`, one lap of the ring ahead of `ret`).
         struct Cursor {
             int item, slot;
             WsItem w;
         };
+        const int rs = (tid - kWsConsumers) >> 5;  // the stage this warp owns (= its SM sub-partition)
         auto load = [&](Cursor& c) { if (c.item < n_items) c.w = ws_item(a, c.item); };
         auto advance = [&](Cursor& c) {
-            if (++c.slot == c.w.slots) { c.slot = 0; c.item += gridDim.x; load(c); }
+            c.slot += kWsStages;
+            if (c.slot >= c.w.slots) { c.slot = rs; c.item += gridDim.x; load(c); }
         };
-        auto issue = [&](const Cursor& c, int stage) {  // lane 0 only
-            if (c.slot < c.w.walked) {
-                const int fi = c.w.f0 - 1 + c.w.it_begin + c.slot;
-                const uint8_t* src = (fi < 0 ? a.prev : a.frames + (int64_t)fi * a.frame_stride) + (int64_t)c.w.px0 * 3;
-                const uint32_t bytes = (uint32_t)c.w.valid_px * 3u;
-                mbar_expect_tx(&sm.full[stage], bytes);
-                bulk_g2s(sm.ring[stage], src, bytes, &sm.full[stage]);
-            } else {
-                mbar_arrive_off<0>(smem_u32(&sm.full[stage]));  // padding slot: complete the phase without a copy
+        auto issue = [&](Cursor& c) {
+            if (lane == 0) {
+                if (c.slot < c.w.walked) {
+                    const int fi = c.w.f0 - 1 + c.w.it_begin + c.slot;
+                    const uint8_t* src = (fi < 0 ? a.prev : a.frames + (int64_t)fi * a.frame_stride) + (int64_t)c.w.px0 * 3;
+                    const uint32_t bytes = (uint32_t)c.w.valid_px * 3u;
+                    mbar_expect_tx(&sm.full[rs], bytes);
+                    bulk_g2s(sm.ring[rs], src, bytes, &sm.full[rs]);
+                } else {
+                    mbar_arrive_off<0>(smem_u32(&sm.full[rs]));  // padding slot: complete the phase without a copy
+                }
             }
+            advance(c);
         };
-        Cursor iss{(int)blockIdx.x, 0, {}}, ret{(int)blockIdx.x, 0, {}};
-        load(iss);
-        ret.w = iss.w;
-        for (int s = 0; s < kWsStages && iss.item < n_items; ++s) {
-            if (lane == 0) issue(iss, s);
-            advance(iss);
-        }
-        int stage = 0;
+        Cursor ret{(int)blockIdx.x, rs, {}};
+        load(ret);
+        Cursor iss = ret;
+        issue(iss);
         uint32_t parity = 0;
         while (ret.item < n_items) {
-            mbar_wait_hint(&sm.empty[stage], parity);
+            mbar_wait_hint(&sm.empty[rs], parity);
             const int it = ret.w.it_begin + ret.slot;             // 0 = halo frame
             const bool real = ret.slot < ret.w.walked;
             const bool own = real && it >= 1;                     // this CTA accounts for frame fi
             const int fi = ret.w.f0 - 1 + it;
-            // the per-lane totals are read BEFORE the stage is re-armed: no consumer can add the next
-            // frame of this stage to them until the copy issued below has landed
+            // the per-lane totals are taken and zeroed BEFORE the stage is re-armed: no consumer can add the
+            // next frame of this stage to them until the copy issued below has landed
             uint32_t tot[4] = {0u, 0u, 0u, 0u};
             if (own && (kHSV || kSUM)) {
 #pragma unroll
-                for (int c = 0; c < 4; ++c)
-                    if ((c < 3 && kHSV) || (c == 3 && kSUM)) tot[c] = sm.accl[stage][c][lane];
+                for (int c = 0; c < 4; ++c) {
+                    if ((c < 3 && kHSV) || (c == 3 && kSUM)) {
+                        tot[c] = sm.accl[rs][c][lane];
+                        sm.accl[rs][c][lane] = 0;
+                    }
+                }
             }
             if (own) {
                 if (kYH) {
 #pragma unroll
                     for (int b = lane; b < 256; b += 32) {
-                        const uint32_t v = sm.yhist[stage][b];
-                        if (v) { sm.yhist[stage][b] = 0; atomicAdd(&a.yhist[(int64_t)fi * 256 + b], v); }
+                        const uint32_t v = sm.yhist[rs][b];
+                        if (v) { sm.yhist[rs][b] = 0; atomicAdd(&a.yhist[(int64_t)fi * 256 + b], v); }
                     }
                 }
                 if (kEDGE) {
 #pragma unroll
                     for (int b = lane; b < 256; b += 32) {
-                        const uint32_t v = sm.vhist[stage][b];
-                        if (v) { sm.vhist[stage][b] = 0; atomicAdd(&a.vhist[(int64_t)fi * 256 + b], v); }
+                        const uint32_t v = sm.vhist[rs][b];
+                        if (v) { sm.vhist[rs][b] = 0; atomicAdd(&a.vhist[(int64_t)fi * 256 + b], v); }
                     }
                 }
                 if (ret.item < a.n_chunks && lane == 0)  // an item of strip 0
                     a.sums[fi].has_prev = (fi > 0 || a.prev != nullptr) ? 1ull : 0ull;
             }
-            __syncwarp();  // the histogram zeroing above is ordered before lane 0 re-arms the stage
-            if (iss.item < n_items) {
-                if (lane == 0) issue(iss, stage);
-                advance(iss);
-            }
+            __syncwarp();  // the zeroing above is ordered before lane 0 re-arms the stage
+            if (iss.item < n_items) issue(iss);
             if (own && (kHSV || kSUM)) {  // after the re-arm: the copy engine's queue is fed first
 #pragma unroll
                 for (int c = 0; c < 4; ++c) {
                     if ((c < 3 && !kHSV) || (c == 3 && !kSUM)) continue;
-                    const uint32_t d = tot[c] - sm.accl_seen[stage][c][lane];
-                    sm.accl_seen[stage][c][lane] = tot[c];
-                    const uint32_t v = __reduce_add_sync(0xFFFFFFFFu, d);
+                    const uint32_t v = __reduce_add_sync(0xFFFFFFFFu, tot[c]);
                     if (lane == 0 && v)
                         atomicAdd(reinterpret_cast<unsigned long long*>(&a.sums[fi]) + (c < 3 ? c : 4),
                                   (unsigned long long)v);
                 }
             }
             advance(ret);
-            if (++stage == kWsStages) { stage = 0; parity ^= 1u; }
+            parity ^= 1u;
         }
         return;
     }
