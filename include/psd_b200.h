@@ -143,8 +143,30 @@ int psd_engine_timing_ms(psd_engine* e, float* total_ms, float* score_kernel_ms,
                          uint64_t* score_kernel_launches);
 /* effective dilate kernel size used for the edge component */
 int psd_engine_edge_kernel_size(const psd_engine* e);
+
+/* ---- slots: several ContentDetector kernel sizes and HashDetector geometries in one engine, as the reference's
+ *      SceneManager runs any mix of detectors (scene_manager.py:337-352, each detector's process_frame on the same
+ *      frame).  Every batch is uploaded, resized, scored by the fused pass and Canny-classified once; each edge
+ *      slot adds a dilation and a SAD (content_detector.py:238), each hash slot its INTER_AREA taps, DCT and
+ *      median (hash_detector.py:130-149) over the one gray pass.  Slot 0 is the psd_config's kernel size /
+ *      geometry.  Slots can be added only while the engine holds no frames (after create or reset, before any
+ *      submit or halo; PSD_ERR_STATE otherwise); a size / geometry already present returns its slot.  Each slot
+ *      has its own carried predecessor and halo result. ---- */
+/* content_detector.py:135-138 kernel_size of another detector (0 = the :39-46 estimate); needs PSD_F_EDGES */
+int psd_engine_add_edge_kernel_size(psd_engine* e, int32_t kernel_size, int32_t* slot);
+/* hash_detector.py:50-51 size / lowpass of another HashDetector (0 = 8 / 2); needs PSD_F_HASH */
+int psd_engine_add_hash_geometry(psd_engine* e, int32_t size, int32_t lowpass, int32_t* slot);
+/* effective kernel size of an edge slot, -1 if there is no such slot */
+int psd_engine_edge_kernel_size_at(const psd_engine* e, int32_t slot);
+/* device array of an edge slot's sad_edges (stream frame i at sad_edges[i], the halo frame's one before; valid until
+ * destroy/reset); NULL for slot 0, whose SADs are psd_frame_sums.sad_edges */
+int psd_engine_device_edge_sads(psd_engine* e, int32_t slot, const uint64_t** sad_edges);
+/* psd_engine_device_hash / psd_engine_read_hash of a hash slot (stride PSD_HASH_WORDS_FOR(that slot's size)) */
+int psd_engine_device_hash_at(psd_engine* e, int32_t slot, const uint64_t** hashes);
+int psd_engine_read_hash_at(psd_engine* e, int32_t slot, int64_t first, int64_t n, uint64_t* out);
 /* debug/test taps: copy intermediate planes of frame `index` of the LAST submitted batch.
- * which: 0 = scored-size BGR (after resize), 1 = V plane, 2 = Canny map (0/255), 3 = dilated edges */
+ * which: 0 = scored-size BGR (after resize), 1 = V plane, 2 = Canny map (0/255), 3 = dilated edges (of the
+ * last edge slot) */
 int psd_engine_debug_plane(psd_engine* e, int which, int64_t index, uint8_t* out, size_t cap);
 
 /* ---- trailing device scans over result arrays (all pointers are DEVICE pointers unless the
@@ -154,6 +176,11 @@ int psd_engine_debug_plane(psd_engine* e, int which, int64_t index, uint8_t* out
 int psd_scan_content(const psd_frame_sums* sums, int64_t n, int64_t n_pixels, const double weights[4],
                      double weight_abs_sum /* sum(abs(w)) as the host computed it */,
                      double* out_components, double* out_content_val, void* stream);
+/* psd_scan_content with the edge component's SAD read from sad_edges[n] (an edge slot's array,
+ * psd_engine_device_edge_sads) when it is non-NULL: content_detector.py:166-180 for that kernel size */
+int psd_scan_content_edges(const psd_frame_sums* sums, const uint64_t* sad_edges, int64_t n, int64_t n_pixels,
+                           const double weights[4], double weight_abs_sum, double* out_components,
+                           double* out_content_val, void* stream);
 /* adaptive_detector.py:100-143: ratio for target i uses scores[i-w .. i+w]; out_ratio[i] is NaN
  * where the window is incomplete.  scores[] is the content_val array incl. frame 0's 0.0. */
 int psd_scan_adaptive(const double* scores, int64_t n, int32_t window_width, double min_content_val,
@@ -249,6 +276,11 @@ int psd_engine_scan_average_host(psd_engine* e, int64_t first, int64_t n, double
 int psd_engine_scan_hist_correl_host(psd_engine* e, int64_t first, int64_t n, int32_t bins,
                                      double* out_correl);
 int psd_engine_scan_hash_dist_host(psd_engine* e, int64_t first, int64_t n, double* out_dist);
+/* the same over an edge slot's / a hash slot's results */
+int psd_engine_scan_content_host_at(psd_engine* e, int32_t edge_slot, int64_t first, int64_t n,
+                                    const double weights[4], double weight_abs_sum, double* out_components,
+                                    double* out_content_val);
+int psd_engine_scan_hash_dist_host_at(psd_engine* e, int32_t hash_slot, int64_t first, int64_t n, double* out_dist);
 
 /* ---- synthetic input generator (bench.py / tests; pyscenedetect_b200/synth.py bit-exact twin) ---- */
 /* params_host: [n][24] int32 rows of ScenePlan.params for frames first..first+n-1 */

@@ -129,8 +129,15 @@ SIGNATURES = {
     "psd_engine_timing_ms": (C.c_int, [_vp, C.POINTER(C.c_float), C.POINTER(C.c_float),
                                         C.POINTER(C.c_uint64)]),
     "psd_engine_edge_kernel_size": (C.c_int, [_vp]),
+    "psd_engine_add_edge_kernel_size": (C.c_int, [_vp, _i32, C.POINTER(_i32)]),
+    "psd_engine_add_hash_geometry": (C.c_int, [_vp, _i32, _i32, C.POINTER(_i32)]),
+    "psd_engine_edge_kernel_size_at": (C.c_int, [_vp, _i32]),
+    "psd_engine_device_edge_sads": (C.c_int, [_vp, _i32, C.POINTER(_vp)]),
+    "psd_engine_device_hash_at": (C.c_int, [_vp, _i32, C.POINTER(_vp)]),
+    "psd_engine_read_hash_at": (C.c_int, [_vp, _i32, _i64, _i64, _vp]),
     "psd_engine_debug_plane": (C.c_int, [_vp, C.c_int, _i64, _vp, C.c_size_t]),
     "psd_scan_content": (C.c_int, [_vp, _i64, _i64, _dp, _dbl, _vp, _vp, _vp]),
+    "psd_scan_content_edges": (C.c_int, [_vp, _vp, _i64, _i64, _dp, _dbl, _vp, _vp, _vp]),
     "psd_scan_adaptive": (C.c_int, [_vp, _i64, _i32, _dbl, _vp, _vp]),
     "psd_scan_average": (C.c_int, [_vp, _i64, _i64, _vp, _vp]),
     "psd_scan_hist_correl": (C.c_int, [_vp, _i64, _i32, _vp, _vp, _vp]),
@@ -149,6 +156,8 @@ SIGNATURES = {
     "psd_engine_scan_average_host": (C.c_int, [_vp, _i64, _i64, _vp]),
     "psd_engine_scan_hist_correl_host": (C.c_int, [_vp, _i64, _i64, _i32, _vp]),
     "psd_engine_scan_hash_dist_host": (C.c_int, [_vp, _i64, _i64, _vp]),
+    "psd_engine_scan_content_host_at": (C.c_int, [_vp, _i32, _i64, _i64, _dp, _dbl, _vp, _vp]),
+    "psd_engine_scan_hash_dist_host_at": (C.c_int, [_vp, _i32, _i64, _i64, _vp]),
     "psd_synth_frames": (C.c_int, [C.c_int, _vp, _vp, _i64, _i32, _i32, _i64, _vp]),
     "psd_test_hsv": (C.c_int, [C.c_int, _vp, _i64, _vp, _vp, _vp, _vp]),
 }

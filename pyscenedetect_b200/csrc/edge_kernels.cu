@@ -604,10 +604,11 @@ static void launch_dilate(const uint32_t* in, uint32_t* out, int n, int H, int W
         in, out, H, Wq, tiles_x, tile_words, bands, n_threads, mask);
 }
 
+// frame f's SAD is added to sad[f * sad_stride] (psd_frame_sums::sad_edges of slot 0, or an edge slot's own array)
 __global__ void __launch_bounds__(256) psd_edge_sad_bits_kernel(const uint32_t* __restrict__ dil,
                                                                 const uint32_t* __restrict__ carry,
                                                                 int64_t per_frame, int have_prev,
-                                                                psd_frame_sums* __restrict__ sums) {
+                                                                uint64_t* __restrict__ sad, int64_t sad_stride) {
     const int64_t f = blockIdx.y;
     if (f == 0 && !have_prev) return;
     const uint32_t* cur = dil + f * per_frame;
@@ -623,7 +624,7 @@ __global__ void __launch_bounds__(256) psd_edge_sad_bits_kernel(const uint32_t* 
     if (threadIdx.x == 0) {
         uint32_t t = 0;
         for (int w = 0; w < 8; ++w) t += part[w];
-        if (t) atomicAdd(reinterpret_cast<unsigned long long*>(&sums[f].sad_edges), 255ull * t);
+        if (t) atomicAdd(reinterpret_cast<unsigned long long*>(sad + f * sad_stride), 255ull * t);
     }
 }
 
@@ -650,8 +651,8 @@ int edge_unpack(const uint32_t* bits, uint8_t* out, int W, int H, bool tile_majo
     return PSD_OK;
 }
 
-int launch_edges(const EdgeBuffers& b, int n, int W, int H, int ksize, bool have_prev,
-                 psd_frame_sums* sums, cudaStream_t stream) {
+int launch_edges(const EdgeBuffers& b, int n, int W, int H, const EdgeSlot* slots, int n_slots, bool have_prev,
+                 cudaStream_t stream) {
     PSD_REQUIRE(n > 0 && n <= 65535, "edge batch out of range");
     const int64_t P = (int64_t)W * H;
     const int Wq = (W + 31) / 32;
@@ -701,30 +702,34 @@ int launch_edges(const EdgeBuffers& b, int n, int W, int H, int ksize, bool have
         PSD_CUDA(cudaLaunchCooperativeKernel((const void*)psd_hyst_bits_kernel, dim3(grid), dim3(256), args, 0, stream));
     }
     count_launch(3);
-    const int r = ksize / 2;
+    // one dilation + SAD per kernel size, in stream order through the one bits_dil plane
     const uint32_t last_mask = (W & 31) ? ((1u << (W & 31)) - 1u) : 0xFFFFFFFFu;
-    if (edge_dilate_separable(ksize)) {   // k >= 19
-        const int rc = launch_dilate_separable(b.bits_in, b.bits_hdil, b.bits_dil, n, W, H, ksize, last_mask, stream);
-        if (rc) return rc;
-        count_launch(1);   // the second pass
-    } else switch (r) {
-        case 1: launch_dilate<1>(b.bits_in, b.bits_dil, n, H, Wq, last_mask, stream); break;
-        case 2: launch_dilate<2>(b.bits_in, b.bits_dil, n, H, Wq, last_mask, stream); break;
-        case 3: launch_dilate<3>(b.bits_in, b.bits_dil, n, H, Wq, last_mask, stream); break;
-        case 4: launch_dilate<4>(b.bits_in, b.bits_dil, n, H, Wq, last_mask, stream); break;
-        case 5: launch_dilate<5>(b.bits_in, b.bits_dil, n, H, Wq, last_mask, stream); break;
-        case 6: launch_dilate<6>(b.bits_in, b.bits_dil, n, H, Wq, last_mask, stream); break;
-        case 7: launch_dilate<7>(b.bits_in, b.bits_dil, n, H, Wq, last_mask, stream); break;
-        case 8: launch_dilate<8>(b.bits_in, b.bits_dil, n, H, Wq, last_mask, stream); break;
-        default: PSD_REQUIRE(false, "edge kernel size %d has no dilation kernel", ksize);
+    for (int s = 0; s < n_slots; ++s) {
+        const int ksize = slots[s].ksize, r = ksize / 2;
+        if (edge_dilate_separable(ksize)) {   // k >= 19
+            const int rc = launch_dilate_separable(b.bits_in, b.bits_hdil, b.bits_dil, n, W, H, ksize, last_mask, stream);
+            if (rc) return rc;
+            count_launch(1);   // the second pass
+        } else switch (r) {
+            case 1: launch_dilate<1>(b.bits_in, b.bits_dil, n, H, Wq, last_mask, stream); break;
+            case 2: launch_dilate<2>(b.bits_in, b.bits_dil, n, H, Wq, last_mask, stream); break;
+            case 3: launch_dilate<3>(b.bits_in, b.bits_dil, n, H, Wq, last_mask, stream); break;
+            case 4: launch_dilate<4>(b.bits_in, b.bits_dil, n, H, Wq, last_mask, stream); break;
+            case 5: launch_dilate<5>(b.bits_in, b.bits_dil, n, H, Wq, last_mask, stream); break;
+            case 6: launch_dilate<6>(b.bits_in, b.bits_dil, n, H, Wq, last_mask, stream); break;
+            case 7: launch_dilate<7>(b.bits_in, b.bits_dil, n, H, Wq, last_mask, stream); break;
+            case 8: launch_dilate<8>(b.bits_in, b.bits_dil, n, H, Wq, last_mask, stream); break;
+            default: PSD_REQUIRE(false, "edge kernel size %d has no dilation kernel", ksize);
+        }
+        PSD_CHECK_LAUNCH();
+        dim3 sg((unsigned)min((int64_t)64, (per_frame + 255) / 256), (unsigned)n);
+        psd_edge_sad_bits_kernel<<<sg, 256, 0, stream>>>(b.bits_dil, slots[s].carry_bits, per_frame, have_prev ? 1 : 0,
+                                                         slots[s].sad, slots[s].sad_stride);
+        PSD_CHECK_LAUNCH();
+        count_launch(2);
+        PSD_CUDA(cudaMemcpyAsync(slots[s].carry_bits, b.bits_dil + (int64_t)(n - 1) * per_frame,
+                                 (size_t)per_frame * 4, cudaMemcpyDeviceToDevice, stream));
     }
-    PSD_CHECK_LAUNCH();
-    dim3 sg((unsigned)min((int64_t)64, (per_frame + 255) / 256), (unsigned)n);
-    psd_edge_sad_bits_kernel<<<sg, 256, 0, stream>>>(b.bits_dil, b.carry_bits, per_frame, have_prev ? 1 : 0, sums);
-    PSD_CHECK_LAUNCH();
-    count_launch(2);
-    PSD_CUDA(cudaMemcpyAsync(b.carry_bits, b.bits_dil + (int64_t)(n - 1) * per_frame,
-                             (size_t)per_frame * 4, cudaMemcpyDeviceToDevice, stream));
     return PSD_OK;
 }
 

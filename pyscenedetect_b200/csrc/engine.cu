@@ -6,6 +6,7 @@
 #include <stdarg.h>
 #include <string.h>
 
+#include <algorithm>
 #include <vector>
 
 #include "psd_common.cuh"
@@ -71,13 +72,21 @@ struct psd_engine {
     // results: slot 0 = halo frame, stream frame i at slot i+1
     psd_frame_sums* d_sums = nullptr;
     uint32_t* d_yhist = nullptr;
-    uint64_t* d_hash = nullptr;   // [capacity][hash.words]
-    HashPlan hash{};
+    // hash slots: slot 0 is the configured geometry, psd_engine_add_hash_geometry appends
+    std::vector<HashPlan> hash;
+    std::vector<uint64_t*> d_hash;   // per slot [capacity][hash[slot].words]
     int64_t capacity = 0;
     int64_t n_frames = 0;
     bool halo_scored = false;
-    // edge path
+    // edge path: Canny scratch shared by every edge slot; slot 0 is the configured kernel size (its SADs are
+    // psd_frame_sums::sad_edges), psd_engine_add_edge_kernel_size appends
     EdgeBuffers eb{};
+    struct EdgeSlotState {
+        int ksize;
+        uint32_t* carry_bits;   // [H][Wq] dilated edges of the predecessor frame
+        uint64_t* sad;          // [capacity], slot numbering of d_sums (nullptr for slot 0)
+    };
+    std::vector<EdgeSlotState> edge;
     // last batch bookkeeping for debug taps
     const uint8_t* last_scored = nullptr;
     int64_t last_scored_stride = 0;
@@ -87,6 +96,22 @@ struct psd_engine {
     std::vector<std::pair<cudaEvent_t, cudaEvent_t>> ev_score, ev_total;
     size_t ev_next = 0;
 };
+
+// a zeroed [cap][words] uint64 array holding the first n_frames + 1 result slots of *p ([old_cap][words], or none)
+static int grow_array(psd_engine* e, uint64_t** p, int64_t old_cap, int64_t cap, int words) {
+    uint64_t* np = nullptr;
+    PSD_CUDA(cudaMalloc(&np, (size_t)cap * words * sizeof(uint64_t)));
+    PSD_CUDA(cudaMemsetAsync(np, 0, (size_t)cap * words * sizeof(uint64_t), e->compute_stream));
+    if (*p) {
+        const int64_t keep = std::min(old_cap, e->n_frames + 1);
+        PSD_CUDA(cudaMemcpyAsync(np, *p, (size_t)keep * words * sizeof(uint64_t), cudaMemcpyDeviceToDevice,
+                                 e->compute_stream));
+        PSD_CUDA(cudaStreamSynchronize(e->compute_stream));
+        cudaFree(*p);
+    }
+    *p = np;
+    return PSD_OK;
+}
 
 static int ensure_capacity(psd_engine* e, int64_t need_slots) {
     if (need_slots <= e->capacity) return PSD_OK;
@@ -114,17 +139,13 @@ static int ensure_capacity(psd_engine* e, int64_t need_slots) {
         }
         e->d_yhist = nh;
     }
-    if (e->features & PSD_F_HASH) {
-        uint64_t* nh = nullptr;
-        PSD_CUDA(cudaMalloc(&nh, (size_t)cap * e->hash.words * sizeof(uint64_t)));
-        PSD_CUDA(cudaMemsetAsync(nh, 0, (size_t)cap * e->hash.words * sizeof(uint64_t), e->compute_stream));
-        if (e->d_hash) {
-            PSD_CUDA(cudaMemcpyAsync(nh, e->d_hash, (size_t)(e->n_frames + 1) * e->hash.words * sizeof(uint64_t),
-                                     cudaMemcpyDeviceToDevice, e->compute_stream));
-            PSD_CUDA(cudaStreamSynchronize(e->compute_stream));
-            cudaFree(e->d_hash);
-        }
-        e->d_hash = nh;
+    for (size_t s = 0; s < e->hash.size(); ++s) {
+        int rc = grow_array(e, &e->d_hash[s], e->capacity, cap, e->hash[s].words);
+        if (rc) return rc;
+    }
+    for (size_t s = 1; s < e->edge.size(); ++s) {
+        int rc = grow_array(e, &e->edge[s].sad, e->capacity, cap, 1);
+        if (rc) return rc;
     }
     e->capacity = cap;
     return PSD_OK;
@@ -166,8 +187,11 @@ static int run_batch(psd_engine* e, const uint8_t* src, int64_t src_frame_stride
     PSD_CUDA(cudaMemsetAsync(e->d_sums + slot0, 0, (size_t)n * sizeof(psd_frame_sums), st));
     if (e->features & PSD_F_YHIST)
         PSD_CUDA(cudaMemsetAsync(e->d_yhist + slot0 * 256, 0, (size_t)n * 256 * sizeof(uint32_t), st));
-    if (e->features & PSD_F_EDGES)
+    if (e->features & PSD_F_EDGES) {
         PSD_CUDA(cudaMemsetAsync(e->eb.vhist, 0, (size_t)n * 256 * sizeof(uint32_t), st));
+        for (size_t s = 1; s < e->edge.size(); ++s)
+            PSD_CUDA(cudaMemsetAsync(e->edge[s].sad + slot0, 0, (size_t)n * sizeof(uint64_t), st));
+    }
     ScoreArgs a{};
     a.frames = scored;
     a.prev = (e->have_carry && !is_halo) ? e->carry : nullptr;
@@ -185,13 +209,22 @@ static int run_batch(psd_engine* e, const uint8_t* src, int64_t src_frame_stride
         if (rc) return rc;
     }
     if (e->features & PSD_F_HASH) {
-        rc = launch_hash(e->hash, scored, scored_stride, (int)n, e->W, e->H, e->d_hash + slot0 * e->hash.words, st);
+        std::vector<uint64_t*> outs(e->hash.size());
+        for (size_t s = 0; s < e->hash.size(); ++s) outs[s] = e->d_hash[s] + slot0 * e->hash[s].words;
+        rc = launch_hash(e->hash.data(), (int)e->hash.size(), scored, scored_stride, (int)n, e->W, e->H, outs.data(), st);
         if (rc) return rc;
     }
     PSD_CUDA(cudaEventRecord(k1, st));
     e->ev_score.push_back({k0, k1});
     if (e->features & PSD_F_EDGES) {
-        rc = launch_edges(e->eb, (int)n, e->W, e->H, e->ksize, a.prev != nullptr, e->d_sums + slot0, st);
+        std::vector<EdgeSlot> slots(e->edge.size());
+        for (size_t s = 0; s < e->edge.size(); ++s) {
+            const bool own = s > 0;   // slot 0 accumulates into psd_frame_sums::sad_edges
+            slots[s] = EdgeSlot{e->edge[s].ksize, e->edge[s].carry_bits,
+                                own ? e->edge[s].sad + slot0 : &e->d_sums[slot0].sad_edges,
+                                own ? 1 : (int64_t)(sizeof(psd_frame_sums) / sizeof(uint64_t))};
+        }
+        rc = launch_edges(e->eb, (int)n, e->W, e->H, slots.data(), (int)slots.size(), a.prev != nullptr, st);
         if (rc) return rc;
     }
     // carry the last frame (scored size) for the next batch
@@ -280,15 +313,26 @@ void psd_engine_destroy(psd_engine* e) {
         if (e->h2d_done[s]) cudaEventDestroy(e->h2d_done[s]);
     }
     cudaFree(e->small); cudaFree(e->d_xofs); cudaFree(e->d_xa); cudaFree(e->d_yofs); cudaFree(e->d_ya);
-    cudaFree(e->carry); cudaFree(e->d_sums); cudaFree(e->d_yhist); cudaFree(e->d_hash);
-    hash_plan_destroy(&e->hash);
+    cudaFree(e->carry); cudaFree(e->d_sums); cudaFree(e->d_yhist);
+    for (uint64_t* p : e->d_hash) cudaFree(p);
+    for (HashPlan& p : e->hash) hash_plan_destroy(&p);
+    for (auto& s : e->edge) { cudaFree(s.carry_bits); cudaFree(s.sad); }
     cudaFree(e->eb.vplane); cudaFree(e->eb.vhist); cudaFree(e->eb.thresholds); cudaFree(e->eb.cand);
     cudaFree(e->eb.tmp); cudaFree(e->eb.bits_in); cudaFree(e->eb.bits_dil); cudaFree(e->eb.bits_hdil);
-    cudaFree(e->eb.carry_bits); cudaFree(e->eb.dirty); cudaFree(e->eb.hyst_flags);
+    cudaFree(e->eb.dirty); cudaFree(e->eb.hyst_flags);
     for (cudaEvent_t ev : e->ev_pool) cudaEventDestroy(ev);
     if (e->copy_stream) cudaStreamDestroy(e->copy_stream);
     if (e->compute_stream) cudaStreamDestroy(e->compute_stream);
     delete e;
+}
+
+// the dilation kernel size of a ContentDetector(kernel_size=k) at the engine's scored size (k = 0: automatic)
+static int effective_ksize(const psd_engine* e, int k) {
+    if (k == 0) {  // content_detector.py:39-46; Python round() is half-to-even like nearbyint
+        k = 4 + (int)nearbyint(sqrt((double)e->W * (double)e->H) / 192.0);
+        if ((k & 1) == 0) k += 1;
+    }
+    return k;
 }
 
 #define ENG_CUDA(expr)                                                                          \
@@ -341,19 +385,18 @@ int psd_engine_create(const psd_config* cfg, psd_engine** out) {
     e->features = cfg->features | ((cfg->features & PSD_F_EDGES) ? PSD_F_HSV : 0);
     e->max_batch = cfg->max_batch;
     if (e->features & PSD_F_EDGES) {
-        int k = cfg->edge_kernel_size;
-        if (k == 0) {  // content_detector.py:39-46; Python round() is half-to-even like nearbyint
-            k = 4 + (int)nearbyint(sqrt((double)e->W * (double)e->H) / 192.0);
-            if ((k & 1) == 0) k += 1;
-        }
+        const int k = effective_ksize(e, cfg->edge_kernel_size);
         if (edge_dilate_check(e->W, k) != PSD_OK) {
             psd_engine_destroy(e);
             return PSD_ERR_INVALID;
         }
         e->ksize = k;
+        e->edge.push_back({k, nullptr, nullptr});
     }
     if (e->features & PSD_F_HASH) {
-        int rc = hash_plan_create(&e->hash, e->W, e->H, cfg->hash_size ? cfg->hash_size : 8,
+        e->hash.emplace_back();
+        e->d_hash.push_back(nullptr);
+        int rc = hash_plan_create(&e->hash[0], e->W, e->H, cfg->hash_size ? cfg->hash_size : 8,
                                   cfg->hash_lowpass ? cfg->hash_lowpass : 2, e->max_batch);
         if (rc) { psd_engine_destroy(e); return rc; }
     }
@@ -393,7 +436,7 @@ int psd_engine_create(const psd_config* cfg, psd_engine** out) {
         ENG_CUDA(cudaMalloc(&e->eb.tmp, (size_t)e->P));
         ENG_CUDA(cudaMalloc(&e->eb.bits_dil, words * 4 * e->max_batch));
         if (edge_dilate_separable(e->ksize)) ENG_CUDA(cudaMalloc(&e->eb.bits_hdil, words * 4 * e->max_batch));
-        ENG_CUDA(cudaMalloc(&e->eb.carry_bits, words * 4));
+        ENG_CUDA(cudaMalloc(&e->edge[0].carry_bits, words * 4));
         ENG_CUDA(cudaMalloc(&e->eb.vhist, (size_t)e->max_batch * 256 * 4));
         ENG_CUDA(cudaMalloc(&e->eb.thresholds, (size_t)e->max_batch * 2 * 4));
         ENG_CUDA(cudaMalloc(&e->eb.hyst_flags, 64));
@@ -585,19 +628,99 @@ int psd_engine_read_yhist(psd_engine* e, int64_t first, int64_t n, uint32_t* out
     return PSD_OK;
 }
 
-int psd_engine_read_hash(psd_engine* e, int64_t first, int64_t n, uint64_t* out) {
+int psd_engine_read_hash_at(psd_engine* e, int32_t slot, int64_t first, int64_t n, uint64_t* out) {
     PSD_REQUIRE(e && out, "psd_engine_read_hash: null argument");
     PSD_REQUIRE(e->features & PSD_F_HASH, "engine was created without PSD_F_HASH");
+    PSD_REQUIRE(slot >= 0 && slot < (int32_t)e->hash.size(), "hash slot %d out of range (%d)", slot, (int)e->hash.size());
     PSD_REQUIRE(first >= -1 && n >= 0 && first + n <= e->n_frames, "frame range out of bounds");
     int rc = psd_engine_sync(e);
     if (rc) return rc;
-    if (n) PSD_CUDA(cudaMemcpy(out, e->d_hash + (first + 1) * e->hash.words, (size_t)n * e->hash.words * 8, cudaMemcpyDeviceToHost));
+    const int words = e->hash[slot].words;
+    if (n) PSD_CUDA(cudaMemcpy(out, e->d_hash[slot] + (first + 1) * words, (size_t)n * words * 8, cudaMemcpyDeviceToHost));
     return PSD_OK;
 }
 
-int psd_engine_device_hash(psd_engine* e, const uint64_t** hashes) {
+int psd_engine_read_hash(psd_engine* e, int64_t first, int64_t n, uint64_t* out) {
+    return psd_engine_read_hash_at(e, 0, first, n, out);
+}
+
+int psd_engine_device_hash_at(psd_engine* e, int32_t slot, const uint64_t** hashes) {
     PSD_REQUIRE(e && hashes, "psd_engine_device_hash: null argument");
-    *hashes = e->d_hash ? e->d_hash + e->hash.words : nullptr;
+    if (e->hash.empty() && slot == 0) { *hashes = nullptr; return PSD_OK; }
+    PSD_REQUIRE(slot >= 0 && slot < (int32_t)e->hash.size(), "hash slot %d out of range (%d)", slot, (int)e->hash.size());
+    *hashes = e->d_hash[slot] + e->hash[slot].words;
+    return PSD_OK;
+}
+
+int psd_engine_device_hash(psd_engine* e, const uint64_t** hashes) { return psd_engine_device_hash_at(e, 0, hashes); }
+
+int psd_engine_device_edge_sads(psd_engine* e, int32_t slot, const uint64_t** sad_edges) {
+    PSD_REQUIRE(e && sad_edges, "psd_engine_device_edge_sads: null argument");
+    PSD_REQUIRE(slot == 0 || (slot > 0 && slot < (int32_t)e->edge.size()), "edge slot %d out of range (%d)", slot,
+                (int)e->edge.size());
+    *sad_edges = slot == 0 ? nullptr : e->edge[slot].sad + 1;
+    return PSD_OK;
+}
+
+int psd_engine_edge_kernel_size_at(const psd_engine* e, int32_t slot) {
+    if (!e || slot < 0 || slot >= (int32_t)e->edge.size()) return -1;
+    return e->edge[slot].ksize;
+}
+
+// slots can be added while the engine holds nothing that was scored with fewer slots
+static int require_empty(psd_engine* e, const char* what) {
+    if (e->n_frames != 0 || e->halo_scored || e->have_carry) {
+        set_error("%s: the engine already holds frames (add slots after create or reset, before any submit or halo)",
+                  what);
+        return PSD_ERR_STATE;
+    }
+    return PSD_OK;
+}
+
+int psd_engine_add_edge_kernel_size(psd_engine* e, int32_t kernel_size, int32_t* slot) {
+    PSD_REQUIRE(e && slot, "psd_engine_add_edge_kernel_size: null argument");
+    PSD_REQUIRE(e->features & PSD_F_EDGES, "engine was created without PSD_F_EDGES");
+    PSD_REQUIRE(kernel_size == 0 || (kernel_size >= 3 && (kernel_size & 1)), "kernel_size must be odd integer >= 3");
+    int rc = require_empty(e, "psd_engine_add_edge_kernel_size");
+    if (rc) return rc;
+    const int k = effective_ksize(e, kernel_size);
+    for (size_t s = 0; s < e->edge.size(); ++s)
+        if (e->edge[s].ksize == k) { *slot = (int32_t)s; return PSD_OK; }
+    rc = edge_dilate_check(e->W, k);
+    if (rc) return rc;
+    PSD_CUDA(cudaSetDevice(e->device));
+    const size_t words = (size_t)e->H * ((e->W + 31) / 32);
+    if (edge_dilate_separable(k) && !e->eb.bits_hdil)
+        PSD_CUDA(cudaMalloc(&e->eb.bits_hdil, words * 4 * e->max_batch));
+    e->edge.push_back({k, nullptr, nullptr});
+    auto& st = e->edge.back();
+    PSD_CUDA(cudaMalloc(&st.carry_bits, words * 4));
+    rc = grow_array(e, &st.sad, 0, e->capacity, 1);
+    if (rc) return rc;
+    *slot = (int32_t)(e->edge.size() - 1);
+    return PSD_OK;
+}
+
+int psd_engine_add_hash_geometry(psd_engine* e, int32_t size, int32_t lowpass, int32_t* slot) {
+    PSD_REQUIRE(e && slot, "psd_engine_add_hash_geometry: null argument");
+    PSD_REQUIRE(e->features & PSD_F_HASH, "engine was created without PSD_F_HASH");
+    PSD_REQUIRE(size >= 0 && lowpass >= 0, "HashDetector needs size >= 1 and lowpass >= 1");
+    int rc = require_empty(e, "psd_engine_add_hash_geometry");
+    if (rc) return rc;
+    size = size ? size : 8;
+    lowpass = lowpass ? lowpass : 2;
+    for (size_t s = 0; s < e->hash.size(); ++s)
+        if (e->hash[s].size == size && e->hash[s].n == (int64_t)size * lowpass) { *slot = (int32_t)s; return PSD_OK; }
+    PSD_CUDA(cudaSetDevice(e->device));
+    HashPlan p{};
+    rc = hash_plan_create(&p, e->W, e->H, size, lowpass, e->max_batch);
+    if (rc) { hash_plan_destroy(&p); return rc; }
+    uint64_t* d = nullptr;
+    rc = grow_array(e, &d, 0, e->capacity, p.words);
+    if (rc) { hash_plan_destroy(&p); return rc; }
+    e->hash.push_back(p);
+    e->d_hash.push_back(d);
+    *slot = (int32_t)(e->hash.size() - 1);
     return PSD_OK;
 }
 
@@ -663,19 +786,29 @@ static int scan_to_host(psd_engine* e, double* d_tmp, double* out, size_t count)
     return PSD_OK;
 }
 
-int psd_engine_scan_content_host(psd_engine* e, int64_t first, int64_t n, const double weights[4],
-                                 double weight_abs_sum, double* out_components, double* out_content_val) {
+int psd_engine_scan_content_host_at(psd_engine* e, int32_t edge_slot, int64_t first, int64_t n,
+                                    const double weights[4], double weight_abs_sum, double* out_components,
+                                    double* out_content_val) {
     PSD_REQUIRE(e && weights && out_content_val, "psd_engine_scan_content_host: null argument");
     PSD_REQUIRE(first >= 0 && n >= 0 && first + n <= e->n_frames, "frame range out of bounds");
+    PSD_REQUIRE(edge_slot == 0 || (edge_slot > 0 && edge_slot < (int32_t)e->edge.size()),
+                "edge slot %d out of range (%d)", edge_slot, (int)e->edge.size());
     if (n == 0) return PSD_OK;
     PSD_CUDA(cudaSetDevice(e->device));
     double* tmp = nullptr;
     PSD_CUDA(cudaMalloc(&tmp, (size_t)n * 5 * sizeof(double)));
-    int rc = psd_scan_content(e->d_sums + 1 + first, n, e->P, weights, weight_abs_sum, tmp + n, tmp, e->compute_stream);
+    const uint64_t* sad_edges = edge_slot ? e->edge[edge_slot].sad + 1 + first : nullptr;
+    int rc = psd_scan_content_edges(e->d_sums + 1 + first, sad_edges, n, e->P, weights, weight_abs_sum, tmp + n, tmp,
+                                    e->compute_stream);
     if (!rc) rc = scan_to_host(e, tmp, out_content_val, (size_t)n);
     if (!rc && out_components) rc = scan_to_host(e, tmp + n, out_components, (size_t)n * 4);
     cudaFree(tmp);
     return rc;
+}
+
+int psd_engine_scan_content_host(psd_engine* e, int64_t first, int64_t n, const double weights[4],
+                                 double weight_abs_sum, double* out_components, double* out_content_val) {
+    return psd_engine_scan_content_host_at(e, 0, first, n, weights, weight_abs_sum, out_components, out_content_val);
 }
 
 int psd_engine_scan_adaptive_host(psd_engine* e, const double* scores_host, int64_t n, int32_t window_width,
@@ -730,20 +863,28 @@ int psd_scan_hash_dist(const uint64_t* hashes, int64_t n, int32_t hash_size, con
     return launch_hash_dist(hashes, n, hash_size, prev_hash, out, (cudaStream_t)stream);
 }
 
-int psd_engine_scan_hash_dist_host(psd_engine* e, int64_t first, int64_t n, double* out) {
+int psd_engine_scan_hash_dist_host_at(psd_engine* e, int32_t hash_slot, int64_t first, int64_t n, double* out) {
     PSD_REQUIRE(e && out, "psd_engine_scan_hash_dist_host: null argument");
     PSD_REQUIRE(e->features & PSD_F_HASH, "engine was created without PSD_F_HASH");
+    PSD_REQUIRE(hash_slot >= 0 && hash_slot < (int32_t)e->hash.size(), "hash slot %d out of range (%d)", hash_slot,
+                (int)e->hash.size());
     PSD_REQUIRE(first >= 0 && n >= 0 && first + n <= e->n_frames, "frame range out of bounds");
     if (n == 0) return PSD_OK;
     PSD_CUDA(cudaSetDevice(e->device));
     double* tmp = nullptr;
     PSD_CUDA(cudaMalloc(&tmp, (size_t)n * sizeof(double)));
+    const HashPlan& p = e->hash[hash_slot];
+    const uint64_t* h = e->d_hash[hash_slot];
     // slot `first` (= stream frame first-1, or the halo slot) precedes slot first+1
-    const uint64_t* prev = (first > 0 || e->halo_scored) ? e->d_hash + first * e->hash.words : nullptr;
-    int rc = psd_scan_hash_dist(e->d_hash + (first + 1) * e->hash.words, n, e->hash.size, prev, tmp, e->compute_stream);
+    const uint64_t* prev = (first > 0 || e->halo_scored) ? h + first * p.words : nullptr;
+    int rc = psd_scan_hash_dist(h + (first + 1) * p.words, n, p.size, prev, tmp, e->compute_stream);
     if (!rc) rc = scan_to_host(e, tmp, out, (size_t)n);
     cudaFree(tmp);
     return rc;
+}
+
+int psd_engine_scan_hash_dist_host(psd_engine* e, int64_t first, int64_t n, double* out) {
+    return psd_engine_scan_hash_dist_host_at(e, 0, first, n, out);
 }
 
 int psd_synth_frames(int device, void* d_out, const int32_t* params_host, int64_t n, int32_t width,

@@ -36,17 +36,31 @@ __device__ __forceinline__ float byte_to_float(uint32_t g) { return __fadd_rn(__
 //      1920-wide frame would otherwise sit in the same banks);
 //   2. thread (row, destination column) walks its taps in shared memory: the integer block sum if both scale
 //      factors are integers, else OpenCV's float32 `buf += S * alpha` in source order (separate multiply and
-//      add: the order and the roundings decide the last bit, so this chain stays sequential).  For n <= 256
-//      every thread has at most one (row, column); for n > 256 the CTA owns one row and loops over columns.
+//      add: the order and the roundings decide the last bit, so this chain stays sequential).  For one geometry
+//      with n <= 256 every thread has at most one (row, column); for n > 256 the CTA owns one row and loops over
+//      columns.  With several geometries the block height follows the smallest n and threads loop as needed.
 // (The first version had one thread per (row, column) read its 3 x 120 bytes straight from global memory, 32
 // lanes 360 bytes apart: 0.085 of the HBM roofline.)
+// One launch serves up to kHashRowsMaxGeo hash geometries (an engine's hash slots): step 1 runs once, step 2 once
+// per geometry, each with its own taps and row buffer.  A geometry's row buffer does not depend on the block of rows
+// a CTA takes or on the other geometries, so it is bit-identical to what a one-geometry launch writes.
+constexpr int kHashRowsMaxGeo = 8;
+struct HashRowsGeo {
+    const int32_t* xstart;
+    const int32_t* xsi;
+    const float* xalpha;
+    const int32_t* xmid;
+    float* rowbuf;   // [frames][H][n]
+    int n, fast;
+};
+struct HashRowsArgs {
+    HashRowsGeo g[kHashRowsMaxGeo];
+    int count;
+};
+
 __global__ void __launch_bounds__(256) psd_hash_rows_kernel(const uint8_t* __restrict__ frames, int64_t frame_stride,
-                                                            int W, int H, int n, int rows_per_cta, int pitch, int fast,
-                                                            const int32_t* __restrict__ xstart,
-                                                            const int32_t* __restrict__ xsi,
-                                                            const float* __restrict__ xalpha,
-                                                            const int32_t* __restrict__ xmid,
-                                                            float* __restrict__ rowbuf) {
+                                                            int W, int H, int rows_per_cta, int pitch,
+                                                            const __grid_constant__ HashRowsArgs geo) {
     extern __shared__ __align__(16) uint8_t sgray[];   // [rows_per_cta][pitch]
     const int tid = threadIdx.x;
     const int64_t f = blockIdx.y;
@@ -80,30 +94,40 @@ __global__ void __launch_bounds__(256) psd_hash_rows_kernel(const uint8_t* __res
         }
     }
     __syncthreads();
-    // ---- 2. (row, destination column) pairs ----
-    for (int c = tid; c < rows * n; c += 256) {
-        const int r = c / n, dx = c - r * n;
-        const uint8_t* srow = sgray + r * pitch;
-        float* out = rowbuf + (f * H + sy0 + r) * (int64_t)n + dx;
-        if (fast) {  // integer scale: exact integer sum of the block's columns
-            const int sxw = W / n;
-            uint32_t s = 0;
-            for (int x = dx * sxw; x < (dx + 1) * sxw; ++x) s += srow[x];
-            *out = __uint_as_float(s);
-        } else {
-            // first (partial) tap, the run of whole pixels, last (partial) tap - in source order
-            float buf = 0.0f;
-            const int k0 = xstart[dx], k1 = xstart[dx + 1];
-            const int km = xmid[2 * dx], nm = xmid[2 * dx + 1];
-            for (int k = k0; k < km; ++k) buf = __fadd_rn(buf, __fmul_rn(byte_to_float(srow[xsi[k]]), xalpha[k]));
-            if (nm > 0) {
-                const uint8_t* sp = srow + xsi[km];
-                const float am = xalpha[km];
+    // ---- 2. (row, destination column) pairs of every geometry ----
+    for (int gi = 0; gi < geo.count; ++gi) {
+        const HashRowsGeo& g = geo.g[gi];
+        const int n = g.n;
+        const int32_t* __restrict__ xstart = g.xstart;
+        const int32_t* __restrict__ xsi = g.xsi;
+        const float* __restrict__ xalpha = g.xalpha;
+        const int32_t* __restrict__ xmid = g.xmid;
+        for (int c = tid; c < rows * n; c += 256) {
+            const int r = c / n, dx = c - r * n;
+            const uint8_t* srow = sgray + r * pitch;
+            float* out = g.rowbuf + (f * H + sy0 + r) * (int64_t)n + dx;
+            if (g.fast) {  // integer scale: exact integer sum of the block's columns
+                const int sxw = W / n;
+                uint32_t s = 0;
+                for (int x = dx * sxw; x < (dx + 1) * sxw; ++x) s += srow[x];
+                *out = __uint_as_float(s);
+            } else {
+                // first (partial) tap, the run of whole pixels, last (partial) tap - in source order
+                float buf = 0.0f;
+                const int k0 = __ldg(xstart + dx), k1 = __ldg(xstart + dx + 1);
+                const int km = __ldg(xmid + 2 * dx), nm = __ldg(xmid + 2 * dx + 1);
+                for (int k = k0; k < km; ++k)
+                    buf = __fadd_rn(buf, __fmul_rn(byte_to_float(srow[__ldg(xsi + k)]), __ldg(xalpha + k)));
+                if (nm > 0) {
+                    const uint8_t* sp = srow + __ldg(xsi + km);
+                    const float am = __ldg(xalpha + km);
 #pragma unroll 8
-                for (int i = 0; i < nm; ++i) buf = __fadd_rn(buf, __fmul_rn(byte_to_float(sp[i]), am));
+                    for (int i = 0; i < nm; ++i) buf = __fadd_rn(buf, __fmul_rn(byte_to_float(sp[i]), am));
+                }
+                for (int k = km + nm; k < k1; ++k)
+                    buf = __fadd_rn(buf, __fmul_rn(byte_to_float(srow[__ldg(xsi + k)]), __ldg(xalpha + k)));
+                *out = buf;
             }
-            for (int k = km + nm; k < k1; ++k) buf = __fadd_rn(buf, __fmul_rn(byte_to_float(srow[xsi[k]]), xalpha[k]));
-            *out = buf;
         }
     }
 }
@@ -406,38 +430,57 @@ void hash_plan_destroy(HashPlan* p) {
     *p = HashPlan{};
 }
 
-int launch_hash(const HashPlan& p, const uint8_t* frames, int64_t frame_stride, int n_frames, int W, int H,
-                uint64_t* hashes, cudaStream_t stream) {
-    // rows kernel: max(1, 256 / n) source rows per CTA, their gray bytes in shared memory
-    const int rows_per_cta = std::max(1, 256 / p.n);
-    const int pitch = ((W + 3) & ~3) + 4;
-    const size_t smem_rows = (size_t)rows_per_cta * pitch;
-    PSD_REQUIRE(smem_rows <= 200 * 1024, "frame too wide for the hash rows kernel (%d columns)", W);
-    PSD_CUDA(cudaFuncSetAttribute(psd_hash_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_rows));
+static int launch_hash_finish(const HashPlan& p, int nb, int H, uint64_t* out, cudaStream_t stream) {
     FoldPlan fp{};
     fp.levels = p.levels;
     for (int k = 0; k < 8; ++k) { fp.len[k] = p.len[k]; fp.off[k] = p.off[k]; }
     const size_t smem = p.global_ws ? 0 : (size_t)p.ws_doubles * sizeof(double);
-    if (!p.global_ws)
+    if (p.global_ws) {
+        psd_hash_finish_kernel<true><<<(unsigned)nb, 256, 0, stream>>>(
+            p.rowbuf, H, p.n, p.size, p.fast, p.area_w, p.area_h, p.ystart, p.ysi, p.ybeta, p.cosn, fp, p.ws,
+            p.ws_doubles, p.words, out);
+    } else {
         PSD_CUDA(cudaFuncSetAttribute(psd_hash_finish_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    for (int f0 = 0; f0 < n_frames; f0 += p.batch) {   // sub-batches share the row buffer and the workspace
-        const int nb = std::min(p.batch, n_frames - f0);
+        psd_hash_finish_kernel<false><<<(unsigned)nb, 256, smem, stream>>>(
+            p.rowbuf, H, p.n, p.size, p.fast, p.area_w, p.area_h, p.ystart, p.ysi, p.ybeta, p.cosn, fp, nullptr, 0,
+            p.words, out);
+    }
+    PSD_CHECK_LAUNCH();
+    count_launch();
+    return PSD_OK;
+}
+
+int launch_hash(const HashPlan* plans, int n_plans, const uint8_t* frames, int64_t frame_stride, int n_frames, int W,
+                int H, uint64_t* const* hashes, cudaStream_t stream) {
+    PSD_REQUIRE(n_plans >= 1, "launch_hash: no hash plan");
+    // rows kernel: max(1, 256 / n) source rows per CTA for the smallest hash image n, their gray bytes in shared
+    // memory; a sub-batch fits every plan's row buffer and workspace
+    int n_min = plans[0].n, batch = plans[0].batch;
+    for (int g = 1; g < n_plans; ++g) { n_min = std::min(n_min, plans[g].n); batch = std::min(batch, plans[g].batch); }
+    const int rows_per_cta = std::max(1, 256 / n_min);
+    const int pitch = ((W + 3) & ~3) + 4;
+    const size_t smem_rows = (size_t)rows_per_cta * pitch;
+    PSD_REQUIRE(smem_rows <= 200 * 1024, "frame too wide for the hash rows kernel (%d columns)", W);
+    PSD_CUDA(cudaFuncSetAttribute(psd_hash_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_rows));
+    for (int f0 = 0; f0 < n_frames; f0 += batch) {   // sub-batches share the row buffers and the workspaces
+        const int nb = std::min(batch, n_frames - f0);
         dim3 rgrid((unsigned)((H + rows_per_cta - 1) / rows_per_cta), (unsigned)nb);
-        psd_hash_rows_kernel<<<rgrid, 256, smem_rows, stream>>>(frames + f0 * frame_stride, frame_stride, W, H, p.n,
-                                                                rows_per_cta, pitch, p.fast, p.xstart, p.xsi, p.xalpha,
-                                                                p.xmid, p.rowbuf);
-        PSD_CHECK_LAUNCH();
-        uint64_t* out = hashes + (int64_t)f0 * p.words;
-        if (p.global_ws)
-            psd_hash_finish_kernel<true><<<(unsigned)nb, 256, 0, stream>>>(
-                p.rowbuf, H, p.n, p.size, p.fast, p.area_w, p.area_h, p.ystart, p.ysi, p.ybeta, p.cosn, fp, p.ws,
-                p.ws_doubles, p.words, out);
-        else
-            psd_hash_finish_kernel<false><<<(unsigned)nb, 256, smem, stream>>>(
-                p.rowbuf, H, p.n, p.size, p.fast, p.area_w, p.area_h, p.ystart, p.ysi, p.ybeta, p.cosn, fp, nullptr, 0,
-                p.words, out);
-        PSD_CHECK_LAUNCH();
-        count_launch(2);
+        for (int g0 = 0; g0 < n_plans; g0 += kHashRowsMaxGeo) {
+            HashRowsArgs geo{};
+            geo.count = std::min(kHashRowsMaxGeo, n_plans - g0);
+            for (int i = 0; i < geo.count; ++i) {
+                const HashPlan& p = plans[g0 + i];
+                geo.g[i] = HashRowsGeo{p.xstart, p.xsi, p.xalpha, p.xmid, p.rowbuf, p.n, p.fast};
+            }
+            psd_hash_rows_kernel<<<rgrid, 256, smem_rows, stream>>>(frames + f0 * frame_stride, frame_stride, W, H,
+                                                                    rows_per_cta, pitch, geo);
+            PSD_CHECK_LAUNCH();
+            count_launch();
+        }
+        for (int g = 0; g < n_plans; ++g) {
+            const int rc = launch_hash_finish(plans[g], nb, H, hashes[g] + (int64_t)f0 * plans[g].words, stream);
+            if (rc) return rc;
+        }
     }
     return PSD_OK;
 }

@@ -82,15 +82,21 @@ struct EdgeBuffers {
     uint32_t* cand;     // [n][edge_tile_words] Canny candidates (weak or strong pixels), 32 per word, TILE-MAJOR:
                         // tile (ty, tx) = 32 rows x 64 columns = 64 consecutive words, row r at words 2r, 2r+1
     uint32_t* bits_in;  // same layout: strong pixels after classify, the Canny map after hysteresis
-    uint32_t* bits_dil; // [n][H][Wq] dilated edges, row-major
-    uint32_t* bits_hdil;// [n][H][Wq] horizontal pass of the separable dilation (kernel sizes >= 19 only, else null)
-    uint32_t* carry_bits; // [H][Wq] dilated edges of the predecessor frame
+    uint32_t* bits_dil; // [n][H][Wq] dilated edges, row-major (of each edge slot in turn)
+    uint32_t* bits_hdil;// [n][H][Wq] horizontal pass of the separable dilation (if a kernel size >= 19 is in use, else null)
     uint8_t* tmp;       // [P] scratch for debug taps
     uint8_t* dirty;     // [2][n][tiles] hysteresis: tiles to revisit (double-buffered by round parity)
     int32_t* hyst_flags;// [3] hysteresis: "some tile changed" per round (rotating)
 };
-int launch_edges(const EdgeBuffers& b, int n, int width, int height, int ksize, bool have_prev,
-                 psd_frame_sums* sums, cudaStream_t stream);
+struct EdgeSlot {          // one dilation kernel size of an engine
+    int ksize;
+    uint32_t* carry_bits;  // [H][Wq] this size's dilated edges of the predecessor frame
+    uint64_t* sad;         // the batch's frame f accumulates into sad[f * sad_stride] (pre-zeroed)
+    int64_t sad_stride;    // uint64 words
+};
+// Canny (thresholds, classify, hysteresis) once, then a dilation and a SAD per slot
+int launch_edges(const EdgeBuffers& b, int n, int width, int height, const EdgeSlot* slots, int n_slots,
+                 bool have_prev, cudaStream_t stream);
 int edge_unpack(const uint32_t* bits, uint8_t* out, int W, int H, bool tile_major, cudaStream_t stream);
 int64_t edge_tile_words(int W, int H);   // words per frame of a tile-major bit plane
 bool edge_dilate_separable(int ksize);  // this kernel size dilates in two passes through EdgeBuffers::bits_hdil
@@ -115,8 +121,10 @@ struct HashPlan {        // per-engine tables for one (frame size, hash size, lo
 };
 int hash_plan_create(HashPlan* p, int W, int H, int size, int lowpass, int max_batch);
 void hash_plan_destroy(HashPlan* p);
-int launch_hash(const HashPlan& p, const uint8_t* frames, int64_t frame_stride, int n_frames, int W, int H,
-                uint64_t* hashes, cudaStream_t stream);
+// every plan's hashes of n_frames frames: hashes[g] receives plan g's ([n_frames][plans[g].words]); one gray
+// pass and one rows launch per sub-batch feed all the plans
+int launch_hash(const HashPlan* plans, int n_plans, const uint8_t* frames, int64_t frame_stride, int n_frames, int W,
+                int H, uint64_t* const* hashes, cudaStream_t stream);
 int launch_hash_dist(const uint64_t* hashes, int64_t n, int size, const uint64_t* prev_hash, double* out,
                      cudaStream_t stream);
 

@@ -11,7 +11,10 @@
 
 namespace psd {
 
-__global__ void psd_scan_content_kernel(const psd_frame_sums* __restrict__ sums, int64_t n,
+// sad_edges: the edge SAD of another dilation kernel size (an engine's edge slot), read in place of
+// sums[i].sad_edges; nullptr = the sums' own
+__global__ void psd_scan_content_kernel(const psd_frame_sums* __restrict__ sums,
+                                        const uint64_t* __restrict__ sad_edges, int64_t n,
                                         double n_pixels, double w0, double w1, double w2, double w3,
                                         double wsum, double* __restrict__ comps,
                                         double* __restrict__ score) {
@@ -25,7 +28,7 @@ __global__ void psd_scan_content_kernel(const psd_frame_sums* __restrict__ sums,
         c[0] = __ddiv_rn(__ull2double_rn(s.sad_hue), n_pixels);
         c[1] = __ddiv_rn(__ull2double_rn(s.sad_sat), n_pixels);
         c[2] = __ddiv_rn(__ull2double_rn(s.sad_lum), n_pixels);
-        c[3] = __ddiv_rn(__ull2double_rn(s.sad_edges), n_pixels);
+        c[3] = __ddiv_rn(__ull2double_rn(sad_edges ? sad_edges[i] : s.sad_edges), n_pixels);
         // sum(component * weight ...) : 0 + p0, + p1, + p2, + p3 (plain sequential fp64 adds)
         double acc = __dadd_rn(0.0, __dmul_rn(c[0], w0));
         acc = __dadd_rn(acc, __dmul_rn(c[1], w1));
@@ -156,17 +159,24 @@ __global__ void psd_scan_compare_kernel(const double* __restrict__ v, int64_t n,
 
 using namespace psd;
 
-extern "C" int psd_scan_content(const psd_frame_sums* sums, int64_t n, int64_t n_pixels,
-                                const double weights[4], double weight_abs_sum, double* out_components,
-                                double* out_content_val, void* stream) {
+extern "C" int psd_scan_content_edges(const psd_frame_sums* sums, const uint64_t* sad_edges, int64_t n,
+                                      int64_t n_pixels, const double weights[4], double weight_abs_sum,
+                                      double* out_components, double* out_content_val, void* stream) {
     PSD_REQUIRE(sums && out_content_val && weights && n >= 0 && n_pixels > 0, "psd_scan_content: bad args");
     if (n == 0) return PSD_OK;
     psd_scan_content_kernel<<<(unsigned)((n + 127) / 128), 128, 0, (cudaStream_t)stream>>>(
-        sums, n, (double)n_pixels, weights[0], weights[1], weights[2], weights[3], weight_abs_sum,
+        sums, sad_edges, n, (double)n_pixels, weights[0], weights[1], weights[2], weights[3], weight_abs_sum,
         out_components, out_content_val);
     PSD_CHECK_LAUNCH();
     count_launch();
     return PSD_OK;
+}
+
+extern "C" int psd_scan_content(const psd_frame_sums* sums, int64_t n, int64_t n_pixels,
+                                const double weights[4], double weight_abs_sum, double* out_components,
+                                double* out_content_val, void* stream) {
+    return psd_scan_content_edges(sums, nullptr, n, n_pixels, weights, weight_abs_sum, out_components,
+                                  out_content_val, stream);
 }
 
 extern "C" int psd_scan_adaptive(const double* scores, int64_t n, int32_t window_width,

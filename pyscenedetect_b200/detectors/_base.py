@@ -29,6 +29,8 @@ class EngineDetector(SceneDetector):
         self._max_batch = 16  # strict mode submits one frame per call; staging is sized by this
         self._scored_size: tuple[int, int] | None = None  # (width, height) detectors see
         self._base_index = 0  # engine frame index of this detector's first frame
+        self._edge_slot = 0   # the engine's slots of this detector's kernel size / hash geometry (attach_engine)
+        self._hash_slot = 0
 
     # -- configuration hooks used by SceneManager's batched fast path --
     def required_features(self) -> int:
@@ -48,9 +50,11 @@ class EngineDetector(SceneDetector):
         self._max_batch = max_batch
         self._scored_size = scored_size
 
-    def attach_engine(self, engine: Engine) -> None:
-        """Share one fused pass between several detectors (SceneManager does this)."""
-        self._engine = engine
+    def attach_engine(self, engine: Engine, edge_slot: int = 0, hash_slot: int = 0) -> None:
+        """Share one fused pass between several detectors (SceneManager does this).  `edge_slot` / `hash_slot`:
+        the engine's slot that holds this detector's dilation kernel size / hash geometry."""
+        self._edge_slot, self._hash_slot = int(edge_slot), int(hash_slot)
+        self._engine = engine.view(edge_slot, hash_slot) if (edge_slot or hash_slot) else engine
         self._owns_engine = False
         self._base_index = engine.frame_count
 
@@ -63,6 +67,7 @@ class EngineDetector(SceneDetector):
                                   edge_kernel_size=self.edge_kernel_size_arg(), **self.engine_kwargs())
             self._owns_engine = True
             self._base_index = 0
+            self._edge_slot = self._hash_slot = 0
         return self._engine
 
     @staticmethod

@@ -77,18 +77,23 @@ class DeviceCuts:
             raise RuntimeError(f"{count} cuts exceed the device cut buffer ({self._cap})")
         return self._cuts.download(count * 8).view(np.int64).tolist() if count else []
 
-    def _content_scores(self, weights, n):
+    def _content_scores(self, weights, n, edge_slot: int = 0):
         sums, _ = self._e.device_results()
         val, comps = self._tmp(n), self._tmp(4 * n)
         w = (C.c_double * 4)(*[float(x) for x in weights])
-        check(self._lib.psd_scan_content(sums, n, self._e.n_pixels, w, float(sum(abs(x) for x in weights)),
-                                         comps.ptr, val.ptr, self._stream), "psd_scan_content")
+        wsum = float(sum(abs(x) for x in weights))
+        if edge_slot:  # the edge SADs of another kernel size replace the sums' own
+            check(self._lib.psd_scan_content_edges(sums, self._e.device_edge_sads(edge_slot), n, self._e.n_pixels,
+                                                   w, wsum, comps.ptr, val.ptr, self._stream), "psd_scan_content_edges")
+        else:
+            check(self._lib.psd_scan_content(sums, n, self._e.n_pixels, w, wsum, comps.ptr, val.ptr, self._stream),
+                  "psd_scan_content")
         return val, comps
 
     def content(self, weights=(1.0, 1.0, 1.0, 0.0), threshold=27.0, min_scene_len=15, fps=30.0,
-                suppress: bool = False, first_frame: int = 0) -> list[int]:
+                suppress: bool = False, first_frame: int = 0, edge_slot: int = 0) -> list[int]:
         n = self._e.frame_count
-        val, _comps = self._content_scores(weights, n)
+        val, _comps = self._content_scores(weights, n, edge_slot)
         flags = DeviceBuffer(max(1, n), self._dev)
         check(self._lib.psd_scan_compare(val.ptr, n, float(threshold), 0, flags.ptr, self._stream))
         check(self._lib.psd_cuts_flash_filter(flags.ptr, n, first_frame, flash_filter_frames(min_scene_len, fps),
@@ -97,9 +102,9 @@ class DeviceCuts:
         return self._fetch()
 
     def adaptive(self, weights=(1.0, 1.0, 1.0, 0.0), adaptive_threshold=3.0, min_scene_len=15,
-                 window_width=2, min_content_val=15.0, fps=30.0, first_frame: int = 0) -> list[int]:
+                 window_width=2, min_content_val=15.0, fps=30.0, first_frame: int = 0, edge_slot: int = 0) -> list[int]:
         n = self._e.frame_count
-        val, _comps = self._content_scores(weights, n)
+        val, _comps = self._content_scores(weights, n, edge_slot)
         ratio = self._tmp(n)
         check(self._lib.psd_scan_adaptive(val.ptr, n, int(window_width), float(min_content_val), ratio.ptr,
                                           self._stream), "psd_scan_adaptive")
@@ -119,11 +124,11 @@ class DeviceCuts:
                                            self._cap, self._stream), "psd_cuts_histogram")
         return self._fetch()
 
-    def hash(self, threshold=0.35, min_scene_len=15, fps=30.0, first_frame: int = 0) -> list[int]:
+    def hash(self, threshold=0.35, min_scene_len=15, fps=30.0, first_frame: int = 0, hash_slot: int = 0) -> list[int]:
         n = self._e.frame_count
-        hashes = self._e.device_hash()
+        e = self._e.view(hash_slot=hash_slot) if hash_slot else self._e
         dist = self._tmp(n)
-        check(self._lib.psd_scan_hash_dist(hashes, n, int(self._e.hash_size), None, dist.ptr, self._stream))
+        check(self._lib.psd_scan_hash_dist(e.device_hash(), n, int(e.hash_size), None, dist.ptr, self._stream))
         check(self._lib.psd_cuts_hash(dist.ptr, n, first_frame, float(threshold), min_len_frames(min_scene_len, fps),
                                       self._cuts.ptr, self._count.ptr, self._cap, self._stream), "psd_cuts_hash")
         return self._fetch()
@@ -177,6 +182,11 @@ def automaton_args(detector) -> tuple[str, dict]:
 
 def cuts_for_detector(dc: DeviceCuts, detector, fps, first_frame: int = 0) -> list[int]:
     """Run the device automaton that corresponds to a (fresh) detector object of this package with the
-    detector's own parameters: the cut list its per-frame `process_frame` + `post_process` would produce."""
+    detector's own parameters: the cut list its per-frame `process_frame` + `post_process` would produce.  The
+    metrics come from the detector's slots of the engine (those `attach_engine` gave it; 0 otherwise)."""
     method, kwargs = automaton_args(detector)
+    if method in ("content", "adaptive") and detector._edge_slot:
+        kwargs["edge_slot"] = detector._edge_slot
+    if method == "hash" and detector._hash_slot:
+        kwargs["hash_slot"] = detector._hash_slot
     return getattr(dc, method)(**kwargs, fps=fps, first_frame=first_frame)

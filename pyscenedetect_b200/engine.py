@@ -4,6 +4,7 @@ replacement for the per-frame cv2/numpy work inside the reference detectors."""
 from __future__ import annotations
 
 import ctypes as C
+import math
 
 import numpy as np
 
@@ -88,6 +89,7 @@ class Engine:
         cfg.max_batch = int(max_batch)
         cfg.hash_size, cfg.hash_lowpass = int(hash_size), int(hash_lowpass)
         self.hash_size = int(hash_size)
+        self._hash_sizes = [self.hash_size]  # per hash slot
         h = C.c_void_p()
         check(self._lib.psd_engine_create(C.byref(cfg), C.byref(h)), "psd_engine_create")
         self._h = h
@@ -168,6 +170,41 @@ class Engine:
     def edge_kernel_size(self) -> int:
         return int(self._lib.psd_engine_edge_kernel_size(self._h))
 
+    # -- slots: more kernel sizes / hash geometries scored from the same pass (before the first frame) --
+    def add_edge_kernel_size(self, kernel_size: int) -> int:
+        """Edge slot of a ContentDetector(kernel_size=...) (0 = automatic) next to the configured one; the slot
+        already holding that effective size if there is one.  RuntimeError once the engine holds frames."""
+        slot = C.c_int32()
+        check(self._lib.psd_engine_add_edge_kernel_size(self._h, int(kernel_size), C.byref(slot)),
+              "psd_engine_add_edge_kernel_size")
+        return slot.value
+
+    def add_hash_geometry(self, size: int, lowpass: int) -> int:
+        """Hash slot of a HashDetector(size=..., lowpass=...); the existing slot if that geometry is present."""
+        slot = C.c_int32()
+        check(self._lib.psd_engine_add_hash_geometry(self._h, int(size), int(lowpass), C.byref(slot)),
+              "psd_engine_add_hash_geometry")
+        if slot.value == len(self._hash_sizes):
+            self._hash_sizes.append(int(size) or 8)
+        return slot.value
+
+    def edge_kernel_size_at(self, slot: int) -> int:
+        return int(self._lib.psd_engine_edge_kernel_size_at(self._h, int(slot)))
+
+    def hash_size_at(self, slot: int) -> int:
+        return self._hash_sizes[slot]
+
+    def device_edge_sads(self, edge_slot: int = 0) -> int | None:
+        """Device array of an edge slot's sad_edges (stream frame i at index i); None for slot 0, whose SADs are
+        the sums' sad_edges."""
+        p = C.c_void_p()
+        check(self._lib.psd_engine_device_edge_sads(self._h, int(edge_slot), C.byref(p)),
+              "psd_engine_device_edge_sads")
+        return p.value
+
+    def view(self, edge_slot: int = 0, hash_slot: int = 0) -> "SlotView":
+        return SlotView(self, edge_slot, hash_slot)
+
     # -- raw integer results --
     def read_sums(self, first: int = 0, n: int | None = None) -> np.ndarray:
         n = self.frame_count - first if n is None else n
@@ -181,17 +218,18 @@ class Engine:
         check(self._lib.psd_engine_read_yhist(self._h, first, n, out.ctypes.data), "psd_engine_read_yhist")
         return out
 
-    def read_hash(self, first: int = 0, n: int | None = None) -> np.ndarray:
+    def read_hash(self, first: int = 0, n: int | None = None, hash_slot: int = 0) -> np.ndarray:
         """-> (n, hash_words(size)) uint64: bit u*size+v of the row (word k // 64, bit k % 64) = DCT[u][v] > median
         (hash_detector.py:156); 4 words for size <= 16."""
         n = self.frame_count - first if n is None else n
-        out = np.zeros((n, hash_words(self.hash_size)), dtype=np.uint64)
-        check(self._lib.psd_engine_read_hash(self._h, first, n, out.ctypes.data), "psd_engine_read_hash")
+        out = np.zeros((n, hash_words(self.hash_size_at(hash_slot))), dtype=np.uint64)
+        check(self._lib.psd_engine_read_hash_at(self._h, int(hash_slot), first, n, out.ctypes.data),
+              "psd_engine_read_hash")
         return out
 
-    def device_hash(self) -> int | None:
+    def device_hash(self, hash_slot: int = 0) -> int | None:
         p = C.c_void_p()
-        check(self._lib.psd_engine_device_hash(self._h, C.byref(p)))
+        check(self._lib.psd_engine_device_hash_at(self._h, int(hash_slot), C.byref(p)))
         return p.value
 
     def device_results(self) -> tuple[int, int | None]:
@@ -200,16 +238,17 @@ class Engine:
         return s.value, h.value
 
     # -- trailing device scans (host-array convenience forms) --
-    def scan_content(self, weights, first: int = 0, n: int | None = None):
+    def scan_content(self, weights, first: int = 0, n: int | None = None, edge_slot: int = 0):
         """-> (content_val[n], components[n,4]) as float64; bit-identical to
-        content_detector.py:166-180."""
+        content_detector.py:166-180 (the edge component of edge slot `edge_slot`)."""
         n = self.frame_count - first if n is None else n
         w = (C.c_double * 4)(*[float(x) for x in weights])
         wsum = float(sum(abs(x) for x in weights))  # same expression as content_detector.py:180
         val = np.zeros(n, dtype=np.float64)
         comps = np.zeros((n, 4), dtype=np.float64)
-        check(self._lib.psd_engine_scan_content_host(self._h, first, n, w, wsum, comps.ctypes.data,
-                                                     val.ctypes.data), "psd_engine_scan_content_host")
+        check(self._lib.psd_engine_scan_content_host_at(self._h, int(edge_slot), first, n, w, wsum,
+                                                        comps.ctypes.data, val.ctypes.data),
+              "psd_engine_scan_content_host")
         return val, comps
 
     def scan_adaptive(self, scores: np.ndarray, window_width: int, min_content_val: float) -> np.ndarray:
@@ -234,11 +273,11 @@ class Engine:
               "psd_engine_scan_hist_correl_host")
         return out
 
-    def scan_hash_dist(self, first: int = 0, n: int | None = None) -> np.ndarray:
+    def scan_hash_dist(self, first: int = 0, n: int | None = None, hash_slot: int = 0) -> np.ndarray:
         """hash_dist of frames [first, first+n) against their predecessors; NaN where there is none."""
         n = self.frame_count - first if n is None else n
         out = np.zeros(n, dtype=np.float64)
-        check(self._lib.psd_engine_scan_hash_dist_host(self._h, first, n, out.ctypes.data),
+        check(self._lib.psd_engine_scan_hash_dist_host_at(self._h, int(hash_slot), first, n, out.ctypes.data),
               "psd_engine_scan_hash_dist_host")
         return out
 
@@ -259,6 +298,46 @@ class Engine:
         check(self._lib.psd_engine_debug_plane(self._h, which, index, out.ctypes.data, out.nbytes),
               "psd_engine_debug_plane")
         return out
+
+
+class SlotView:
+    """An Engine with one edge slot and one hash slot selected: what a detector (or a sweep's pixel group) that
+    shares the engine reads.  Everything else is the engine's own."""
+
+    def __init__(self, engine: Engine, edge_slot: int = 0, hash_slot: int = 0):
+        self._engine = engine
+        self.edge_slot, self.hash_slot = int(edge_slot), int(hash_slot)
+
+    def __getattr__(self, name):
+        return getattr(self._engine, name)
+
+    @property
+    def hash_size(self) -> int:
+        return self._engine.hash_size_at(self.hash_slot)
+
+    def device_edge_sads(self) -> int | None:
+        return self._engine.device_edge_sads(self.edge_slot)
+
+    def device_hash(self) -> int | None:
+        return self._engine.device_hash(hash_slot=self.hash_slot)
+
+    def read_hash(self, first: int = 0, n: int | None = None) -> np.ndarray:
+        return self._engine.read_hash(first, n, hash_slot=self.hash_slot)
+
+    def scan_content(self, weights, first: int = 0, n: int | None = None):
+        return self._engine.scan_content(weights, first, n, edge_slot=self.edge_slot)
+
+    def scan_hash_dist(self, first: int = 0, n: int | None = None) -> np.ndarray:
+        return self._engine.scan_hash_dist(first, n, hash_slot=self.hash_slot)
+
+
+def effective_kernel_size(kernel_size: int, width: int, height: int) -> int:
+    """The dilation kernel size of ContentDetector(kernel_size=...) on width x height frames (0 = automatic,
+    content_detector.py:39-46)."""
+    if kernel_size:
+        return int(kernel_size)
+    k = 4 + round(math.sqrt(width * height) / 192)
+    return k + 1 if k % 2 == 0 else k
 
 
 def bind_host_to_gpu_numa_node(device: int = 0) -> dict:
@@ -301,5 +380,5 @@ def synth_frames_device(dptr: int, params: np.ndarray, width: int, height: int,
           "psd_synth_frames")
 
 
-__all__ = ["Engine", "PinnedBuffer", "DeviceBuffer", "synth_frames_device", "bind_host_to_gpu_numa_node", "F_HSV", "F_BGRSUM",
+__all__ = ["Engine", "SlotView", "effective_kernel_size", "PinnedBuffer", "DeviceBuffer", "synth_frames_device", "bind_host_to_gpu_numa_node", "F_HSV", "F_BGRSUM",
            "F_YHIST", "F_EDGES", "F_HASH"]

@@ -5,9 +5,10 @@ The reference's benchmark harness (benchmark/sweep.py:142-187) decodes a video o
 and runs a complete SceneManager + detector per cell, so the per-frame cv2 arithmetic runs once per cell.
 Almost no grid parameter changes that arithmetic, only the cut automaton after it.  Here:
 
-* cells whose pixel-pass parameters agree (`required_features`, `edge_kernel_size_arg`, `engine_kwargs`:
-  the rules SceneManager.detect_scenes applies) form one pixel group with one `Engine`; the video is
-  decoded once and every batch goes to every group's engine;
+* cells whose pixel-pass parameters agree (`required_features`, `edge_kernel_size_arg`, `engine_kwargs`)
+  form one pixel group; `run` decodes the video once into ONE `Engine` that holds every group's dilation
+  kernel size and hash geometry as a slot (as SceneManager.detect_scenes does for its detectors), so each
+  batch is uploaded, resized, scored and Canny-classified once;
 * each distinct metric array (content_val per weight vector, adaptive ratio per (weights, window_width,
   min_content_val), average_rgb, hist correlation per `bins`, hash distance) is computed once by the
   existing psd_scan_* kernels;
@@ -37,7 +38,7 @@ from ._capi import F_EDGES, check
 from .detectors._base import EngineDetector
 from .device_cuts import automaton_args, flash_filter_frames, histogram_threshold, min_len_frames
 from .engine import DeviceBuffer, Engine
-from .scene_manager import FrameBatches, SceneManager
+from .scene_manager import FrameBatches, SceneManager, shared_engine
 
 _KIND = {"content": _capi.SWEEP_CONTENT, "adaptive": _capi.SWEEP_ADAPTIVE, "threshold": _capi.SWEEP_THRESHOLD,
          "histogram": _capi.SWEEP_HISTOGRAM, "hash": _capi.SWEEP_HASH}
@@ -273,44 +274,45 @@ class ParameterSweep:
 
     # -- the whole pass --
     def run(self, video, ground_truth: GroundTruth | None = None) -> SweepResult:
-        """Decode `video` once, score it with one Engine per pixel group (SceneManager's default geometry:
-        auto-downscale, no crop), then evaluate every cell.  Without ground truth nothing is scored (every
-        count is against an empty truth) and `totals` is not updated."""
+        """Decode `video` once, score it with one Engine (SceneManager's default geometry: auto-downscale, no
+        crop) that holds every pixel group's kernel size and hash geometry as a slot, then evaluate every cell.
+        Without ground truth nothing is scored (every count is against an empty truth) and `totals` is not
+        updated."""
         fw, fh = video.frame_size
         box, (w, h), (sw, sh) = SceneManager()._geometry(fw, fh)
-        engines = [g.make_engine(w, h, sw, sh, self.device, self.batch_size) for g in self.groups]
+        engine, slots = shared_engine([(g.features, g.edge_kernel_size, dict(g.engine_kwargs)) for g in self.groups],
+                                      w, h, sw, sh, device=self.device, max_batch=self.batch_size)
         gather = FrameBatches(video, box, (w, h), self.batch_size)
         first_frame = None
         try:
-            while True:
-                item = gather.next()  # overlaps the GPU's work on the previous batch
-                for e in engines:
-                    e.sync()  # retire the previous batch before its buffer is reused
-                if item is None:
-                    break
-                tcs, frames, pinned = item
-                if first_frame is None:
-                    first_frame = tcs[0].frame_num
-                for e in engines:
-                    e.submit(frames, pinned=pinned)
+            try:
+                while True:
+                    item = gather.next()  # overlaps the GPU's work on the previous batch
+                    engine.sync()  # retire the previous batch before its buffer is reused
+                    if item is None:
+                        break
+                    tcs, frames, pinned = item
+                    if first_frame is None:
+                        first_frame = tcs[0].frame_num
+                    engine.submit(frames, pinned=pinned)
+            finally:
+                gather.close()
+            if first_frame is None:
+                raise ValueError("the video has no frames")
+            end_frame = video.position.frame_num + 1  # SceneManager.get_scene_list's end (last position + 1)
+            # each pixel group reads the engine through its slots
+            return self.run_scored([engine.view(es, hs) for es, hs in slots], video.frame_rate, ground_truth,
+                                   first_frame=first_frame, end_frame=end_frame)
         finally:
-            gather.close()
-        if first_frame is None:
-            raise ValueError("the video has no frames")
-        end_frame = video.position.frame_num + 1  # SceneManager.get_scene_list's end (last position + 1)
-        try:
-            return self.run_scored(engines, video.frame_rate, ground_truth, first_frame=first_frame,
-                                   end_frame=end_frame)
-        finally:
-            for e in engines:
-                e.close()
+            engine.close()
 
     # -- the grid stage over results already held on the device --
     def run_scored(self, engines, fps, ground_truth: GroundTruth | None = None, first_frame: int = 0,
                    end_frame: int | None = None) -> SweepResult:
         """Evaluate every cell over frames the engines already scored: `engines[i]` holds pixel group
-        `self.groups[i]`'s results for the same frames, the first of which is frame `first_frame`.
-        `end_frame` defaults to first_frame + frame count."""
+        `self.groups[i]`'s results for the same frames, the first of which is frame `first_frame` - an Engine
+        per group, or a view (`Engine.view`) of one engine with the group's slots selected.  `end_frame`
+        defaults to first_frame + frame count."""
         if len(engines) != len(self.groups):
             raise ValueError(f"{len(self.groups)} pixel groups need as many engines, got {len(engines)}")
         lib = self._lib = self._lib or _capi.load()
@@ -355,8 +357,11 @@ class ParameterSweep:
                 sums, _ = e.device_results()
                 wts = key[2]
                 w = (C.c_double * 4)(*[float(x) for x in wts])
-                check(lib.psd_scan_content(sums, n, e.n_pixels, w, float(sum(abs(x) for x in wts)), comps.ptr,
-                                           arrays[key].ptr, st), "psd_scan_content")
+                # a view (Engine.view) of an edge slot other than 0 supplies that slot's edge SADs
+                sads = e.device_edge_sads() if getattr(e, "edge_slot", 0) else None
+                check(lib.psd_scan_content_edges(sums, sads, n, e.n_pixels, w,
+                                                 float(sum(abs(x) for x in wts)), comps.ptr, arrays[key].ptr, st),
+                      "psd_scan_content")
             elif key[0] == "adaptive_ratio":
                 check(lib.psd_scan_adaptive(arrays[("content_val",) + key[1:3]].ptr, n, key[3], key[4],
                                             arrays[key].ptr, st), "psd_scan_adaptive")
