@@ -3,10 +3,36 @@ call, as SceneManager drives it: scene_manager.py:426-428) and batched submissio
 
 from __future__ import annotations
 
+from dataclasses import dataclass
+
 import numpy as np
 
+from .._capi import F_EDGES
 from ..compat import SceneDetector
 from ..engine import Engine
+
+
+@dataclass(frozen=True)
+class PixelGroup:
+    """What a detector needs from the fused pixel pass: the Engine arguments of detectors (or sweep cells) that
+    can share one score pass."""
+
+    features: int
+    edge_kernel_size: int
+    engine_kwargs: tuple  # sorted (name, value) pairs
+
+    def make_engine(self, src_width: int, src_height: int, width: int, height: int, device: int = 0,
+                    max_batch: int = 64) -> Engine:
+        return Engine(src_width, src_height, self.features, width=width, height=height, device=device,
+                      max_batch=max_batch, edge_kernel_size=self.edge_kernel_size, **dict(self.engine_kwargs))
+
+
+def pixel_group_of(detector) -> PixelGroup:
+    """The features a detector needs, its dilation kernel size argument when it uses the edge component
+    (content_detector.py:135-138; 0 otherwise) and its extra Engine arguments (the hash geometry)."""
+    feats = detector.required_features()
+    return PixelGroup(feats, detector.edge_kernel_size_arg() if feats & F_EDGES else 0,
+                      tuple(sorted(detector.engine_kwargs().items())))
 
 
 class EngineDetector(SceneDetector):
@@ -29,8 +55,6 @@ class EngineDetector(SceneDetector):
         self._max_batch = 16  # strict mode submits one frame per call; staging is sized by this
         self._scored_size: tuple[int, int] | None = None  # (width, height) detectors see
         self._base_index = 0  # engine frame index of this detector's first frame
-        self._edge_slot = 0   # the engine's slots of this detector's kernel size / hash geometry (attach_engine)
-        self._hash_slot = 0
 
     # -- configuration hooks used by SceneManager's batched fast path --
     def required_features(self) -> int:
@@ -50,24 +74,21 @@ class EngineDetector(SceneDetector):
         self._max_batch = max_batch
         self._scored_size = scored_size
 
-    def attach_engine(self, engine: Engine, edge_slot: int = 0, hash_slot: int = 0) -> None:
-        """Share one fused pass between several detectors (SceneManager does this).  `edge_slot` / `hash_slot`:
-        the engine's slot that holds this detector's dilation kernel size / hash geometry."""
-        self._edge_slot, self._hash_slot = int(edge_slot), int(hash_slot)
-        self._engine = engine.view(edge_slot, hash_slot) if (edge_slot or hash_slot) else engine
+    def attach_engine(self, holder) -> None:
+        """Share one fused pass between several detectors (SceneManager does this).  `holder` holds this
+        detector's results: an Engine, a `SlotView` of one (`Engine.view`) or gathered results."""
+        self._engine = holder
         self._owns_engine = False
-        self._base_index = engine.frame_count
+        self._base_index = holder.frame_count
 
     def _ensure_engine(self, frames: np.ndarray) -> Engine:
         if self._engine is None:
             h, w = frames.shape[-3], frames.shape[-2]
             sw, sh = self._scored_size if self._scored_size else (w, h)
-            self._engine = Engine(w, h, self.required_features(), width=sw, height=sh,
-                                  device=self._device, max_batch=self._max_batch,
-                                  edge_kernel_size=self.edge_kernel_size_arg(), **self.engine_kwargs())
+            self._engine = pixel_group_of(self).make_engine(w, h, sw, sh, device=self._device,
+                                                            max_batch=self._max_batch)
             self._owns_engine = True
             self._base_index = 0
-            self._edge_slot = self._hash_slot = 0
         return self._engine
 
     @staticmethod

@@ -57,6 +57,34 @@ def min_len_frames(length, fps) -> int:
     raise TypeError("unsupported min_scene_len")
 
 
+def scan_metric(lib, holder, key: tuple, out: int, content_val: int | None = None) -> None:
+    """Launch the psd_scan_* that fills one metric array `out` (float64 per frame) from every frame a result holder
+    (an Engine, a `SlotView` of one or `sharding.GatheredResults`) holds, on the holder's stream.  `key` is a
+    `ParameterSweep` metric key without its group index: ("content_val", weights), ("adaptive_ratio", weights,
+    window_width, min_content_val), which reads `content_val` (that weight vector's array), ("average_rgb",),
+    ("hist_correl", bins) or ("hash_dist",)."""
+    n, st = holder.frame_count, holder.compute_stream
+    kind = key[0]
+    if kind == "content_val":
+        sums, _ = holder.device_results()
+        w = (C.c_double * 4)(*[float(x) for x in key[1]])
+        wsum = float(sum(abs(x) for x in key[1]))  # same expression as content_detector.py:180
+        # NULL edge SADs: the sums' own sad_edges (edge slot 0)
+        check(lib.psd_scan_content_edges(sums, holder.device_edge_sads(), n, holder.n_pixels, w, wsum, None, out, st),
+              "psd_scan_content_edges")
+    elif kind == "adaptive_ratio":
+        check(lib.psd_scan_adaptive(content_val, n, int(key[2]), float(key[3]), out, st), "psd_scan_adaptive")
+    elif kind == "average_rgb":
+        sums, _ = holder.device_results()
+        check(lib.psd_scan_average(sums, n, holder.n_pixels * 3, out, st), "psd_scan_average")
+    elif kind == "hist_correl":
+        _, yhist = holder.device_results()
+        check(lib.psd_scan_hist_correl(yhist, n, int(key[1]), None, out, st), "psd_scan_hist_correl")
+    else:
+        check(lib.psd_scan_hash_dist(holder.device_hash(), n, int(holder.hash_size), None, out, st),
+              "psd_scan_hash_dist")
+
+
 class DeviceCuts:
     def __init__(self, engine: Engine, max_cuts: int = 1 << 16):
         self._e = engine
@@ -67,8 +95,10 @@ class DeviceCuts:
         self._count = DeviceBuffer(8, self._dev)
         self._stream = engine.compute_stream
 
-    def _tmp(self, n_doubles: int) -> DeviceBuffer:
-        return DeviceBuffer(max(8, n_doubles * 8), self._dev)
+    def _scan(self, key: tuple, content_val: DeviceBuffer | None = None) -> DeviceBuffer:
+        out = DeviceBuffer(max(8, self._e.frame_count * 8), self._dev)
+        scan_metric(self._lib, self._e, key, out.ptr, content_val.ptr if content_val is not None else None)
+        return out
 
     def _fetch(self) -> list[int]:
         self._e.sync()
@@ -77,23 +107,10 @@ class DeviceCuts:
             raise RuntimeError(f"{count} cuts exceed the device cut buffer ({self._cap})")
         return self._cuts.download(count * 8).view(np.int64).tolist() if count else []
 
-    def _content_scores(self, weights, n, edge_slot: int = 0):
-        sums, _ = self._e.device_results()
-        val, comps = self._tmp(n), self._tmp(4 * n)
-        w = (C.c_double * 4)(*[float(x) for x in weights])
-        wsum = float(sum(abs(x) for x in weights))
-        if edge_slot:  # the edge SADs of another kernel size replace the sums' own
-            check(self._lib.psd_scan_content_edges(sums, self._e.device_edge_sads(edge_slot), n, self._e.n_pixels,
-                                                   w, wsum, comps.ptr, val.ptr, self._stream), "psd_scan_content_edges")
-        else:
-            check(self._lib.psd_scan_content(sums, n, self._e.n_pixels, w, wsum, comps.ptr, val.ptr, self._stream),
-                  "psd_scan_content")
-        return val, comps
-
     def content(self, weights=(1.0, 1.0, 1.0, 0.0), threshold=27.0, min_scene_len=15, fps=30.0,
-                suppress: bool = False, first_frame: int = 0, edge_slot: int = 0) -> list[int]:
+                suppress: bool = False, first_frame: int = 0) -> list[int]:
         n = self._e.frame_count
-        val, _comps = self._content_scores(weights, n, edge_slot)
+        val = self._scan(("content_val", weights))
         flags = DeviceBuffer(max(1, n), self._dev)
         check(self._lib.psd_scan_compare(val.ptr, n, float(threshold), 0, flags.ptr, self._stream))
         check(self._lib.psd_cuts_flash_filter(flags.ptr, n, first_frame, flash_filter_frames(min_scene_len, fps),
@@ -102,12 +119,10 @@ class DeviceCuts:
         return self._fetch()
 
     def adaptive(self, weights=(1.0, 1.0, 1.0, 0.0), adaptive_threshold=3.0, min_scene_len=15,
-                 window_width=2, min_content_val=15.0, fps=30.0, first_frame: int = 0, edge_slot: int = 0) -> list[int]:
+                 window_width=2, min_content_val=15.0, fps=30.0, first_frame: int = 0) -> list[int]:
         n = self._e.frame_count
-        val, _comps = self._content_scores(weights, n, edge_slot)
-        ratio = self._tmp(n)
-        check(self._lib.psd_scan_adaptive(val.ptr, n, int(window_width), float(min_content_val), ratio.ptr,
-                                          self._stream), "psd_scan_adaptive")
+        val = self._scan(("content_val", weights))
+        ratio = self._scan(("adaptive_ratio", weights, window_width, min_content_val), val)
         check(self._lib.psd_cuts_adaptive(ratio.ptr, val.ptr, n, first_frame, int(window_width),
                                           float(adaptive_threshold), float(min_content_val),
                                           min_len_frames(min_scene_len, fps), self._cuts.ptr, self._count.ptr,
@@ -116,19 +131,15 @@ class DeviceCuts:
 
     def histogram(self, threshold=0.20, bins=128, min_scene_len=15, fps=30.0, first_frame: int = 0) -> list[int]:
         n = self._e.frame_count
-        _, hist = self._e.device_results()
-        corr = self._tmp(n)
-        check(self._lib.psd_scan_hist_correl(hist, n, int(bins), None, corr.ptr, self._stream))
+        corr = self._scan(("hist_correl", bins))
         check(self._lib.psd_cuts_histogram(corr.ptr, n, first_frame, histogram_threshold(threshold),
                                            min_len_frames(min_scene_len, fps), self._cuts.ptr, self._count.ptr,
                                            self._cap, self._stream), "psd_cuts_histogram")
         return self._fetch()
 
-    def hash(self, threshold=0.35, min_scene_len=15, fps=30.0, first_frame: int = 0, hash_slot: int = 0) -> list[int]:
+    def hash(self, threshold=0.35, min_scene_len=15, fps=30.0, first_frame: int = 0) -> list[int]:
         n = self._e.frame_count
-        e = self._e.view(hash_slot=hash_slot) if hash_slot else self._e
-        dist = self._tmp(n)
-        check(self._lib.psd_scan_hash_dist(e.device_hash(), n, int(e.hash_size), None, dist.ptr, self._stream))
+        dist = self._scan(("hash_dist",))
         check(self._lib.psd_cuts_hash(dist.ptr, n, first_frame, float(threshold), min_len_frames(min_scene_len, fps),
                                       self._cuts.ptr, self._count.ptr, self._cap, self._stream), "psd_cuts_hash")
         return self._fetch()
@@ -136,9 +147,7 @@ class DeviceCuts:
     def threshold(self, threshold=12, min_scene_len=15, fade_bias=0.0, add_final_scene=False,
                   ceiling: bool = False, fps=30.0, first_frame: int = 0) -> list[int]:
         n = self._e.frame_count
-        sums, _ = self._e.device_results()
-        avg = self._tmp(n)
-        check(self._lib.psd_scan_average(sums, n, self._e.n_pixels * 3, avg.ptr, self._stream))
+        avg = self._scan(("average_rgb",))
         check(self._lib.psd_cuts_threshold(avg.ptr, n, first_frame, float(int(threshold)), 1 if ceiling else 0,
                                            float(fade_bias), min_len_frames(min_scene_len, fps),
                                            1 if add_final_scene else 0, self._cuts.ptr, self._count.ptr,
@@ -183,10 +192,10 @@ def automaton_args(detector) -> tuple[str, dict]:
 def cuts_for_detector(dc: DeviceCuts, detector, fps, first_frame: int = 0) -> list[int]:
     """Run the device automaton that corresponds to a (fresh) detector object of this package with the
     detector's own parameters: the cut list its per-frame `process_frame` + `post_process` would produce.  The
-    metrics come from the detector's slots of the engine (those `attach_engine` gave it; 0 otherwise)."""
+    metrics come from the result holder `attach_engine` gave the detector (its slots of a shared engine), else from
+    `dc`'s."""
     method, kwargs = automaton_args(detector)
-    if method in ("content", "adaptive") and detector._edge_slot:
-        kwargs["edge_slot"] = detector._edge_slot
-    if method == "hash" and detector._hash_slot:
-        kwargs["hash_slot"] = detector._hash_slot
+    holder = detector._engine
+    if holder is not None and not detector._owns_engine and holder is not dc._e:
+        dc = DeviceCuts(holder, dc._cap)
     return getattr(dc, method)(**kwargs, fps=fps, first_frame=first_frame)

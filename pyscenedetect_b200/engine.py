@@ -4,7 +4,6 @@ replacement for the per-frame cv2/numpy work inside the reference detectors."""
 from __future__ import annotations
 
 import ctypes as C
-import math
 
 import numpy as np
 
@@ -202,8 +201,9 @@ class Engine:
               "psd_engine_device_edge_sads")
         return p.value
 
-    def view(self, edge_slot: int = 0, hash_slot: int = 0) -> "SlotView":
-        return SlotView(self, edge_slot, hash_slot)
+    def view(self, edge_slot: int = 0, hash_slot: int = 0) -> "Engine | SlotView":
+        """The results of the given slots: the engine itself for slots 0 / 0, else a `SlotView`."""
+        return SlotView(self, edge_slot, hash_slot) if edge_slot or hash_slot else self
 
     # -- raw integer results --
     def read_sums(self, first: int = 0, n: int | None = None) -> np.ndarray:
@@ -331,15 +331,6 @@ class SlotView:
         return self._engine.scan_hash_dist(first, n, hash_slot=self.hash_slot)
 
 
-def effective_kernel_size(kernel_size: int, width: int, height: int) -> int:
-    """The dilation kernel size of ContentDetector(kernel_size=...) on width x height frames (0 = automatic,
-    content_detector.py:39-46)."""
-    if kernel_size:
-        return int(kernel_size)
-    k = 4 + round(math.sqrt(width * height) / 192)
-    return k + 1 if k % 2 == 0 else k
-
-
 def bind_host_to_gpu_numa_node(device: int = 0) -> dict:
     """Pin the calling process to the CPUs of the GPU's NUMA node so that page-locked staging
     buffers allocated afterwards are local to the GPU's PCIe root (first-touch placement).  Returns
@@ -380,5 +371,5 @@ def synth_frames_device(dptr: int, params: np.ndarray, width: int, height: int,
           "psd_synth_frames")
 
 
-__all__ = ["Engine", "SlotView", "effective_kernel_size", "PinnedBuffer", "DeviceBuffer", "synth_frames_device", "bind_host_to_gpu_numa_node", "F_HSV", "F_BGRSUM",
+__all__ = ["Engine", "SlotView", "PinnedBuffer", "DeviceBuffer", "synth_frames_device", "bind_host_to_gpu_numa_node", "F_HSV", "F_BGRSUM",
            "F_YHIST", "F_EDGES", "F_HASH"]

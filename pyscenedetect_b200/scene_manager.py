@@ -25,9 +25,9 @@ import logging
 import numpy as np
 
 from .compat import FrameTimecode, StatsManager
-from .detectors._base import EngineDetector
+from .detectors._base import EngineDetector, pixel_group_of
 from ._capi import F_EDGES, F_HASH
-from .engine import Engine, PinnedBuffer, effective_kernel_size
+from .engine import Engine, PinnedBuffer
 
 DEFAULT_MIN_WIDTH = 256
 logger = logging.getLogger("pyscenedetect_b200")
@@ -55,41 +55,31 @@ def get_scenes_from_cuts(cut_list, start_pos, end_pos):
     return scene_list
 
 
-def pixel_pass_of(detector) -> tuple[int, int, dict]:
-    """What a detector needs from the pixel pass: its features, its dilation kernel size argument if it uses the
-    edge component (content_detector.py:135-138; 0 otherwise) and its extra Engine arguments (the hash geometry)."""
-    feats = detector.required_features()
-    return feats, detector.edge_kernel_size_arg() if feats & F_EDGES else 0, detector.engine_kwargs()
-
-
-def shared_engine(passes, src_width: int, src_height: int, width: int, height: int, device: int = 0,
+def shared_engine(groups, src_width: int, src_height: int, width: int, height: int, device: int = 0,
                   max_batch: int = 64):
-    """One Engine for several pixel passes (`pixel_pass_of` tuples): the union of their features, the first edge
-    user's kernel size and the first hash user's geometry in the configuration, and every other distinct effective
-    kernel size and geometry as a further slot, in order of appearance.  -> (engine, [(edge_slot, hash_slot)] per
-    pass); a pass that does not use the edge component or the hash gets slot 0 for it."""
+    """One Engine for several `PixelGroup`s: the union of their features, the first edge user's kernel size and
+    the first hash user's geometry in the configuration, and every other distinct effective kernel size and
+    geometry as a further slot, in order of appearance (the engine deduplicates).  -> (engine, one result holder
+    per group: `engine.view` of the group's slots); a group that does not use the edge component or the hash
+    reads slot 0 for it."""
     features = 0
-    for feats, _, _ in passes:
-        features |= feats
-    ks = [k for feats, k, _ in passes if feats & F_EDGES]
-    geo = [(kw["hash_size"], kw["hash_lowpass"]) for feats, _, kw in passes if feats & F_HASH]
-    extra = dict(hash_size=geo[0][0], hash_lowpass=geo[0][1]) if geo else {}
+    for g in groups:
+        features |= g.features
+    k0 = next((g.edge_kernel_size for g in groups if g.features & F_EDGES), 0)
+    geo0 = next((dict(g.engine_kwargs) for g in groups if g.features & F_HASH), {})
     engine = Engine(src_width, src_height, features, width=width, height=height, device=device, max_batch=max_batch,
-                    edge_kernel_size=ks[0] if ks else 0, **extra)
-    edge_slots = {effective_kernel_size(ks[0], width, height): 0} if ks else {}
-    hash_slots = {geo[0]: 0} if geo else {}
-    for k in ks:
-        k = effective_kernel_size(k, width, height)
-        if k not in edge_slots:
-            edge_slots[k] = engine.add_edge_kernel_size(k)
-    for g in geo:
-        if g not in hash_slots:
-            hash_slots[g] = engine.add_hash_geometry(*g)
-    slots = []
-    for feats, k, kw in passes:
-        slots.append((edge_slots[effective_kernel_size(k, width, height)] if feats & F_EDGES else 0,
-                      hash_slots[(kw["hash_size"], kw["hash_lowpass"])] if feats & F_HASH else 0))
-    return engine, slots
+                    edge_kernel_size=k0, **geo0)
+    holders = []
+    for g in groups:
+        # the configured kernel size argument and geometry are slot 0 without asking, so a scorer with one slot of
+        # each (tests/fake_engine.py) needs no slot calls for a mix that has nothing else
+        kw = dict(g.engine_kwargs)
+        edge_slot = (engine.add_edge_kernel_size(g.edge_kernel_size)
+                     if g.features & F_EDGES and g.edge_kernel_size != k0 else 0)
+        hash_slot = (engine.add_hash_geometry(kw["hash_size"], kw["hash_lowpass"])
+                     if g.features & F_HASH and kw != geo0 else 0)
+        holders.append(engine.view(edge_slot, hash_slot) if edge_slot or hash_slot else engine)
+    return engine, holders
 
 
 class FrameBatches:
@@ -310,10 +300,10 @@ class SceneManager:
         self._frame_tail = []
         fw, fh = video.frame_size
         (x0, y0, x1, y1), (w, h), (sw, sh) = self._geometry(fw, fh)
-        self._engine, slots = shared_engine([pixel_pass_of(d) for d in self._detector_list], w, h, sw, sh,
-                                            device=self._device, max_batch=self._batch_size)
-        for d, (edge_slot, hash_slot) in zip(self._detector_list, slots):
-            d.attach_engine(self._engine, edge_slot=edge_slot, hash_slot=hash_slot)
+        self._engine, holders = shared_engine([pixel_group_of(d) for d in self._detector_list], w, h, sw, sh,
+                                              device=self._device, max_batch=self._batch_size)
+        for d, holder in zip(self._detector_list, holders):
+            d.attach_engine(holder)
         fps = video.frame_rate
         base = getattr(video, "base_timecode", None)
         self._base_timecode = base if base is not None else FrameTimecode(0, fps)

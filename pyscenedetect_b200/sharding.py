@@ -122,6 +122,9 @@ class GatheredResults:
     def device_hash(self):
         return self._hashes.ptr if self._hashes is not None else None
 
+    def device_edge_sads(self):
+        return None  # the gathered sums' own sad_edges
+
     def sync(self):
         pass
 
@@ -196,6 +199,7 @@ def detect_sharded(frames_local: np.ndarray, first_index: int, total_frames: int
     import time
 
     from .compat import FrameTimecode
+    from .detectors._base import pixel_group_of
     t_start = time.perf_counter()
     if engine_factory is None:
         from .engine import Engine as engine_factory  # noqa: N813
@@ -203,9 +207,10 @@ def detect_sharded(frames_local: np.ndarray, first_index: int, total_frames: int
         results_factory = GatheredResults
     ring, h, w = frames_local.shape[0], frames_local.shape[1], frames_local.shape[2]
     n_local = ring if n_local is None else int(n_local)
-    features = detector.required_features()
+    group = pixel_group_of(detector)
+    features = group.features
     eng = engine_factory(w, h, features, device=device, max_batch=batch_size,
-                         edge_kernel_size=detector.edge_kernel_size_arg(), **detector.engine_kwargs())
+                         edge_kernel_size=group.edge_kernel_size, **dict(group.engine_kwargs))
     halo = comm.exchange_halo(frames_local[(n_local - 1) % ring] if n_local else None, (h, w, 3))
     if halo is not None:
         if isinstance(halo, np.ndarray):
@@ -242,14 +247,14 @@ def detect_sharded(frames_local: np.ndarray, first_index: int, total_frames: int
     assert all_sums.dtype == SUMS_DTYPE and all_sums.shape[0] == total_frames
     res = (results_factory(all_sums, all_hist, w * h, device, hashes=all_hash, **detector.engine_kwargs())
            if all_hash is not None else results_factory(all_sums, all_hist, w * h, device))
+    detector.attach_engine(res)
+    detector._base_index = 0
     if detector.stats_manager is None and hasattr(res, "device_results"):
         from .device_cuts import DeviceCuts, cuts_for_detector
         cut_frames = sorted(set(cuts_for_detector(DeviceCuts(res), detector, fps)))
         note(time.perf_counter())
         return cut_frames, all_sums
-    detector.attach_engine(res)
-    detector._base_index = 0
-    tcs = [FrameTimecode(i, fps) for i in range(total_frames)]
+    tcs =[FrameTimecode(i, fps) for i in range(total_frames)]
     cuts = []
     for i in range(0, total_frames, 4096):
         cuts += detector.consume_results(tcs[i:i + 4096], i)

@@ -34,10 +34,10 @@ from dataclasses import dataclass, field
 import numpy as np
 
 from . import _capi
-from ._capi import F_EDGES, check
-from .detectors._base import EngineDetector
-from .device_cuts import automaton_args, flash_filter_frames, histogram_threshold, min_len_frames
-from .engine import DeviceBuffer, Engine
+from ._capi import check
+from .detectors._base import EngineDetector, PixelGroup, pixel_group_of
+from .device_cuts import automaton_args, flash_filter_frames, histogram_threshold, min_len_frames, scan_metric
+from .engine import DeviceBuffer
 from .scene_manager import FrameBatches, SceneManager, shared_engine
 
 _KIND = {"content": _capi.SWEEP_CONTENT, "adaptive": _capi.SWEEP_ADAPTIVE, "threshold": _capi.SWEEP_THRESHOLD,
@@ -106,20 +106,6 @@ class CellTotals:
 
 
 @dataclass(frozen=True)
-class PixelGroup:
-    """Cells that share one fused score pass: the Engine arguments they need."""
-
-    features: int
-    edge_kernel_size: int
-    engine_kwargs: tuple  # sorted (name, value) pairs
-
-    def make_engine(self, src_width: int, src_height: int, width: int, height: int, device: int = 0,
-                    max_batch: int = 64) -> Engine:
-        return Engine(src_width, src_height, self.features, width=width, height=height, device=device,
-                      max_batch=max_batch, edge_kernel_size=self.edge_kernel_size, **dict(self.engine_kwargs))
-
-
-@dataclass(frozen=True)
 class CellPlan:
     """One cell's automaton: kind, the metric key(s) it reads and the psd_sweep_cell fields; `min_scene_len`
     is converted to frames per video (`min_frames`)."""
@@ -162,14 +148,6 @@ def plan_cell(detector, group: int) -> CellPlan:
     return CellPlan("threshold", ("average_rgb", group), None, float(int(a["threshold"])),
                     mode=1 if a["ceiling"] else 0, fade_bias=float(a["fade_bias"]),
                     add_final_scene=1 if a["add_final_scene"] else 0, min_scene_len=a["min_scene_len"])
-
-
-def pixel_group_of(detector) -> PixelGroup:
-    """SceneManager.detect_scenes' rules: the features a detector needs, its dilation kernel when it uses the
-    edge component, and its extra Engine arguments."""
-    feats = detector.required_features()
-    return PixelGroup(feats, detector.edge_kernel_size_arg() if feats & F_EDGES else 0,
-                      tuple(sorted(detector.engine_kwargs().items())))
 
 
 class SweepResult:
@@ -280,8 +258,7 @@ class ParameterSweep:
         updated."""
         fw, fh = video.frame_size
         box, (w, h), (sw, sh) = SceneManager()._geometry(fw, fh)
-        engine, slots = shared_engine([(g.features, g.edge_kernel_size, dict(g.engine_kwargs)) for g in self.groups],
-                                      w, h, sw, sh, device=self.device, max_batch=self.batch_size)
+        engine, holders = shared_engine(self.groups, w, h, sw, sh, device=self.device, max_batch=self.batch_size)
         gather = FrameBatches(video, box, (w, h), self.batch_size)
         first_frame = None
         try:
@@ -300,9 +277,8 @@ class ParameterSweep:
             if first_frame is None:
                 raise ValueError("the video has no frames")
             end_frame = video.position.frame_num + 1  # SceneManager.get_scene_list's end (last position + 1)
-            # each pixel group reads the engine through its slots
-            return self.run_scored([engine.view(es, hs) for es, hs in slots], video.frame_rate, ground_truth,
-                                   first_frame=first_frame, end_frame=end_frame)
+            return self.run_scored(holders, video.frame_rate, ground_truth, first_frame=first_frame,
+                                   end_frame=end_frame)
         finally:
             engine.close()
 
@@ -311,8 +287,8 @@ class ParameterSweep:
                    end_frame: int | None = None) -> SweepResult:
         """Evaluate every cell over frames the engines already scored: `engines[i]` holds pixel group
         `self.groups[i]`'s results for the same frames, the first of which is frame `first_frame` - an Engine
-        per group, or a view (`Engine.view`) of one engine with the group's slots selected.  `end_frame`
-        defaults to first_frame + frame count."""
+        per group, or the group's view (`Engine.view`) of one engine that holds every group's slots.
+        `end_frame` defaults to first_frame + frame count."""
         if len(engines) != len(self.groups):
             raise ValueError(f"{len(self.groups)} pixel groups need as many engines, got {len(engines)}")
         lib = self._lib = self._lib or _capi.load()
@@ -324,8 +300,7 @@ class ParameterSweep:
         n_cells, n_tol, cap, dev = len(self.cells), len(self.tolerances), self.cap, self.device
         # allocations first, so the timed stage below is launches only
         arrays = {key: DeviceBuffer(n * 8, dev) for key in self.metric_keys}
-        comps = DeviceBuffer(4 * n * 8, dev)  # psd_scan_content's components (not read)
-        cuts = DeviceBuffer(n_cells * cap * 8, dev)
+        cuts =DeviceBuffer(n_cells * cap * 8, dev)
         count = DeviceBuffer(n_cells * 4, dev)
         n_pred = DeviceBuffer(n_cells * 4, dev)
         hard = DeviceBuffer(n_cells * n_tol * 5 * 8, dev)
@@ -351,29 +326,8 @@ class ParameterSweep:
 
         t0 = time.perf_counter()
         for key in self.metric_keys:  # one scan launch per distinct metric array
-            e = engines[key[1]]
-            st = e.compute_stream
-            if key[0] == "content_val":
-                sums, _ = e.device_results()
-                wts = key[2]
-                w = (C.c_double * 4)(*[float(x) for x in wts])
-                # a view (Engine.view) of an edge slot other than 0 supplies that slot's edge SADs
-                sads = e.device_edge_sads() if getattr(e, "edge_slot", 0) else None
-                check(lib.psd_scan_content_edges(sums, sads, n, e.n_pixels, w,
-                                                 float(sum(abs(x) for x in wts)), comps.ptr, arrays[key].ptr, st),
-                      "psd_scan_content")
-            elif key[0] == "adaptive_ratio":
-                check(lib.psd_scan_adaptive(arrays[("content_val",) + key[1:3]].ptr, n, key[3], key[4],
-                                            arrays[key].ptr, st), "psd_scan_adaptive")
-            elif key[0] == "average_rgb":
-                sums, _ = e.device_results()
-                check(lib.psd_scan_average(sums, n, e.n_pixels * 3, arrays[key].ptr, st), "psd_scan_average")
-            elif key[0] == "hist_correl":
-                _, yhist = e.device_results()
-                check(lib.psd_scan_hist_correl(yhist, n, key[2], None, arrays[key].ptr, st), "psd_scan_hist_correl")
-            else:
-                check(lib.psd_scan_hash_dist(e.device_hash(), n, int(e.hash_size), None, arrays[key].ptr, st),
-                      "psd_scan_hash_dist")
+            val = arrays[("content_val",) + key[1:3]].ptr if key[0] == "adaptive_ratio" else None
+            scan_metric(lib, engines[key[1]], (key[0],) + key[2:], arrays[key].ptr, val)
         if len(engines) > 1:  # the cells read every group's arrays: order them after every group's scans
             for e in engines[1:]:
                 e.sync()

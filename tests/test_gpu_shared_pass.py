@@ -1,7 +1,8 @@
 """Detectors that disagree on the dilation kernel size or the hash geometry in one SceneManager, one engine and one
 sweep: the reference's own SceneManager on such mixes (tests/golden/shared_pass_v1.json, recorded by
-tests/golden/make_shared_pass_golden.py), every slot of a many-slot engine against a one-slot engine on the same
-frames, the launches that stay shared, and ParameterSweep.run with one engine for several pixel groups."""
+tests/golden/make_shared_pass_golden.py), each detector's device automaton over the slots it is attached to, every
+slot of a many-slot engine against a one-slot engine on the same frames, the launches that stay shared, and
+ParameterSweep.run with one engine for several pixel groups."""
 
 import ctypes as C
 import json
@@ -36,8 +37,9 @@ def _frames(n, w, h, seed):
 
 @pytest.mark.parametrize("batch", [7, 64])
 @pytest.mark.parametrize("name", [c["name"] for c in _cases()])
-def test_shared_pass_scene_manager_matches_reference(name, batch):
+def test_shared_pass_scene_manager_attaches_views_and_matches_reference(name, batch):
     from pyscenedetect_b200 import StatsManager
+    from pyscenedetect_b200.engine import SlotView
     from pyscenedetect_b200.scene_manager import SceneManager
     from pyscenedetect_b200.video import ArrayVideoStream
     case = next(c for c in _cases() if c["name"] == name)
@@ -51,36 +53,73 @@ def test_shared_pass_scene_manager_matches_reference(name, batch):
         sm.downscale = case.get("downscale", 1)
     assert sm.detect_scenes(ArrayVideoStream(frames, case["fps"])) == frames.shape[0]
     # more than one kernel size or hash geometry really is in the one engine
-    assert max(d._edge_slot for d in sm._detector_list) + max(d._hash_slot for d in sm._detector_list) >= 1
+    assert any(isinstance(d._engine, SlotView) for d in sm._detector_list)
     assert [c.frame_num for c in sm.get_cut_list()] == case["cuts"]
     assert [[a.frame_num, b.frame_num] for a, b in sm.get_scene_list()] == case["scene_list"]
     _check_stats(case, stats, frames.shape[0])
+
+
+@pytest.mark.parametrize("name", [c["name"] for c in _cases()])
+def test_device_cuts_read_each_detectors_slots(name):
+    """`cuts_for_detector` over the shared engine of a SceneManager runs each detector's automaton over the slots
+    the detector is attached to: the cuts of a one-slot engine that scored the same frames for that detector
+    alone.  The cases hold non-zero edge slots (the first two) and non-zero hash slots (the last two)."""
+    from pyscenedetect_b200 import StatsManager
+    from pyscenedetect_b200.device_cuts import DeviceCuts, cuts_for_detector
+    from pyscenedetect_b200.engine import SlotView
+    from pyscenedetect_b200.scene_manager import SceneManager
+    from pyscenedetect_b200.sweep import pixel_group_of
+    from pyscenedetect_b200.video import ArrayVideoStream
+    case = next(c for c in _cases() if c["name"] == name)
+    frames, fps = case_frames(case), case["fps"]
+    sm = SceneManager(StatsManager())   # the StatsManager turns the edge component on for every content detector
+    for det, kw in case["dets"]:
+        sm.add_detector(_detector(det, kw))
+    sm.auto_downscale = bool(case.get("auto_downscale"))
+    if not sm.auto_downscale:
+        sm.downscale = case.get("downscale", 1)
+    sm.detect_scenes(ArrayVideoStream(frames, fps))
+    assert any(isinstance(d._engine, SlotView) for d in sm._detector_list)
+    _, (w, h), (sw, sh) = sm._geometry(frames.shape[2], frames.shape[1])
+    dc = DeviceCuts(sm._engine)
+    for d, (det, kw) in zip(sm._detector_list, case["dets"]):
+        alone = pixel_group_of(d).make_engine(w, h, sw, sh)   # d's own kernel size and hash geometry in slot 0
+        alone.submit(frames)
+        want = cuts_for_detector(DeviceCuts(alone), _detector(det, kw), fps)
+        alone.close()
+        assert cuts_for_detector(dc, d, fps) == want, (det, kw)
 
 
 KS = (3, 5, 17, 19, 63)
 GEOS = ((8, 2), (16, 2), (8, 3), (64, 2))   # (64, 2): a 128x128 hash image, whose finish runs from global memory
 
 
-def _edge_sads(eng, slot):
-    """stream frames' sad_edges of an edge slot, on the host"""
+def _edge_sads(holder):
+    """stream frames' sad_edges of a holder's edge slot, on the host"""
     from pyscenedetect_b200 import _capi
-    n = eng.frame_count
-    if slot == 0:
-        return eng.read_sums()["sad_edges"].copy()
-    out = np.zeros(n, dtype=np.uint64)
-    eng.sync()
-    assert _capi.load().psd_memcpy_d2h(eng.device, out.ctypes.data, eng.device_edge_sads(slot), n * 8) == 0
+    p = holder.device_edge_sads()
+    if p is None:
+        return holder.read_sums()["sad_edges"].copy()
+    out = np.zeros(holder.frame_count, dtype=np.uint64)
+    holder.sync()
+    assert _capi.load().psd_memcpy_d2h(holder.device, out.ctypes.data, p, out.nbytes) == 0
     return out
 
 
-def _snapshot(eng, edge_slots, hash_slots):
+def _snapshot(edges, hashes):
+    """{kernel size: holder}, {geometry: holder} -> every slot's results through the holders' slot-free accessors"""
     res = {}
-    for k, s in edge_slots.items():
-        val, comps = eng.scan_content(ALL, edge_slot=s)
-        res[("edges", k)] = (_edge_sads(eng, s).tobytes(), val.tobytes(), comps.tobytes())
-    for g, s in hash_slots.items():
-        res[("hash", g)] = (eng.read_hash(hash_slot=s).tobytes(), eng.scan_hash_dist(hash_slot=s).tobytes())
+    for k, e in edges.items():
+        val, comps = e.scan_content(ALL)
+        res[("edges", k)] = (_edge_sads(e).tobytes(), val.tobytes(), comps.tobytes())
+    for g, e in hashes.items():
+        res[("hash", g)] = (e.read_hash().tobytes(), e.scan_hash_dist().tobytes())
     return res
+
+
+def _slot(holder, which):
+    from pyscenedetect_b200.engine import SlotView
+    return getattr(holder, which) if isinstance(holder, SlotView) else 0
 
 
 def _feed(eng, frames, dev_buf, halo):
@@ -93,40 +132,49 @@ def _feed(eng, frames, dev_buf, halo):
     eng.submit_device(dev_buf.ptr, frames.shape[0] - 40)
 
 
-def test_every_slot_equals_a_one_slot_engine():
+def test_every_slot_holder_equals_a_one_slot_engine():
     from pyscenedetect_b200.engine import F_EDGES, F_HASH, F_HSV, DeviceBuffer, Engine
     from pyscenedetect_b200.scene_manager import shared_engine
+    from pyscenedetect_b200.sweep import PixelGroup
     w, h = 320, 180
     video = _frames(71, w, h, 5)
     second = _frames(30, w, h, 6)
     buf = DeviceBuffer(video.nbytes)
-    passes = [(F_HSV | F_EDGES, k, {}) for k in KS] + [(F_HASH, 0, dict(hash_size=s, hash_lowpass=lp)) for s, lp in GEOS]
-    multi, slots = shared_engine(passes, w, h, w, h, max_batch=8)
-    edge_slots = {k: slots[i][0] for i, k in enumerate(KS)}
-    hash_slots = {g: slots[len(KS) + i][1] for i, g in enumerate(GEOS)}
-    assert list(edge_slots.values()) == list(range(len(KS))) and list(hash_slots.values()) == list(range(len(GEOS)))
+    groups = [PixelGroup(F_HSV | F_EDGES, k, ()) for k in KS] + \
+        [PixelGroup(F_HASH, 0, (("hash_lowpass", lp), ("hash_size", s))) for s, lp in GEOS]
+    multi, holders = shared_engine(groups, w, h, w, h, max_batch=8)
+    edges = dict(zip(KS, holders[:len(KS)]))
+    hashes = dict(zip(GEOS, holders[len(KS):]))
+    assert [_slot(e, "edge_slot") for e in edges.values()] == list(range(len(KS)))
+    assert [_slot(e, "hash_slot") for e in hashes.values()] == list(range(len(GEOS)))
     assert [multi.edge_kernel_size_at(s) for s in range(len(KS))] == list(KS) and multi.edge_kernel_size_at(9) == -1
     _feed(multi, video[1:], buf, video[0])
-    got = _snapshot(multi, edge_slots, hash_slots)
+    got = _snapshot(edges, hashes)
+    # the engine's own slot keywords give what the holders give
+    for s, k in enumerate(KS):
+        assert multi.scan_content(ALL, edge_slot=s)[0].tobytes() == got[("edges", k)][1], k
+    for s, g in enumerate(GEOS):
+        assert multi.read_hash(hash_slot=s).tobytes() == got[("hash", g)][0], g
+        assert multi.scan_hash_dist(hash_slot=s).tobytes() == got[("hash", g)][1], g
     multi.reset()
     multi.submit(second)
-    got2 = _snapshot(multi, edge_slots, hash_slots)
+    got2 = _snapshot(edges, hashes)
     multi.close()
     for k in KS:
         one = Engine(w, h, F_HSV | F_EDGES, max_batch=8, edge_kernel_size=k)
         _feed(one, video[1:], buf, video[0])
-        assert _snapshot(one, {k: 0}, {}) == {key: v for key, v in got.items() if key == ("edges", k)}, k
+        assert _snapshot({k: one}, {}) == {key: v for key, v in got.items() if key == ("edges", k)}, k
         one.reset()
         one.submit(second)
-        assert _snapshot(one, {k: 0}, {})[("edges", k)] == got2[("edges", k)], k
+        assert _snapshot({k: one}, {})[("edges", k)] == got2[("edges", k)], k
         one.close()
     for g in GEOS:
         one = Engine(w, h, F_HASH, max_batch=8, hash_size=g[0], hash_lowpass=g[1])
         _feed(one, video[1:], buf, video[0])
-        assert _snapshot(one, {}, {g: 0})[("hash", g)] == got[("hash", g)], g
+        assert _snapshot({}, {g: one})[("hash", g)] == got[("hash", g)], g
         one.reset()
         one.submit(second)
-        assert _snapshot(one, {}, {g: 0})[("hash", g)] == got2[("hash", g)], g
+        assert _snapshot({}, {g: one})[("hash", g)] == got2[("hash", g)], g
         one.close()
     # the slots saw real edges and hashes
     assert all(np.frombuffer(got[("edges", k)][0], np.uint64).any() for k in KS)

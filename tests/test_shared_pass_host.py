@@ -8,33 +8,45 @@ from ctypes import c_int32 as C_int32
 import numpy as np
 import pytest
 
+from oracle import ref_detectors as R
+from pyscenedetect_b200.engine import Engine, SlotView
 from tests.fake_engine import OracleEngine
 
 ALL = (1.0, 1.0, 1.0, 1.0)
 
 
 class SlotEngine(OracleEngine):
+    """The engine's slot contract: `add_*` returns the slot that already holds the effective kernel size or the
+    geometry, else appends one."""
     made: list = []
 
     def __init__(self, *a, **kw):
         super().__init__(*a, **kw)
         self.config = (kw.get("edge_kernel_size", 0), kw.get("hash_size"), kw.get("hash_lowpass"))
+        self._edge_sizes = [self._effective(self.config[0])]
+        self._geometries = [(self.hash_size, self.hash_lowpass)]
         self.added_edges, self.added_hashes, self.scans = [], [], []
         SlotEngine.made.append(self)
 
+    def _effective(self, k):
+        return k or R.estimated_kernel_size(self.width, self.height)
+
     def add_edge_kernel_size(self, k):
         assert self.frame_count == 0
-        self.added_edges.append(k)
-        return len(self.added_edges)
+        k = self._effective(k)
+        if k not in self._edge_sizes:
+            self._edge_sizes.append(k)
+            self.added_edges.append(k)
+        return self._edge_sizes.index(k)
 
     def add_hash_geometry(self, size, lowpass):
         assert self.frame_count == 0
-        self.added_hashes.append((size, lowpass))
-        return len(self.added_hashes)
+        if (size, lowpass) not in self._geometries:
+            self._geometries.append((size, lowpass))
+            self.added_hashes.append((size, lowpass))
+        return self._geometries.index((size, lowpass))
 
-    def view(self, edge_slot=0, hash_slot=0):
-        from pyscenedetect_b200.engine import SlotView
-        return SlotView(self, edge_slot, hash_slot)
+    view = Engine.view
 
     def scan_content(self, weights, first=0, n=None, edge_slot=0):
         self.scans.append(("content", edge_slot))
@@ -43,6 +55,15 @@ class SlotEngine(OracleEngine):
     def scan_hash_dist(self, first=0, n=None, hash_slot=0):
         self.scans.append(("hash", hash_slot))
         return super().scan_hash_dist(first, n)
+
+
+def _slots(d):
+    """(edge slot, hash slot) of the holder a detector is attached to: a view, or the engine itself for 0 / 0"""
+    (eng,) = SlotEngine.made
+    if d._engine is eng:
+        return 0, 0
+    assert isinstance(d._engine, SlotView) and d._engine._engine is eng
+    return d._engine.edge_slot, d._engine.hash_slot
 
 
 @pytest.fixture
@@ -68,7 +89,7 @@ def _run(dets, w=640, h=360, stats=True, n=6):
     return sm
 
 
-def test_kernel_sizes_deduplicate_automatic_and_explicit(patched):
+def test_engine_deduplicates_automatic_and_explicit_kernel_sizes(patched):
     from pyscenedetect_b200.detectors import AdaptiveDetector, ContentDetector
     # 640x360 is auto-downscaled to 256x144, where the automatic kernel size is 5
     dets = [ContentDetector(kernel_size=5), AdaptiveDetector(), ContentDetector(weights=ALL, kernel_size=7),
@@ -77,20 +98,20 @@ def test_kernel_sizes_deduplicate_automatic_and_explicit(patched):
     (eng,) = patched.made
     assert eng.config[0] == 5                 # the first edge detector's argument configures slot 0
     assert eng.added_edges == [7, 3]          # then every other effective size, in detector order
-    assert [d._edge_slot for d in dets] == [0, 0, 1, 1, 2]
+    assert [_slots(d)[0] for d in dets] == [0, 0, 1, 1, 2]
     assert {s for kind, s in eng.scans if kind == "content"} == {0, 1, 2}
 
 
-def test_automatic_first_then_its_explicit_twin(patched):
+def test_automatic_first_then_its_explicit_twin_shares_slot_0(patched):
     from pyscenedetect_b200.detectors import AdaptiveDetector, ContentDetector
     dets = [AdaptiveDetector(), ContentDetector(kernel_size=5), ContentDetector(kernel_size=9)]
     _run(dets)
     (eng,) = patched.made
     assert eng.config[0] == 0 and eng.added_edges == [9]
-    assert [d._edge_slot for d in dets] == [0, 0, 1]
+    assert [_slots(d)[0] for d in dets] == [0, 0, 1]
 
 
-def test_edge_free_detectors_do_not_take_slots(patched):
+def test_edge_free_detectors_take_no_edge_slot(patched):
     from pyscenedetect_b200.detectors import ContentDetector
     # without a StatsManager a ContentDetector with edge weight 0 has no edge component: its kernel size is moot
     dets = [ContentDetector(kernel_size=9), ContentDetector(weights=ALL, kernel_size=3),
@@ -98,10 +119,10 @@ def test_edge_free_detectors_do_not_take_slots(patched):
     _run(dets, stats=False)
     (eng,) = patched.made
     assert eng.config[0] == 3 and eng.added_edges == [5]
-    assert [d._edge_slot for d in dets] == [0, 0, 1]
+    assert [_slots(d)[0] for d in dets] == [0, 0, 1]
 
 
-def test_hash_geometries_in_detector_order(patched):
+def test_hash_geometry_slots_in_detector_order(patched):
     from pyscenedetect_b200.detectors import HashDetector, HistogramDetector
     dets = [HashDetector(size=16), HistogramDetector(), HashDetector(), HashDetector(size=8, lowpass=3),
             HashDetector(size=16, threshold=0.2)]
@@ -109,7 +130,7 @@ def test_hash_geometries_in_detector_order(patched):
     (eng,) = patched.made
     assert eng.config[1:] == (16, 2)
     assert eng.added_hashes == [(8, 2), (8, 3)]
-    assert [d._hash_slot for d in dets] == [0, 0, 1, 2, 0]
+    assert [_slots(d)[1] for d in dets] == [0, 0, 1, 2, 0]
     assert {s for kind, s in eng.scans if kind == "hash"} == {0, 1, 2}
 
 
@@ -120,14 +141,6 @@ def test_one_size_one_geometry_adds_no_slot(patched):
     (eng,) = patched.made
     assert eng.added_edges == [] and eng.added_hashes == []
     assert all(d._engine is eng for d in dets)   # slot 0 everywhere: the engine itself, no view
-
-
-def test_effective_kernel_size_matches_the_reference_estimate():
-    from oracle import ref_detectors as R
-    from pyscenedetect_b200.engine import effective_kernel_size
-    for w, h in ((256, 144), (133, 99), (160, 90), (640, 360), (1920, 1080), (3840, 2160), (1, 1), (500, 499)):
-        assert effective_kernel_size(0, w, h) == R.estimated_kernel_size(w, h), (w, h)
-        assert effective_kernel_size(7, w, h) == 7
 
 
 def test_c_abi_slot_calls_reject_null_engines():

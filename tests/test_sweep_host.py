@@ -129,9 +129,12 @@ class _Eng:
     def device_hash(self):
         return 3
 
+    def device_edge_sads(self):
+        return None
+
 
 @pytest.mark.parametrize("det", ["content", "adaptive", "threshold", "histogram", "hash"])
-def test_cell_arguments_equal_cuts_for_detector(golden, monkeypatch, det):
+def test_cell_arguments_equal_device_cuts_launches(golden, monkeypatch, det):
     from pyscenedetect_b200 import device_cuts
     from pyscenedetect_b200.sweep import ParameterSweep
     monkeypatch.setattr(device_cuts, "DeviceBuffer", _Buf)
@@ -150,11 +153,11 @@ def test_cell_arguments_equal_cuts_for_detector(golden, monkeypatch, det):
             c, calls = sw.cells[k], rec.calls
             mf = c.min_frames(fps)
             if det == "content":
-                assert list(calls["psd_scan_content"][3]) == [float(x) for x in c.metric[2]]
+                assert list(calls["psd_scan_content_edges"][4]) == [float(x) for x in c.metric[2]]
                 assert calls["psd_scan_compare"][2] == c.threshold
                 assert calls["psd_cuts_flash_filter"][3:5] == (mf, c.mode)
             elif det == "adaptive":
-                assert list(calls["psd_scan_content"][3]) == [float(x) for x in c.metric2[2]]
+                assert list(calls["psd_scan_content_edges"][4]) == [float(x) for x in c.metric2[2]]
                 assert calls["psd_scan_adaptive"][2:4] == (c.window, c.min_content_val) == c.metric[3:5]
                 assert calls["psd_cuts_adaptive"][4:8] == (c.window, c.threshold, c.min_content_val, mf)
             elif det == "histogram":
