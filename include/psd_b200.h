@@ -51,6 +51,18 @@ extern "C" {
 
 typedef struct psd_engine psd_engine;
 
+/* Where the bytes of n frames of 8-bit B, G, R samples lie, in signed byte strides from a base pointer that
+ * addresses channel B of pixel (0,0) of frame 0: channel c (0 = B, 1 = G, 2 = R) of pixel (x,y) of frame f is at
+ * base + f*frame_stride + y*row_stride + x*pixel_stride + c*channel_stride.
+ *   packed BGR24:          {H*3W, 3W, 3, 1}
+ *   packed RGB24:          base = R byte + 2, {H*3W, 3W, 3, -1}
+ *   planar RGB (NCHW):     base = B plane, {3HW, W, 1, -HW}
+ * A crop is a base offset with the same strides, frame skipping multiplies frame_stride, and a zero stride
+ * repeats a frame (a broadcast view). */
+typedef struct psd_frame_layout {
+    int64_t frame_stride, row_stride, pixel_stride, channel_stride;
+} psd_frame_layout;
+
 /* Engine configuration.  (src_width,src_height) is the size of the frames submitted;
  * (width,height) the size the detectors score at.  If they differ the engine applies the
  * exact cv2.resize(..., INTER_LINEAR) fixed-point bilinear of scene_manager.py:670-678. */
@@ -121,6 +133,14 @@ int psd_engine_submit_host(psd_engine* e, const uint8_t* bgr, int64_t n_frames,
  * The memory must stay valid until psd_engine_sync(). */
 int psd_engine_submit_device(psd_engine* e, const void* dptr, int64_t n_frames,
                              int64_t frame_stride);
+/* Score n frames of device (or managed) memory on the engine's device in any layout (psd_frame_layout): packed
+ * 16-byte-aligned BGR is read in place, a resizing engine reads the 2x2 taps of each output pixel straight from
+ * the layout, anything else is first gathered to packed BGR (psd_gather_bgr) max_batch frames at a time.
+ * PSD_ERR_INVALID for host memory or memory of another device.  The work is queued on the engine's compute
+ * stream (psd_engine_compute_stream), which does not wait for any other stream: make it wait for the producer
+ * of the frames first.  The memory must stay valid until psd_engine_sync(). */
+int psd_engine_submit_device_layout(psd_engine* e, const void* base, int64_t n_frames,
+                                    const psd_frame_layout* layout);
 int psd_engine_sync(psd_engine* e);
 /* the engine's compute stream (cudaStream_t): launch the psd_scan_* kernels (or record events)
  * on it to stay ordered after the engine's own kernels */
@@ -286,6 +306,12 @@ int psd_engine_scan_hash_dist_host_at(psd_engine* e, int32_t hash_slot, int64_t 
 /* params_host: [n][24] int32 rows of ScenePlan.params for frames first..first+n-1 */
 int psd_synth_frames(int device, void* d_out, const int32_t* params_host, int64_t n, int32_t width,
                      int32_t height, int64_t frame_stride, void* stream);
+
+/* ---- layout conversion ---- */
+/* n frames of width x height in `layout` at device (or managed) memory `base` -> packed BGR24 at device memory
+ * dst, dst_frame_stride bytes apart; queued on `stream` (a cudaStream_t or NULL), not waited for */
+int psd_gather_bgr(int device, const void* base, const psd_frame_layout* layout, int64_t n, int32_t width,
+                   int32_t height, void* dst, int64_t dst_frame_stride, void* stream);
 
 /* ---- test hooks ---- */
 /* device BGR (n pixels, a multiple of 16) -> H,S,V and Y planes with the device functions the fused pass uses */

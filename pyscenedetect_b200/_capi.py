@@ -53,6 +53,16 @@ class PsdConfig(C.Structure):
     ]
 
 
+class PsdFrameLayout(C.Structure):
+    """psd_frame_layout: signed byte strides of frames whose base pointer addresses channel B of pixel (0,0)."""
+    _fields_ = [
+        ("frame_stride", C.c_int64),
+        ("row_stride", C.c_int64),
+        ("pixel_stride", C.c_int64),
+        ("channel_stride", C.c_int64),
+    ]
+
+
 SWEEP_CONTENT = 0
 SWEEP_ADAPTIVE = 1
 SWEEP_THRESHOLD = 2
@@ -117,6 +127,7 @@ SIGNATURES = {
     "psd_engine_set_halo_device": (C.c_int, [_vp, _vp]),
     "psd_engine_submit_host": (C.c_int, [_vp, _vp, _i64, _i64, _i64, _u32]),
     "psd_engine_submit_device": (C.c_int, [_vp, _vp, _i64, _i64]),
+    "psd_engine_submit_device_layout": (C.c_int, [_vp, _vp, _i64, C.POINTER(PsdFrameLayout)]),
     "psd_engine_sync": (C.c_int, [_vp]),
     "psd_engine_compute_stream": (_vp, [_vp]),
     "psd_engine_frame_count": (_i64, [_vp]),
@@ -159,6 +170,7 @@ SIGNATURES = {
     "psd_engine_scan_content_host_at": (C.c_int, [_vp, _i32, _i64, _i64, _dp, _dbl, _vp, _vp]),
     "psd_engine_scan_hash_dist_host_at": (C.c_int, [_vp, _i32, _i64, _i64, _vp]),
     "psd_synth_frames": (C.c_int, [C.c_int, _vp, _vp, _i64, _i32, _i32, _i64, _vp]),
+    "psd_gather_bgr": (C.c_int, [C.c_int, _vp, C.POINTER(PsdFrameLayout), _i64, _i32, _i32, _vp, _i64, _vp]),
     "psd_test_hsv": (C.c_int, [C.c_int, _vp, _i64, _vp, _vp, _vp, _vp]),
 }
 

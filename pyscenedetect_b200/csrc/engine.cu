@@ -160,27 +160,37 @@ static cudaEvent_t next_event(psd_engine* e) {
     return e->ev_pool[e->ev_next++];
 }
 
-// Score `n` tightly-packed-row frames at `src` (source size) that are visible to compute_stream.
+static psd_frame_layout packed_layout(const psd_engine* e, int64_t frame_stride) {
+    return psd_frame_layout{frame_stride, (int64_t)e->sw * 3, 3, 1};
+}
+
+// the fused pass reads the frames where they are: packed BGR, a frame apart or more, 16-byte aligned
+static bool reads_in_place(const psd_engine* e, const uint8_t* src, const psd_frame_layout& l) {
+    return !e->resize && layout_packed_bgr(l, e->sw) && l.frame_stride >= e->src_frame_bytes &&
+           (((uintptr_t)src | (uintptr_t)l.frame_stride) & 15) == 0;
+}
+
+// Score `n` frames at `src` (source size, in layout `l`) that are visible to compute_stream: resized from the
+// layout, read in place, or gathered to packed BGR in `small` first (n <= max_batch unless read in place).
 // slot0: result slot of the first frame (0 = halo slot).
-static int run_batch(psd_engine* e, const uint8_t* src, int64_t src_frame_stride, int64_t n,
+static int run_batch(psd_engine* e, const uint8_t* src, const psd_frame_layout& l, int64_t n,
                      int64_t slot0, bool is_halo) {
     cudaStream_t st = e->compute_stream;
     cudaEvent_t t0 = next_event(e), t1 = next_event(e), k0 = next_event(e), k1 = next_event(e);
     if (!t0 || !t1 || !k0 || !k1) { set_error("cudaEventCreate failed"); return PSD_ERR_CUDA; }
     PSD_CUDA(cudaEventRecord(t0, st));
     const uint8_t* scored = src;
-    int64_t scored_stride = src_frame_stride;
+    int64_t scored_stride = l.frame_stride;
     if (e->resize) {
         ResizeTaps taps{e->d_xofs, e->d_xa, e->d_yofs, e->d_ya};
-        int rc = launch_resize(src, src_frame_stride, (int64_t)e->sw * 3, e->sw, e->sh, e->small, e->small_stride,
-                               e->W, e->H, n, taps, st);
+        int rc = launch_resize(src, l, e->sw, e->sh, e->small, e->small_stride, e->W, e->H, n, taps, st);
         if (rc) return rc;
         scored = e->small;
         scored_stride = e->small_stride;
-    } else if (((uintptr_t)src | (uintptr_t)src_frame_stride) & 15) {
+    } else if (!reads_in_place(e, src, l)) {
         if (!e->small) PSD_CUDA(cudaMalloc(&e->small, (size_t)e->small_stride * e->max_batch));
-        PSD_CUDA(cudaMemcpy2DAsync(e->small, (size_t)e->small_stride, src, (size_t)src_frame_stride,
-                                   (size_t)e->frame_bytes, (size_t)n, cudaMemcpyDeviceToDevice, st));
+        int rc = launch_gather(src, l, n, e->sw, e->sh, e->small, e->small_stride, st);
+        if (rc) return rc;
         scored = e->small;
         scored_stride = e->small_stride;
     }
@@ -519,7 +529,7 @@ int psd_engine_set_halo_device(psd_engine* e, const void* dptr) {
     PSD_REQUIRE(e->n_frames == 0, "halo must be set before the first frame is submitted");
     PSD_CUDA(cudaSetDevice(e->device));
     e->have_carry = false;
-    int rc = run_batch(e, (const uint8_t*)dptr, e->src_frame_bytes, 1, 0, true);
+    int rc = run_batch(e, (const uint8_t*)dptr, packed_layout(e, e->src_frame_bytes), 1, 0, true);
     if (rc) return rc;
     e->halo_scored = true;
     return PSD_OK;
@@ -542,26 +552,50 @@ int psd_engine_set_halo_host(psd_engine* e, const uint8_t* bgr, int64_t row_pitc
     return PSD_OK;
 }
 
+// PSD_OK if p is device or managed memory of `device`
+static int require_device_memory(const void* p, int device, const char* what) {
+    cudaPointerAttributes at{};
+    if (cudaPointerGetAttributes(&at, p) != cudaSuccess) {
+        cudaGetLastError();
+        set_error("%s: %p is not CUDA memory", what, p);
+        return PSD_ERR_INVALID;
+    }
+    PSD_REQUIRE(at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged,
+                "%s: %p is not device or managed memory", what, p);
+    PSD_REQUIRE(at.device == device, "%s: %p is memory of device %d, not of device %d", what, p, at.device, device);
+    return PSD_OK;
+}
+
 int psd_engine_submit_device(psd_engine* e, const void* dptr, int64_t n, int64_t frame_stride) {
     PSD_REQUIRE(e && dptr, "psd_engine_submit_device: null argument");
-    PSD_REQUIRE(n >= 0, "negative frame count");
     PSD_REQUIRE(frame_stride >= e->src_frame_bytes, "frame_stride smaller than a frame");
-    if (n == 0) return PSD_OK;
+    const psd_frame_layout l = packed_layout(e, frame_stride);
+    return psd_engine_submit_device_layout(e, dptr, n, &l);
+}
+
+int psd_engine_submit_device_layout(psd_engine* e, const void* base, int64_t n, const psd_frame_layout* layout) {
+    PSD_REQUIRE(e && layout, "psd_engine_submit_device_layout: null argument");
+    PSD_REQUIRE(n >= 0, "negative frame count");
+    if (n == 0) return PSD_OK;  // an empty array may have no data pointer at all
+    PSD_REQUIRE(base, "psd_engine_submit_device_layout: null frames");
     PSD_CUDA(cudaSetDevice(e->device));
-    int rc = ensure_capacity(e, e->n_frames + n + 1);
+    int rc = require_device_memory(base, e->device, "psd_engine_submit_device_layout");
     if (rc) return rc;
-    const uint8_t* p = (const uint8_t*)dptr;
-    // Frames the fused pass can read where they are (no resize, no edge or hash scratch, 16-byte aligned) are
-    // scored in one launch: max_batch only sizes staging and those per-batch buffers, and every launch costs a
-    // pipeline fill and drain and a work split whose busiest SM sets the launch's time.  Only the kernels'
-    // int32 frame counts limit such a batch (2^30 keeps their grid arithmetic clear of overflow too).
-    const bool in_place = !e->resize && !(e->features & (PSD_F_EDGES | PSD_F_HASH)) &&
-                          (((uintptr_t)p | (uintptr_t)frame_stride) & 15) == 0;
+    rc = ensure_capacity(e, e->n_frames + n + 1);
+    if (rc) return rc;
+    const uint8_t* p = (const uint8_t*)base;
+    const psd_frame_layout l = *layout;
+    // Frames the fused pass can read where they are (no resize, no edge or hash scratch, packed and 16-byte
+    // aligned) are scored in one launch: max_batch only sizes staging and those per-batch buffers, and every launch
+    // costs a pipeline fill and drain and a work split whose busiest SM sets the launch's time.  Only the kernels'
+    // int32 frame counts limit such a batch (2^30 keeps their grid arithmetic clear of overflow too).  Every other
+    // batch is resized or gathered into max_batch frames of scratch.
+    const bool in_place = !(e->features & (PSD_F_EDGES | PSD_F_HASH)) && reads_in_place(e, p, l);
     const int64_t batch = in_place ? ((int64_t)1 << 30) : (int64_t)e->max_batch;
     int64_t done = 0;
     while (done < n) {
         const int64_t b = (n - done < batch) ? (n - done) : batch;
-        rc = run_batch(e, p + done * frame_stride, frame_stride, b, e->n_frames + 1, false);
+        rc = run_batch(e, p + done * l.frame_stride, l, b, e->n_frames + 1, false);
         if (rc) return rc;
         e->n_frames += b;
         done += b;
@@ -588,7 +622,7 @@ int psd_engine_submit_host(psd_engine* e, const uint8_t* bgr, int64_t n, int64_t
         e->next_slot ^= 1;
         rc = stage_host(e, bgr + done * frame_stride, b, frame_stride, row_pitch, flags, slot);
         if (rc) return rc;
-        rc = run_batch(e, e->dev_stage[slot], e->src_frame_bytes, b, e->n_frames + 1, false);
+        rc = run_batch(e, e->dev_stage[slot], packed_layout(e, e->src_frame_bytes), b, e->n_frames + 1, false);
         if (rc) return rc;
         PSD_CUDA(cudaEventRecord(e->slot_free[slot], e->compute_stream));
         e->n_frames += b;
@@ -905,6 +939,21 @@ int psd_synth_frames(int device, void* d_out, const int32_t* params_host, int64_
     }
     if (!rc && cudaStreamSynchronize((cudaStream_t)stream) != cudaSuccess) { set_error("synth sync failed: %s", cudaGetErrorString(cudaGetLastError())); rc = PSD_ERR_CUDA; }
     cudaFree(d_params);
+    return rc;
+}
+
+int psd_gather_bgr(int device, const void* base, const psd_frame_layout* layout, int64_t n, int32_t width,
+                   int32_t height, void* dst, int64_t dst_frame_stride, void* stream) {
+    PSD_REQUIRE(layout, "psd_gather_bgr: null layout");
+    PSD_REQUIRE(n >= 0 && width > 0 && height > 0, "psd_gather_bgr: bad frame count or size");
+    if (n == 0) return PSD_OK;
+    PSD_REQUIRE(base && dst, "psd_gather_bgr: null frames");
+    PSD_REQUIRE(n <= 1 || dst_frame_stride >= (int64_t)width * height * 3, "dst_frame_stride smaller than a frame");
+    PSD_CUDA(cudaSetDevice(device));
+    int rc = require_device_memory(base, device, "psd_gather_bgr source");
+    if (!rc) rc = require_device_memory(dst, device, "psd_gather_bgr destination");
+    if (!rc) rc = launch_gather((const uint8_t*)base, *layout, n, width, height, (uint8_t*)dst, dst_frame_stride,
+                                (cudaStream_t)stream);
     return rc;
 }
 

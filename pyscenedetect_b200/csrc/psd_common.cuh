@@ -70,9 +70,17 @@ struct ResizeTaps {  // device arrays built on the host exactly as OpenCV builds
     const int32_t* yofs;  // [dh]
     const int16_t* ya;    // [dh][2]
 };
-int launch_resize(const uint8_t* src, int64_t src_frame_stride, int64_t src_row_pitch, int sw, int sh,
-                  uint8_t* dst, int64_t dst_frame_stride, int dw, int dh, int64_t n, const ResizeTaps& taps,
-                  cudaStream_t stream);
+int launch_resize(const uint8_t* src, const psd_frame_layout& layout, int sw, int sh, uint8_t* dst,
+                  int64_t dst_frame_stride, int dw, int dh, int64_t n, const ResizeTaps& taps, cudaStream_t stream);
+
+// ---- layout gather (gather_kernel.cu) ----
+// n frames of w x h in `layout` -> packed BGR24, dst_frame_stride apart (no argument checks: callers validate)
+int launch_gather(const uint8_t* src, const psd_frame_layout& layout, int64_t n, int w, int h, uint8_t* dst,
+                  int64_t dst_frame_stride, cudaStream_t stream);
+// the layout is packed BGR24 rows (3 bytes per pixel, B first, rows 3*w bytes apart)
+inline bool layout_packed_bgr(const psd_frame_layout& l, int w) {
+    return l.pixel_stride == 3 && l.channel_stride == 1 && l.row_stride == 3 * (int64_t)w;
+}
 
 // ---- edge path (edge_kernels.cu) ----
 struct EdgeBuffers {

@@ -7,6 +7,7 @@ from dataclasses import dataclass
 
 import numpy as np
 
+from .. import _dlpack
 from .._capi import F_EDGES
 from ..compat import SceneDetector
 from ..engine import Engine
@@ -33,6 +34,14 @@ def pixel_group_of(detector) -> PixelGroup:
     feats = detector.required_features()
     return PixelGroup(feats, detector.edge_kernel_size_arg() if feats & F_EDGES else 0,
                       tuple(sorted(detector.engine_kwargs().items())))
+
+
+def frame_format(frames, device: int = 0) -> tuple[tuple, bool]:
+    """(shape, whether the samples are uint8) of numpy frames, or of CUDA frames of `device` read from their DLPack
+    view (ValueError for frames on another device)."""
+    if _dlpack.is_dlpack(frames):
+        return _dlpack.frame_format(frames, device)
+    return frames.shape, frames.dtype == np.uint8
 
 
 class EngineDetector(SceneDetector):
@@ -81,9 +90,9 @@ class EngineDetector(SceneDetector):
         self._owns_engine = False
         self._base_index = holder.frame_count
 
-    def _ensure_engine(self, frames: np.ndarray) -> Engine:
+    def _ensure_engine(self, frames) -> Engine:
         if self._engine is None:
-            h, w = frames.shape[-3], frames.shape[-2]
+            h, w = frame_format(frames, self._device)[0][-3:-1]
             sw, sh = self._scored_size if self._scored_size else (w, h)
             self._engine = pixel_group_of(self).make_engine(w, h, sw, sh, device=self._device,
                                                             max_batch=self._max_batch)
@@ -91,10 +100,18 @@ class EngineDetector(SceneDetector):
             self._base_index = 0
         return self._engine
 
+    def _frames_device(self) -> int:
+        """The CUDA device that device frames must be on: the engine's."""
+        return getattr(self._engine, "device", self._device)
+
     @staticmethod
-    def _as_batch(frame_img) -> np.ndarray:
+    def _as_batch(frame_img):
+        """A numpy frame or batch as a batch; CUDA frames (any DLPack exporter) as they are: `Engine.submit` takes
+        one frame or a batch."""
+        if _dlpack.is_dlpack(frame_img):
+            return frame_img
         if not isinstance(frame_img, np.ndarray):
-            raise ValueError("frame_img must be a numpy.ndarray")
+            raise ValueError("frame_img must be a numpy.ndarray or a CUDA array that exports DLPack")
         return frame_img[None] if frame_img.ndim == 3 else frame_img
 
     # -- the two entry points --
@@ -120,7 +137,7 @@ class EngineDetector(SceneDetector):
         (frames [first, first+len(timecodes)) ) - used by the multi-GPU gather path."""
         return self._consume(list(timecodes), first)
 
-    def _validate(self, frames: np.ndarray) -> None:
+    def _validate(self, frames) -> None:
         pass
 
     def _consume(self, timecodes: list, first: int) -> list:  # pragma: no cover - abstract

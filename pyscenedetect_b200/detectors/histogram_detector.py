@@ -7,7 +7,7 @@ import typing as ty
 import numpy as np
 
 from .._capi import F_YHIST
-from ._base import EngineDetector
+from ._base import EngineDetector, frame_format
 
 
 class HistogramDetector(EngineDetector):
@@ -31,10 +31,11 @@ class HistogramDetector(EngineDetector):
     def get_metrics(self) -> list[str]:
         return [self._metric_key]
 
-    def _validate(self, frames: np.ndarray) -> None:
-        if frames.dtype != np.uint8:
+    def _validate(self, frames) -> None:
+        shape, uint8 = frame_format(frames, self._frames_device())
+        if not uint8:
             raise ValueError("Image must be 8-bit rgb for HistogramDetector")
-        if frames.shape[-1] != 3:
+        if shape[-1] != 3:
             raise ValueError("Image must have three color channels for HistogramDetector")
 
     def set_halo(self, frame_img: np.ndarray) -> None:

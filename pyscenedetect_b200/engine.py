@@ -7,7 +7,7 @@ import ctypes as C
 
 import numpy as np
 
-from . import _capi
+from . import _capi, _dlpack
 from ._capi import F_BGRSUM, F_EDGES, F_HASH, F_HSV, F_YHIST, SUMS_DTYPE, check, hash_words
 
 
@@ -99,12 +99,18 @@ class Engine:
         self.max_batch = int(max_batch)
         self.n_pixels = self.width * self.height
         self.src_frame_bytes = self.src_width * self.src_height * 3
+        self._held = []  # DLPack capsules of submitted device frames, released once the engine has synchronised
+
+    def _synced(self):
+        """The compute stream has finished everything queued so far: the device frames submitted can go."""
+        self._held.clear()
 
     # -- lifetime --
     def close(self):
         if getattr(self, "_h", None) is not None and self._h.value:
             self._lib.psd_engine_destroy(self._h)
             self._h = None
+            self._synced()
 
     def __del__(self):
         try:
@@ -114,6 +120,7 @@ class Engine:
 
     def reset(self):
         check(self._lib.psd_engine_reset(self._h), "psd_engine_reset")
+        self._synced()
 
     # -- input --
     def _check_frames(self, frames: np.ndarray) -> np.ndarray:
@@ -139,8 +146,31 @@ class Engine:
     def set_halo_device(self, dptr: int):
         check(self._lib.psd_engine_set_halo_device(self._h, dptr), "psd_engine_set_halo_device")
 
-    def submit(self, frames: np.ndarray, pinned: bool = False):
-        """Score a batch of host frames (N,H,W,3) uint8; strided views (crop) are honoured."""
+    def submit(self, frames, pinned: bool = False, channel_order: str = "bgr"):
+        """Score a batch of frames (N,H,W,3) or one frame (H,W,3), uint8: a numpy array in host memory, or CUDA
+        memory of this engine's device from any DLPack exporter (a torch tensor, say), of any strides (a crop, a
+        frame step, `nchw.permute(0, 2, 3, 1)`).  `channel_order` "rgb": the last axis is R, G, B.
+
+        Device frames are read on the engine's compute stream after the exporter's current stream has reached
+        this call (the DLPack stream handshake), and must not be overwritten until the engine has synchronised
+        (`sync()` or any read or host scan): the engine keeps a reference until then.  torch exports a CUDA tensor
+        only while its device is torch's current device (`torch.cuda.set_device`); any refusal of the exporter
+        raises ValueError, as do frames on another device than the engine's."""
+        if _dlpack.is_dlpack(frames):
+            v = _dlpack.import_frames(frames, stream=self.compute_stream, device=self.device,
+                                      channel_order=channel_order)
+            if (v.width, v.height) != (self.src_width, self.src_height):
+                raise ValueError(f"frame size {v.width}x{v.height} does not match engine "
+                                 f"{self.src_width}x{self.src_height}")
+            layout = _capi.PsdFrameLayout(*v.layout)
+            check(self._lib.psd_engine_submit_device_layout(self._h, v.base, v.n, C.byref(layout)),
+                  "psd_engine_submit_device_layout")
+            self._held.append(v.capsule)
+            return
+        if channel_order not in ("bgr", "rgb"):
+            raise ValueError(f"channel_order must be 'bgr' or 'rgb', not {channel_order!r}")
+        if channel_order == "rgb" and isinstance(frames, np.ndarray):
+            frames = frames[..., ::-1]
         f = self._check_frames(frames)
         n = f.shape[0]
         fs = f.strides[0] if n > 1 else f.strides[1] * self.src_height
@@ -155,6 +185,7 @@ class Engine:
 
     def sync(self):
         check(self._lib.psd_engine_sync(self._h), "psd_engine_sync")
+        self._synced()
 
     @property
     def compute_stream(self) -> int:
@@ -210,12 +241,14 @@ class Engine:
         n = self.frame_count - first if n is None else n
         out = np.zeros(n, dtype=SUMS_DTYPE)
         check(self._lib.psd_engine_read_sums(self._h, first, n, out.ctypes.data), "psd_engine_read_sums")
+        self._synced()
         return out
 
     def read_yhist(self, first: int = 0, n: int | None = None) -> np.ndarray:
         n = self.frame_count - first if n is None else n
         out = np.zeros((n, 256), dtype=np.uint32)
         check(self._lib.psd_engine_read_yhist(self._h, first, n, out.ctypes.data), "psd_engine_read_yhist")
+        self._synced()
         return out
 
     def read_hash(self, first: int = 0, n: int | None = None, hash_slot: int = 0) -> np.ndarray:
@@ -225,6 +258,7 @@ class Engine:
         out = np.zeros((n, hash_words(self.hash_size_at(hash_slot))), dtype=np.uint64)
         check(self._lib.psd_engine_read_hash_at(self._h, int(hash_slot), first, n, out.ctypes.data),
               "psd_engine_read_hash")
+        self._synced()
         return out
 
     def device_hash(self, hash_slot: int = 0) -> int | None:
@@ -249,6 +283,8 @@ class Engine:
         check(self._lib.psd_engine_scan_content_host_at(self._h, int(edge_slot), first, n, w, wsum,
                                                         comps.ctypes.data, val.ctypes.data),
               "psd_engine_scan_content_host")
+        if n:
+            self._synced()
         return val, comps
 
     def scan_adaptive(self, scores: np.ndarray, window_width: int, min_content_val: float) -> np.ndarray:
@@ -257,6 +293,8 @@ class Engine:
         check(self._lib.psd_engine_scan_adaptive_host(self._h, s.ctypes.data, s.shape[0],
                                                       int(window_width), float(min_content_val),
                                                       out.ctypes.data), "psd_engine_scan_adaptive_host")
+        if out.shape[0]:
+            self._synced()
         return out
 
     def scan_average(self, first: int = 0, n: int | None = None) -> np.ndarray:
@@ -264,6 +302,8 @@ class Engine:
         out = np.zeros(n, dtype=np.float64)
         check(self._lib.psd_engine_scan_average_host(self._h, first, n, out.ctypes.data),
               "psd_engine_scan_average_host")
+        if out.shape[0]:
+            self._synced()
         return out
 
     def scan_hist_correl(self, bins: int, first: int = 0, n: int | None = None) -> np.ndarray:
@@ -271,6 +311,8 @@ class Engine:
         out = np.zeros(n, dtype=np.float64)
         check(self._lib.psd_engine_scan_hist_correl_host(self._h, first, n, int(bins), out.ctypes.data),
               "psd_engine_scan_hist_correl_host")
+        if out.shape[0]:
+            self._synced()
         return out
 
     def scan_hash_dist(self, first: int = 0, n: int | None = None, hash_slot: int = 0) -> np.ndarray:
@@ -279,6 +321,8 @@ class Engine:
         out = np.zeros(n, dtype=np.float64)
         check(self._lib.psd_engine_scan_hash_dist_host_at(self._h, int(hash_slot), first, n, out.ctypes.data),
               "psd_engine_scan_hash_dist_host")
+        if out.shape[0]:
+            self._synced()
         return out
 
     # -- instrumentation --
@@ -371,5 +415,38 @@ def synth_frames_device(dptr: int, params: np.ndarray, width: int, height: int,
           "psd_synth_frames")
 
 
-__all__ = ["Engine", "SlotView", "PinnedBuffer", "DeviceBuffer", "synth_frames_device", "bind_host_to_gpu_numa_node", "F_HSV", "F_BGRSUM",
-           "F_YHIST", "F_EDGES", "F_HASH"]
+def gather_bgr(frames, dst: int, dst_frame_stride: int | None = None, channel_order: str = "bgr", device: int = 0,
+               stream: int | None = None):
+    """Copy CUDA frames of any layout (a DLPack exporter, as `Engine.submit` takes them) to packed BGR24 at device
+    pointer `dst`, `dst_frame_stride` bytes apart (default: packed).  Queued on `stream` (cudaStream_t, default
+    the legacy default stream) after the exporter's current stream; returns the imported view, whose capsule must
+    outlive the copy."""
+    v = _dlpack.import_frames(frames, stream=stream or 1, device=device, channel_order=channel_order)
+    layout = _capi.PsdFrameLayout(*v.layout)
+    check(_capi.load().psd_gather_bgr(device, v.base, C.byref(layout), v.n, v.width, v.height, dst,
+                                      int(dst_frame_stride or v.width * v.height * 3), stream),
+          "psd_gather_bgr")
+    return v
+
+
+def download_bgr(frames, channel_order: str = "bgr", device: int = 0,
+                 scratch: DeviceBuffer | None = None) -> np.ndarray:
+    """CUDA frames of any layout -> a host numpy BGR24 array of the same (N,H,W,3) or (H,W,3) shape.  `scratch`: a
+    device buffer of at least the frames' packed size to gather into (default: one allocated and freed here; a
+    reused one spares the cudaFree, which waits for the whole device)."""
+    meta = _dlpack.import_frames(frames, device=device)
+    fb = meta.width * meta.height * 3
+    own = scratch is None or scratch.nbytes < meta.n * fb
+    buf = DeviceBuffer(max(1, meta.n * fb), device) if own else scratch
+    try:
+        gather_bgr(frames, buf.ptr, fb, channel_order, device)
+        out = buf.download(meta.n * fb)   # cudaMemcpy: ordered after the gather on the legacy default stream
+    finally:
+        if own:
+            buf.close()
+    shape = (meta.n, meta.height, meta.width, 3) if meta.ndim == 4 else (meta.height, meta.width, 3)
+    return out.reshape(shape)
+
+
+__all__ = ["Engine", "SlotView", "PinnedBuffer", "DeviceBuffer", "synth_frames_device", "gather_bgr", "download_bgr",
+           "bind_host_to_gpu_numa_node", "F_HSV", "F_BGRSUM", "F_YHIST", "F_EDGES", "F_HASH"]

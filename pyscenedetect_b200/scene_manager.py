@@ -24,10 +24,11 @@ import logging
 
 import numpy as np
 
+from . import _dlpack
 from .compat import FrameTimecode, StatsManager
 from .detectors._base import EngineDetector, pixel_group_of
 from ._capi import F_EDGES, F_HASH
-from .engine import Engine, PinnedBuffer
+from .engine import DeviceBuffer, Engine, PinnedBuffer, download_bgr
 
 DEFAULT_MIN_WIDTH = 256
 logger = logging.getLogger("pyscenedetect_b200")
@@ -88,6 +89,14 @@ class FrameBatches:
     `read_batch` and no crop / frame skip is read zero-copy; otherwise frames are copied into one of two
     page-locked buffers, so that a batch can be gathered while the GPU scores the previous one.
 
+    Frames on the GPU (the stream's or the frames' `__dlpack_device__` says CUDA) never go through the host.  A
+    stream with `read_batch` yields views `[o::frame_skip + 1, y0:y1, x0:x1]` of what it returns; a stream with
+    only `read` yields a list of cropped frame views, which the engine takes one at a time.  Either way the frames,
+    their positions and the frames read past the last one are those of the host path.  Unlike host frames, CUDA
+    frames are not copied as they are read: what `read` / `read_batch` return must stay unchanged until the batch
+    after the one it belongs to has been scored (a decoder that recycles its output surfaces needs a pool of more
+    than two batches, or must return copies).
+
     `next()` returns (timecodes, frames, pinned) or None at the end.  The frames of a batch stay valid until
     the batch after the next one is gathered: the caller must have synchronised the engines that read a batch
     before asking for the batch two after it.  `close()` frees the buffers, after the last batch is done."""
@@ -99,15 +108,43 @@ class FrameBatches:
         self._batch_size = int(batch_size)
         self._frame_skip = frame_skip
         self._end_frame = end_frame
-        self._zero_copy = hasattr(video, "read_batch") and not cropped and frame_skip == 0
+        self._device_views = hasattr(video, "read_batch") and _dlpack.on_cuda(video)
+        self._zero_copy = hasattr(video, "read_batch") and not cropped and frame_skip == 0 and not self._device_views
+        self._start = video.frame_number
         self._pinned = [None, None]
         self._which = 0
         self._done = False
         self._processed = 0
 
+    def _next_views(self):
+        """The next batch of a CUDA stream with `read_batch`: frames start + j * step (step = frame_skip + 1) are
+        processed, each followed by the frame_skip frames it skips; with an end frame, those before it (and the
+        first frame in any case), as the host loop reads them."""
+        video, end_frame, step = self._video, self._end_frame, self._frame_skip + 1
+        x0, y0, x1, y1 = self._box
+        while True:
+            pos = video.frame_number
+            skip = (self._start - pos) % step   # frames still to skip after the last processed one
+            count = self._batch_size
+            if end_frame is not None:
+                count = min(count, max(-(-(end_frame - pos - skip) // step), 1 if self._processed == 0 else 0))
+            want = skip + count * step
+            chunk = video.read_batch(want) if want > 0 else None
+            if chunk is None:
+                self._done = True
+                return None
+            k = len(range(skip, chunk.shape[0], step))
+            if k == 0:
+                continue
+            self._processed += k
+            tcs = [FrameTimecode(pos + skip + j * step, video.frame_rate) for j in range(k)]
+            return tcs, chunk[skip::step, y0:y1, x0:x1], False
+
     def next(self):
         if self._done:
             return None
+        if self._device_views:
+            return self._next_views()
         video, end_frame, zero_copy = self._video, self._end_frame, self._zero_copy
         x0, y0, x1, y1 = self._box
         w, h = self._size
@@ -127,16 +164,21 @@ class FrameBatches:
                     tcs = [FrameTimecode(pos0 + i, fps) for i in range(view.shape[0])]
             else:
                 which = self._which
-                if self._pinned[which] is None:
-                    self._pinned[which] = PinnedBuffer(self._batch_size * w * h * 3)
-                buf = self._pinned[which].array.reshape(self._batch_size, h, w, 3)
+                buf, views = None, []
                 k = 0
                 while k < want:
                     frame = video.read()
                     if frame is False:
                         self._done = True
                         break
-                    np.copyto(buf[k], frame[y0:y1, x0:x1])
+                    if _dlpack.is_dlpack(frame):
+                        views.append(frame[y0:y1, x0:x1])
+                    else:
+                        if buf is None:
+                            if self._pinned[which] is None:
+                                self._pinned[which] = PinnedBuffer(self._batch_size * w * h * 3)
+                            buf = self._pinned[which].array.reshape(self._batch_size, h, w, 3)
+                        np.copyto(buf[k], frame[y0:y1, x0:x1])
                     tcs.append(video.position)
                     k += 1
                     for _ in range(self._frame_skip):  # scene_manager.py:682-685
@@ -145,7 +187,7 @@ class FrameBatches:
                     if end_frame is not None and not (video.position.frame_num + 1) < end_frame:
                         self._done = True
                         break
-                batch = buf[:k] if k else None
+                batch = (views if buf is None else buf[:k]) if k else None
         if batch is None:
             self._done = True
             return None
@@ -178,6 +220,8 @@ class SceneManager:
         self._frame_size = None
         self._frame_buffer_size = 0          # max event_buffer_length of the detectors (scene_manager.py:352)
         self._frame_tail: list = []          # last `_frame_buffer_size` (timecode, frame copy) pairs of the previous batch
+        self._channel_order = "bgr"          # of the frames the stream returns
+        self._scratch: DeviceBuffer | None = None  # one cropped frame: CUDA frames copied out for callbacks
 
     # -- configuration (scene_manager.py:254-335) --
     @property
@@ -316,6 +360,7 @@ class SceneManager:
             end_frame = (self._base_timecode + end_time).frame_num
         elif duration is not None:
             end_frame = ((self._base_timecode + duration) + start_frame_num).frame_num
+        self._channel_order = getattr(video, "channel_order", "bgr")
         gather = FrameBatches(video, (x0, y0, x1, y1), (w, h), self._batch_size, cropped=self._crop is not None,
                               frame_skip=frame_skip, end_frame=end_frame)
         pending = None  # (timecodes, frames_view, first engine index)
@@ -326,7 +371,11 @@ class SceneManager:
             nxt = None
             if batch is not None:
                 first = self._engine.frame_count
-                self._engine.submit(batch, pinned=use_pinned)
+                if isinstance(batch, np.ndarray):
+                    self._engine.submit(batch, pinned=use_pinned)
+                else:  # CUDA frames: a view, or a list of frames from a stream without read_batch
+                    for frames in (batch if isinstance(batch, list) else [batch]):
+                        self._engine.submit(frames, channel_order=self._channel_order)
                 if self._start_pos is None:
                     self._start_pos = tcs[0]
                 self._last_pos = tcs[-1]
@@ -344,15 +393,30 @@ class SceneManager:
             for d in self._detector_list:
                 self._cutting_list += d.post_process(self._last_pos)
         gather.close()
+        if self._scratch is not None:
+            self._scratch.close()
+            self._scratch = None
         return video.frame_number - start_frame_num
 
     def _consume(self, timecodes, frames, first, callback) -> None:
         """Per-frame state machines over one scored batch.  A detector may report a cut up to
         `event_buffer_length` frames behind the frame it is looking at (AdaptiveDetector's window,
         FlashFilter's merge), so callbacks search the tail of the previous batch as well - the
-        reference's `_frame_buffer` (scene_manager.py:422-434)."""
+        reference's `_frame_buffer` (scene_manager.py:422-434).  Callbacks receive numpy BGR frames: CUDA frames
+        are copied out for them (and only for them) through psd_gather_bgr."""
+        on_device = isinstance(frames, list) or _dlpack.is_dlpack(frames)
+
+        def host(frame):
+            if not on_device:
+                return np.array(frame)  # the staging buffer is reused
+            if self._scratch is None:  # reused: freeing device memory would wait for the whole device
+                self._scratch = DeviceBuffer(self._engine.src_frame_bytes, self._engine.device)
+            return download_bgr(frame, self._channel_order, self._engine.device, self._scratch)
+
+        # process_batch only validates the frames of a batch the engine already holds: one stands for a list
+        sample = frames[0] if isinstance(frames, list) else frames
         for d in self._detector_list:
-            cuts = d.process_batch(timecodes, frames, first=first)
+            cuts = d.process_batch(timecodes, sample, first=first)
             self._cutting_list += cuts
             if callback:
                 for cut in cuts:
@@ -361,8 +425,8 @@ class SceneManager:
                             callback(frame, tc)
                     for tc, frame in zip(timecodes, frames):
                         if cut == tc:
-                            callback(frame, tc)
+                            callback(frame if not on_device else host(frame), tc)
         if callback and self._frame_buffer_size > 0:
             k = self._frame_buffer_size
-            tail = [(tc, np.array(f)) for tc, f in list(zip(timecodes, frames))[-k:]]  # the staging buffer is reused
+            tail = [(tc, host(f)) for tc, f in list(zip(timecodes, frames))[-k:]]
             self._frame_tail = (self._frame_tail + tail)[-k:]
