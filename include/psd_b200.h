@@ -317,6 +317,20 @@ int psd_gather_bgr(int device, const void* base, const psd_frame_layout* layout,
 /* device BGR (n pixels, a multiple of 16) -> H,S,V and Y planes with the device functions the fused pass uses */
 int psd_test_hsv(int device, const uint8_t* bgr_host, int64_t n_pixels, uint8_t* h_out, uint8_t* s_out,
                  uint8_t* v_out, uint8_t* y_out);
+/* HashDetector's stages through the engine's hash kernels: n_frames packed BGR24 frames (width x height, frame_stride
+ * bytes apart) in DEVICE memory of `device`, and n_geo (1 to 16) geometries {size, lowpass} in geometries[n_geo][2].
+ * Builds each geometry's plan for n_frames frames and runs the hash pass once.  Host outputs, geometry g's block
+ * after geometry g-1's, n = size * lowpass:
+ *   rowbuf_out [n_frames][height][n] float32: the horizontal pass (raw uint32 column sums where width and height
+ *              are multiples of n), or NULL
+ *   hash_out   [n_frames][PSD_HASH_WORDS_FOR(size)]
+ *   image_out  [n_frames][n][n] float64: the normalised image, or NULL
+ *   low_out    [n_frames][size][size] float32: the low band of the DCT, or NULL
+ * A non-NULL image_out or low_out keeps the finish kernel's working set in global memory for every geometry.  Any of
+ * rowbuf_out, image_out, low_out needs n_frames to fit one sub-batch of every geometry (PSD_ERR_INVALID otherwise). */
+int psd_test_hash_stages(int device, const void* frames, int64_t n_frames, int32_t width, int32_t height,
+                         int64_t frame_stride, const int32_t* geometries, int32_t n_geo, float* rowbuf_out,
+                         uint64_t* hash_out, double* image_out, float* low_out);
 
 #ifdef __cplusplus
 }

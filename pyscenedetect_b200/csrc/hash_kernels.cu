@@ -30,7 +30,8 @@ __device__ __forceinline__ uint32_t gray_word(uint32_t px) {
 // byte -> float32 without the conversion unit: 0x4B000000 | g is 2^23 + g
 __device__ __forceinline__ float byte_to_float(uint32_t g) { return __fadd_rn(__uint_as_float(0x4B000000u | g), -8388608.0f); }
 
-// The horizontal pass.  A CTA takes a block of consecutive source rows of one frame (max(1, 256 / n) of them):
+// The horizontal pass.  A CTA takes a block of consecutive source rows of one frame (max(1, 256 / n) of them, fewer
+// if their gray bytes would not fit kHashRowsSmemBytes):
 //   1. all threads pull the block - it is contiguous in memory - 16 pixels (three 16-byte loads) at a time,
 //      convert to gray and park the gray bytes in shared memory (row pitch W rounded up + 4: two rows of a
 //      1920-wide frame would otherwise sit in the same banks);
@@ -360,8 +361,9 @@ static int upload(const std::vector<T>& v, T** out) {
 
 constexpr int kHashStaticSmem = 2048;                       // the finish kernel's static shared memory, rounded up
 constexpr int64_t kHashWorkspaceBytes = (int64_t)512 << 20;  // row buffer + finish workspace of one sub-batch
+constexpr int kHashRowsSmemBytes = 200 * 1024;              // the rows kernel's gray block (rows_per_cta * pitch)
 
-int hash_plan_create(HashPlan* p, int W, int H, int size, int lowpass, int max_batch) {
+int hash_plan_create(HashPlan* p, int W, int H, int size, int lowpass, int max_batch, bool force_global_ws) {
     PSD_REQUIRE(size >= 1 && lowpass >= 1, "HashDetector needs size >= 1 and lowpass >= 1");
     const int64_t n64 = (int64_t)size * lowpass;
     PSD_REQUIRE(W >= n64 && H >= n64, "frames smaller than the %lldx%lld hash image are not supported",
@@ -413,7 +415,7 @@ int hash_plan_create(HashPlan* p, int W, int H, int size, int lowpass, int max_b
     int dev = 0, smem_optin = 0;
     PSD_CUDA(cudaGetDevice(&dev));
     PSD_CUDA(cudaDeviceGetAttribute(&smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
-    p->global_ws = (size_t)p->ws_doubles * sizeof(double) > (size_t)smem_optin - kHashStaticSmem;
+    p->global_ws = force_global_ws || (size_t)p->ws_doubles * sizeof(double) > (size_t)smem_optin - kHashStaticSmem;
     // frames per sub-batch: the row buffer and the workspace together stay within kHashWorkspaceBytes
     // (or one frame's worth, if that is larger)
     const int64_t per_frame = (int64_t)H * n * (int64_t)sizeof(float) +
@@ -453,14 +455,15 @@ static int launch_hash_finish(const HashPlan& p, int nb, int H, uint64_t* out, c
 int launch_hash(const HashPlan* plans, int n_plans, const uint8_t* frames, int64_t frame_stride, int n_frames, int W,
                 int H, uint64_t* const* hashes, cudaStream_t stream) {
     PSD_REQUIRE(n_plans >= 1, "launch_hash: no hash plan");
-    // rows kernel: max(1, 256 / n) source rows per CTA for the smallest hash image n, their gray bytes in shared
-    // memory; a sub-batch fits every plan's row buffer and workspace
+    // rows kernel: max(1, 256 / n) source rows per CTA for the smallest hash image n, as many as fit
+    // kHashRowsSmemBytes of gray bytes in shared memory (a small n on a wide frame: 256 rows of 1920 would not);
+    // the row buffers do not depend on the block height.  A sub-batch fits every plan's row buffer and workspace.
     int n_min = plans[0].n, batch = plans[0].batch;
     for (int g = 1; g < n_plans; ++g) { n_min = std::min(n_min, plans[g].n); batch = std::min(batch, plans[g].batch); }
-    const int rows_per_cta = std::max(1, 256 / n_min);
     const int pitch = ((W + 3) & ~3) + 4;
+    PSD_REQUIRE(pitch <= kHashRowsSmemBytes, "frame too wide for the hash rows kernel (%d columns)", W);
+    const int rows_per_cta = std::max(1, std::min(256 / n_min, kHashRowsSmemBytes / pitch));
     const size_t smem_rows = (size_t)rows_per_cta * pitch;
-    PSD_REQUIRE(smem_rows <= 200 * 1024, "frame too wide for the hash rows kernel (%d columns)", W);
     PSD_CUDA(cudaFuncSetAttribute(psd_hash_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_rows));
     for (int f0 = 0; f0 < n_frames; f0 += batch) {   // sub-batches share the row buffers and the workspaces
         const int nb = std::min(batch, n_frames - f0);
@@ -496,3 +499,65 @@ int launch_hash_dist(const uint64_t* hashes, int64_t n, int size, const uint64_t
 }
 
 }  // namespace psd
+
+// ---- test hook: every stage of the hash pass through the production kernels ----
+extern "C" int psd_test_hash_stages(int device, const void* frames, int64_t n_frames, int32_t width, int32_t height,
+                                    int64_t frame_stride, const int32_t* geometries, int32_t n_geo, float* rowbuf_out,
+                                    uint64_t* hash_out, double* image_out, float* low_out) {
+    using namespace psd;
+    PSD_REQUIRE(frames && geometries && hash_out, "psd_test_hash_stages: null argument");
+    PSD_REQUIRE(n_frames >= 1 && n_frames <= (1 << 30), "psd_test_hash_stages: bad frame count %lld", (long long)n_frames);
+    PSD_REQUIRE(n_geo >= 1 && n_geo <= 16, "psd_test_hash_stages: 1 to 16 geometries, not %d", n_geo);
+    PSD_REQUIRE(width >= 1 && height >= 1 && frame_stride >= (int64_t)width * height * 3,
+                "psd_test_hash_stages: bad frame size or stride");
+    PSD_CUDA(cudaSetDevice(device));
+    cudaPointerAttributes at{};
+    if (cudaPointerGetAttributes(&at, frames) != cudaSuccess) cudaGetLastError();
+    PSD_REQUIRE((at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged) && at.device == device,
+                "psd_test_hash_stages: frames are not memory of device %d", device);
+    const bool force_global = image_out || low_out;
+    struct Owned {   // released on every return
+        std::vector<HashPlan> plans;
+        uint64_t* d_hash = nullptr;
+        ~Owned() { for (HashPlan& p : plans) hash_plan_destroy(&p); cudaFree(d_hash); }
+    } o;
+    o.plans.resize(n_geo);
+    int64_t words_total = 0;
+    for (int g = 0; g < n_geo; ++g) {
+        HashPlan& p = o.plans[g];
+        const int rc = hash_plan_create(&p, width, height, geometries[2 * g], geometries[2 * g + 1], (int)n_frames,
+                                        force_global);
+        if (rc) return rc;
+        PSD_REQUIRE(!(rowbuf_out || force_global) || p.batch >= n_frames,
+                    "psd_test_hash_stages: the stages of %lld frames need %lld frames per sub-batch, geometry %d has %d",
+                    (long long)n_frames, (long long)n_frames, g, p.batch);
+        words_total += n_frames * p.words;
+    }
+    PSD_CUDA(cudaMalloc(&o.d_hash, (size_t)words_total * sizeof(uint64_t)));
+    std::vector<uint64_t*> outs(n_geo);
+    for (int64_t g = 0, w = 0; g < n_geo; w += n_frames * o.plans[g].words, ++g) outs[g] = o.d_hash + w;
+    int rc = launch_hash(o.plans.data(), n_geo, (const uint8_t*)frames, frame_stride, (int)n_frames, width, height,
+                         outs.data(), 0);
+    if (rc) return rc;
+    PSD_CUDA(cudaDeviceSynchronize());
+    PSD_CUDA(cudaMemcpy(hash_out, o.d_hash, (size_t)words_total * sizeof(uint64_t), cudaMemcpyDeviceToHost));
+    for (const HashPlan& p : o.plans) {
+        const int64_t n2 = (int64_t)p.n * p.n, m = (int64_t)p.size * p.size;
+        if (rowbuf_out) {
+            const int64_t cnt = n_frames * height * p.n;
+            PSD_CUDA(cudaMemcpy(rowbuf_out, p.rowbuf, (size_t)cnt * sizeof(float), cudaMemcpyDeviceToHost));
+            rowbuf_out += cnt;
+        }
+        for (int64_t f = 0; f < n_frames && force_global; ++f) {
+            const double* ws = p.ws + f * p.ws_doubles;   // x [n][n] at 0, the low band after 2 n^2 + 2 size n
+            if (image_out)
+                PSD_CUDA(cudaMemcpy(image_out + f * n2, ws, (size_t)n2 * sizeof(double), cudaMemcpyDeviceToHost));
+            if (low_out)
+                PSD_CUDA(cudaMemcpy(low_out + f * m, ws + 2 * n2 + 2 * (int64_t)p.size * p.n, (size_t)m * sizeof(float),
+                                    cudaMemcpyDeviceToHost));
+        }
+        if (image_out) image_out += n_frames * n2;
+        if (low_out) low_out += n_frames * m;
+    }
+    return PSD_OK;
+}

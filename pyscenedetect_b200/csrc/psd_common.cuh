@@ -127,7 +127,9 @@ struct HashPlan {        // per-engine tables for one (frame size, hash size, lo
     float* rowbuf = nullptr;  // [batch][H][n] horizontal pass
     double* ws = nullptr;     // [batch][ws_doubles] finish workspace (global_ws only)
 };
-int hash_plan_create(HashPlan* p, int W, int H, int size, int lowpass, int max_batch);
+// force_global_ws: the finish kernel's working set in `ws` even where it fits shared memory (psd_test_hash_stages
+// reads the normalised image and the low band from there)
+int hash_plan_create(HashPlan* p, int W, int H, int size, int lowpass, int max_batch, bool force_global_ws = false);
 void hash_plan_destroy(HashPlan* p);
 // every plan's hashes of n_frames frames: hashes[g] receives plan g's ([n_frames][plans[g].words]); one gray
 // pass and one rows launch per sub-batch feed all the plans

@@ -2,7 +2,6 @@
 from the reference (tests/golden/hash_sizes_v1.json), the folded float64 DCT model against cv2, the hash stride
 and the detector's argument range."""
 
-import math
 import os
 import shutil
 import subprocess
@@ -12,6 +11,7 @@ import pytest
 
 from oracle import intmath as M
 from oracle import ref_detectors as R
+from tests import hash_twin as T
 from tests.hash_sizes_util import case_names, get_case, near_median
 from tests.hash_sizes_util import plan_frames as _frames
 
@@ -35,55 +35,10 @@ def test_oracle_reproduces_recorded_case(name):
     assert got == {int(t): v[0] for t, v in case["metrics"].items()}
 
 
-def _fold_levels(a):
-    """oracle/intmath.py:dct_fold_1d's levels, for every column of `a` at once (axis 0 folds)."""
-    levels = [a]
-    while levels[-1].shape[0] % 2 == 0 and levels[-1].shape[0] > 1 and len(levels) < 8:
-        p = levels[-1]
-        h = p.shape[0] // 2
-        levels.append(p[:h] + p[::-1][:h])
-    return levels
-
-
-def _dct_fold_cols(a, size, costab, n):
-    """dct_fold_1d applied to every column of `a` ((len, cols) float64) -> (size, cols): numpy element-wise
-    float64 operations in the same order, column by column, as the pure-Python twin."""
-    levels = _fold_levels(a)
-    out = np.zeros((size, a.shape[1]))
-    for u in range(size):
-        k = len(levels) - 1 if u == 0 else 0
-        if u:
-            while k + 1 < len(levels) and u % (2 << k) == 0:
-                k += 1
-        lv = levels[k]
-        nk = lv.shape[0]
-        acc = np.zeros(a.shape[1])
-        if nk % 2 == 0 and (u >> k) & 1:
-            for i in range(nk // 2):
-                acc = acc + (lv[i] - lv[nk - 1 - i]) * costab[((2 * i + 1) * u) % (4 * n)]
-        else:
-            for i in range(nk):
-                acc = acc + lv[i] * costab[((2 * i + 1) * u) % (4 * n)]
-        out[u] = acc
-    return out
-
-
 def phash_bits_columns(bgr, size, factor):
-    """intmath.phash_bits with the column loops vectorised (same per-column accumulation order)."""
-    n = size * factor
-    r = M.resize_area(M.bgr_to_gray(bgr), n)
-    mx = int(r.max()) or 1
-    x = (r.astype(np.float32) / np.float32(mx)).astype(np.float64)
-    costab = np.cos(np.pi * np.arange(4 * n) / (2.0 * n))
-    t = _dct_fold_cols(x, size, costab, n)             # t[u][j]
-    d = _dct_fold_cols(t.T.copy(), size, costab, n)     # d[v][u]
-    s0, s1 = math.sqrt(1.0 / n), math.sqrt(2.0 / n)
-    su = np.where(np.arange(size) > 0, s1, s0)
-    low = ((d.T * su[:, None]) * su[None, :]).astype(np.float32)
-    flat = np.sort(low.ravel())
-    m = flat.size
-    med = flat[m // 2] if m % 2 else np.float32(np.float32(flat[m // 2 - 1] + flat[m // 2]) * np.float32(0.5))
-    return low > med
+    """intmath.phash_bits with the column loops vectorised (same per-column accumulation order): the stage twin
+    of the device hash, tests/hash_twin.py."""
+    return T.stages(bgr, size, factor).bits.reshape(size, size)
 
 
 @pytest.mark.parametrize("shape,size,lowpass", [((160, 90), 8, 2), ((131, 97), 4, 2), ((64, 64), 16, 4),
