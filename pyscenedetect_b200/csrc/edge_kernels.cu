@@ -555,7 +555,14 @@ static int hdil_rows(int W, int ksize) {
     return rows;
 }
 
-bool edge_dilate_separable(int ksize) { return ksize / 2 >= kLargeMinR; }
+// this kernel size dilates in two passes through EdgeBuffers::bits_hdil
+static bool edge_dilate_separable(int ksize) { return ksize / 2 >= kLargeMinR; }
+
+// words per frame of a tile-major bit plane
+static int64_t edge_tile_words(int W, int H) {
+    const int Wq = (W + 31) / 32;
+    return (int64_t)((Wq + 1) / 2) * ((H + kHystTileH - 1) / kHystTileH) * kTileWords;
+}
 
 int edge_dilate_check(int W, int ksize) {
     if (!edge_dilate_separable(ksize)) return PSD_OK;
@@ -638,21 +645,47 @@ __global__ void psd_edge_unpack_kernel(const uint32_t* __restrict__ bits, uint8_
     out[i] = ((w >> (x & 31)) & 1u) ? 255 : 0;
 }
 
-int64_t edge_tile_words(int W, int H) {
+int edge_unpack(const EdgeBuffers& b, int64_t index, bool canny_map, int W, int H, cudaStream_t stream) {
     const int Wq = (W + 31) / 32;
-    return (int64_t)((Wq + 1) / 2) * ((H + kHystTileH - 1) / kHystTileH) * kTileWords;
-}
-
-int edge_unpack(const uint32_t* bits, uint8_t* out, int W, int H, bool tile_major, cudaStream_t stream) {
-    const int Wq = (W + 31) / 32;
-    psd_edge_unpack_kernel<<<(unsigned)(((int64_t)W * H + 255) / 256), 256, 0, stream>>>(bits, out, W, H, Wq,
-                                                                                         tile_major ? (Wq + 1) / 2 : 0);
+    const uint32_t* bits = canny_map ? b.bits_in + index * edge_tile_words(W, H) : b.bits_dil + index * H * (int64_t)Wq;
+    psd_edge_unpack_kernel<<<(unsigned)(((int64_t)W * H + 255) / 256), 256, 0, stream>>>(bits, b.tmp, W, H, Wq,
+                                                                                         canny_map ? (Wq + 1) / 2 : 0);
     PSD_CHECK_LAUNCH();
     return PSD_OK;
 }
 
-int launch_edges(const EdgeBuffers& b, int n, int W, int H, const EdgeSlot* slots, int n_slots, bool have_prev,
-                 cudaStream_t stream) {
+int edge_buffers_create(EdgeBuffers* b, int W, int H, int max_batch, int ksize) {
+    const size_t P = (size_t)W * H, words = (size_t)H * ((W + 31) / 32);
+    PSD_CUDA(cudaMalloc(&b->vplane, P * max_batch));
+    // the two planes of the hysteresis are tile-major and padded to whole 64 x 32 tiles; the padding is never
+    // written, so it is zeroed once here
+    const size_t tiled = (size_t)edge_tile_words(W, H) * 4 * max_batch;
+    PSD_CUDA(cudaMalloc(&b->cand, tiled)); PSD_CUDA(cudaMalloc(&b->bits_in, tiled));
+    PSD_CUDA(cudaMemset(b->cand, 0, tiled)); PSD_CUDA(cudaMemset(b->bits_in, 0, tiled));
+    PSD_CUDA(cudaMalloc(&b->tmp, P));
+    PSD_CUDA(cudaMalloc(&b->bits_dil, words * 4 * max_batch));
+    PSD_CUDA(cudaMalloc(&b->vhist, (size_t)max_batch * 256 * 4));
+    PSD_CUDA(cudaMalloc(&b->thresholds, (size_t)max_batch * 2 * 4));
+    PSD_CUDA(cudaMalloc(&b->hyst_flags, 64));
+    const size_t n_tiles = (size_t)max_batch * ((W + 63) / 64) * ((H + 31) / 32);
+    PSD_CUDA(cudaMalloc(&b->dirty, 2 * n_tiles));
+    return edge_buffers_add_ksize(b, W, H, max_batch, ksize);
+}
+
+int edge_buffers_add_ksize(EdgeBuffers* b, int W, int H, int max_batch, int ksize) {
+    if (edge_dilate_separable(ksize) && !b->bits_hdil)
+        PSD_CUDA(cudaMalloc(&b->bits_hdil, (size_t)H * ((W + 31) / 32) * 4 * max_batch));
+    return PSD_OK;
+}
+
+void edge_buffers_destroy(EdgeBuffers* b) {
+    cudaFree(b->vplane); cudaFree(b->vhist); cudaFree(b->thresholds); cudaFree(b->cand); cudaFree(b->bits_in);
+    cudaFree(b->bits_dil); cudaFree(b->bits_hdil); cudaFree(b->tmp); cudaFree(b->dirty); cudaFree(b->hyst_flags);
+    *b = EdgeBuffers{};
+}
+
+int launch_edges(const EdgeBuffers& b, int n, int W, int H, const EdgeSlot* slots, int n_slots, int64_t first,
+                 bool have_prev, cudaStream_t stream) {
     PSD_REQUIRE(n > 0 && n <= 65535, "edge batch out of range");
     const int64_t P = (int64_t)W * H;
     const int Wq = (W + 31) / 32;
@@ -723,8 +756,9 @@ int launch_edges(const EdgeBuffers& b, int n, int W, int H, const EdgeSlot* slot
         }
         PSD_CHECK_LAUNCH();
         dim3 sg((unsigned)min((int64_t)64, (per_frame + 255) / 256), (unsigned)n);
+        const FrameRows& sads = slots[s].sads;
         psd_edge_sad_bits_kernel<<<sg, 256, 0, stream>>>(b.bits_dil, slots[s].carry_bits, per_frame, have_prev ? 1 : 0,
-                                                         slots[s].sad, slots[s].sad_stride);
+                                                         sads.at<uint64_t>(first), sads.row_bytes / 8);
         PSD_CHECK_LAUNCH();
         count_launch(2);
         PSD_CUDA(cudaMemcpyAsync(slots[s].carry_bits, b.bits_dil + (int64_t)(n - 1) * per_frame,

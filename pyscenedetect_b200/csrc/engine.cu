@@ -6,7 +6,9 @@
 #include <stdarg.h>
 #include <string.h>
 
-#include <algorithm>
+#include <stddef.h>
+
+#include <memory>
 #include <vector>
 
 #include "psd_common.cuh"
@@ -52,7 +54,6 @@ struct psd_engine {
     int64_t src_frame_bytes = 0, frame_bytes = 0, P = 0;
     bool resize = false;
     uint32_t features = 0;
-    int ksize = 0;
     int max_batch = 0;
     cudaStream_t copy_stream = nullptr, compute_stream = nullptr;
     // staging (double buffered)
@@ -69,24 +70,19 @@ struct psd_engine {
     // carry (predecessor of the next frame, scored size)
     uint8_t* carry = nullptr;
     bool have_carry = false;
-    // results: slot 0 = halo frame, stream frame i at slot i+1
-    psd_frame_sums* d_sums = nullptr;
-    uint32_t* d_yhist = nullptr;
+    // per-frame results, `capacity` rows each (FrameRows: row 0 is the halo frame's)
+    FrameRows sums{nullptr, sizeof(psd_frame_sums)};
+    FrameRows yhist{nullptr, 256 * sizeof(uint32_t)};
     // hash slots: slot 0 is the configured geometry, psd_engine_add_hash_geometry appends
-    std::vector<HashPlan> hash;
-    std::vector<uint64_t*> d_hash;   // per slot [capacity][hash[slot].words]
+    struct HashSlot { HashPlan plan; FrameRows rows; };   // rows of plan.words uint64
+    std::vector<HashSlot> hash;
     int64_t capacity = 0;
     int64_t n_frames = 0;
     bool halo_scored = false;
-    // edge path: Canny scratch shared by every edge slot; slot 0 is the configured kernel size (its SADs are
-    // psd_frame_sums::sad_edges), psd_engine_add_edge_kernel_size appends
+    // edge path: Canny scratch shared by every edge slot; slot 0 is the configured kernel size,
+    // psd_engine_add_edge_kernel_size appends
     EdgeBuffers eb{};
-    struct EdgeSlotState {
-        int ksize;
-        uint32_t* carry_bits;   // [H][Wq] dilated edges of the predecessor frame
-        uint64_t* sad;          // [capacity], slot numbering of d_sums (nullptr for slot 0)
-    };
-    std::vector<EdgeSlotState> edge;
+    std::vector<EdgeSlot> edge;
     // last batch bookkeeping for debug taps
     const uint8_t* last_scored = nullptr;
     int64_t last_scored_stride = 0;
@@ -97,56 +93,56 @@ struct psd_engine {
     size_t ev_next = 0;
 };
 
-// a zeroed [cap][words] uint64 array holding the first n_frames + 1 result slots of *p ([old_cap][words], or none)
-static int grow_array(psd_engine* e, uint64_t** p, int64_t old_cap, int64_t cap, int words) {
-    uint64_t* np = nullptr;
-    PSD_CUDA(cudaMalloc(&np, (size_t)cap * words * sizeof(uint64_t)));
-    PSD_CUDA(cudaMemsetAsync(np, 0, (size_t)cap * words * sizeof(uint64_t), e->compute_stream));
-    if (*p) {
-        const int64_t keep = std::min(old_cap, e->n_frames + 1);
-        PSD_CUDA(cudaMemcpyAsync(np, *p, (size_t)keep * words * sizeof(uint64_t), cudaMemcpyDeviceToDevice,
-                                 e->compute_stream));
-        PSD_CUDA(cudaStreamSynchronize(e->compute_stream));
-        cudaFree(*p);
+int FrameRows::grow(int64_t cap, int64_t keep, cudaStream_t stream) {
+    uint8_t* p = nullptr;
+    PSD_CUDA(cudaMalloc(&p, (size_t)cap * row_bytes));
+    PSD_CUDA(cudaMemsetAsync(p, 0, (size_t)cap * row_bytes, stream));
+    if (d) {
+        PSD_CUDA(cudaMemcpyAsync(p, d, (size_t)keep * row_bytes, cudaMemcpyDeviceToDevice, stream));
+        PSD_CUDA(cudaStreamSynchronize(stream));
+        cudaFree(d);
     }
-    *p = np;
+    d = p;
     return PSD_OK;
 }
 
-static int ensure_capacity(psd_engine* e, int64_t need_slots) {
-    if (need_slots <= e->capacity) return PSD_OK;
+int FrameRows::zero(int64_t first, int64_t n, cudaStream_t stream) const {
+    PSD_CUDA(cudaMemsetAsync(at<uint8_t>(first), 0, (size_t)n * row_bytes, stream));
+    return PSD_OK;
+}
+
+// The result arrays the score and edge passes accumulate into (zeroed before each batch), then, with `all`, the hash
+// slots' (whose pass writes whole rows).  Edge slot 0's SAD rows are part of the sums.
+static std::vector<FrameRows*> result_arrays(psd_engine* e, bool all) {
+    std::vector<FrameRows*> v{&e->sums};
+    if (e->features & PSD_F_YHIST) v.push_back(&e->yhist);
+    for (size_t s = 1; s < e->edge.size(); ++s) v.push_back(&e->edge[s].sads);
+    if (all)
+        for (auto& h : e->hash) v.push_back(&h.rows);
+    return v;
+}
+
+// the row before stream frame `first`'s (frame first - 1, or the halo frame), nullptr if that frame was not scored
+template <class T>
+static const T* previous_row(const psd_engine* e, const FrameRows& r, int64_t first) {
+    return (first > 0 || e->halo_scored) ? r.at<T>(first - 1) : nullptr;
+}
+
+// edge slot 0's SAD rows: psd_frame_sums::sad_edges of the sums, 8 words apart
+static FrameRows sums_sad_rows(const psd_engine* e) {
+    return FrameRows{e->sums.d + offsetof(psd_frame_sums, sad_edges), e->sums.row_bytes};
+}
+
+static int ensure_capacity(psd_engine* e, int64_t need_rows) {
+    if (need_rows <= e->capacity) return PSD_OK;
     int64_t cap = e->capacity ? e->capacity : 4096;
-    while (cap < need_slots) cap *= 2;
-    psd_frame_sums* ns = nullptr;
-    PSD_CUDA(cudaMalloc(&ns, (size_t)cap * sizeof(psd_frame_sums)));
-    PSD_CUDA(cudaMemsetAsync(ns, 0, (size_t)cap * sizeof(psd_frame_sums), e->compute_stream));
-    if (e->d_sums) {
-        PSD_CUDA(cudaMemcpyAsync(ns, e->d_sums, (size_t)(e->n_frames + 1) * sizeof(psd_frame_sums),
-                                 cudaMemcpyDeviceToDevice, e->compute_stream));
-        PSD_CUDA(cudaStreamSynchronize(e->compute_stream));
-        cudaFree(e->d_sums);
-    }
-    e->d_sums = ns;
-    if (e->features & PSD_F_YHIST) {
-        uint32_t* nh = nullptr;
-        PSD_CUDA(cudaMalloc(&nh, (size_t)cap * 256 * sizeof(uint32_t)));
-        PSD_CUDA(cudaMemsetAsync(nh, 0, (size_t)cap * 256 * sizeof(uint32_t), e->compute_stream));
-        if (e->d_yhist) {
-            PSD_CUDA(cudaMemcpyAsync(nh, e->d_yhist, (size_t)(e->n_frames + 1) * 256 * sizeof(uint32_t),
-                                     cudaMemcpyDeviceToDevice, e->compute_stream));
-            PSD_CUDA(cudaStreamSynchronize(e->compute_stream));
-            cudaFree(e->d_yhist);
-        }
-        e->d_yhist = nh;
-    }
-    for (size_t s = 0; s < e->hash.size(); ++s) {
-        int rc = grow_array(e, &e->d_hash[s], e->capacity, cap, e->hash[s].words);
-        if (rc) return rc;
-    }
-    for (size_t s = 1; s < e->edge.size(); ++s) {
-        int rc = grow_array(e, &e->edge[s].sad, e->capacity, cap, 1);
-        if (rc) return rc;
-    }
+    while (cap < need_rows) cap *= 2;
+    int rc = PSD_OK;
+    for (FrameRows* r : result_arrays(e, true))
+        if ((rc = r->grow(cap, e->n_frames + 1, e->compute_stream))) break;
+    if (!e->edge.empty())   // slot 0's SADs move with the sums
+        e->edge[0].sads = sums_sad_rows(e);
+    if (rc) return rc;
     e->capacity = cap;
     return PSD_OK;
 }
@@ -172,9 +168,8 @@ static bool reads_in_place(const psd_engine* e, const uint8_t* src, const psd_fr
 
 // Score `n` frames at `src` (source size, in layout `l`) that are visible to compute_stream: resized from the
 // layout, read in place, or gathered to packed BGR in `small` first (n <= max_batch unless read in place).
-// slot0: result slot of the first frame (0 = halo slot).
-static int run_batch(psd_engine* e, const uint8_t* src, const psd_frame_layout& l, int64_t n,
-                     int64_t slot0, bool is_halo) {
+// first: stream frame of the first frame (-1 = the halo frame).
+static int run_batch(psd_engine* e, const uint8_t* src, const psd_frame_layout& l, int64_t n, int64_t first) {
     cudaStream_t st = e->compute_stream;
     cudaEvent_t t0 = next_event(e), t1 = next_event(e), k0 = next_event(e), k1 = next_event(e);
     if (!t0 || !t1 || !k0 || !k1) { set_error("cudaEventCreate failed"); return PSD_ERR_CUDA; }
@@ -194,22 +189,19 @@ static int run_batch(psd_engine* e, const uint8_t* src, const psd_frame_layout& 
         scored = e->small;
         scored_stride = e->small_stride;
     }
-    PSD_CUDA(cudaMemsetAsync(e->d_sums + slot0, 0, (size_t)n * sizeof(psd_frame_sums), st));
-    if (e->features & PSD_F_YHIST)
-        PSD_CUDA(cudaMemsetAsync(e->d_yhist + slot0 * 256, 0, (size_t)n * 256 * sizeof(uint32_t), st));
-    if (e->features & PSD_F_EDGES) {
-        PSD_CUDA(cudaMemsetAsync(e->eb.vhist, 0, (size_t)n * 256 * sizeof(uint32_t), st));
-        for (size_t s = 1; s < e->edge.size(); ++s)
-            PSD_CUDA(cudaMemsetAsync(e->edge[s].sad + slot0, 0, (size_t)n * sizeof(uint64_t), st));
+    for (FrameRows* r : result_arrays(e, false)) {
+        int rc = r->zero(first, n, st);
+        if (rc) return rc;
     }
+    if (e->features & PSD_F_EDGES) PSD_CUDA(cudaMemsetAsync(e->eb.vhist, 0, (size_t)n * 256 * sizeof(uint32_t), st));
     ScoreArgs a{};
     a.frames = scored;
-    a.prev = (e->have_carry && !is_halo) ? e->carry : nullptr;
+    a.prev = (e->have_carry && first >= 0) ? e->carry : nullptr;
     a.frame_stride = scored_stride;
     a.n_frames = (int32_t)n;
     a.n_pixels = (int32_t)e->P;
-    a.sums = e->d_sums + slot0;
-    a.yhist = (e->features & PSD_F_YHIST) ? e->d_yhist + slot0 * 256 : nullptr;
+    a.sums = e->sums.at<psd_frame_sums>(first);
+    a.yhist = (e->features & PSD_F_YHIST) ? e->yhist.at<uint32_t>(first) : nullptr;
     a.vhist = (e->features & PSD_F_EDGES) ? e->eb.vhist : nullptr;
     a.vplane = (e->features & PSD_F_EDGES) ? e->eb.vplane : nullptr;
     PSD_CUDA(cudaEventRecord(k0, st));
@@ -219,22 +211,15 @@ static int run_batch(psd_engine* e, const uint8_t* src, const psd_frame_layout& 
         if (rc) return rc;
     }
     if (e->features & PSD_F_HASH) {
-        std::vector<uint64_t*> outs(e->hash.size());
-        for (size_t s = 0; s < e->hash.size(); ++s) outs[s] = e->d_hash[s] + slot0 * e->hash[s].words;
-        rc = launch_hash(e->hash.data(), (int)e->hash.size(), scored, scored_stride, (int)n, e->W, e->H, outs.data(), st);
+        std::vector<HashPlan> plans; std::vector<uint64_t*> outs;
+        for (const auto& h : e->hash) { plans.push_back(h.plan); outs.push_back(h.rows.at<uint64_t>(first)); }
+        rc = launch_hash(plans.data(), (int)plans.size(), scored, scored_stride, (int)n, e->W, e->H, outs.data(), st);
         if (rc) return rc;
     }
     PSD_CUDA(cudaEventRecord(k1, st));
     e->ev_score.push_back({k0, k1});
     if (e->features & PSD_F_EDGES) {
-        std::vector<EdgeSlot> slots(e->edge.size());
-        for (size_t s = 0; s < e->edge.size(); ++s) {
-            const bool own = s > 0;   // slot 0 accumulates into psd_frame_sums::sad_edges
-            slots[s] = EdgeSlot{e->edge[s].ksize, e->edge[s].carry_bits,
-                                own ? e->edge[s].sad + slot0 : &e->d_sums[slot0].sad_edges,
-                                own ? 1 : (int64_t)(sizeof(psd_frame_sums) / sizeof(uint64_t))};
-        }
-        rc = launch_edges(e->eb, (int)n, e->W, e->H, slots.data(), (int)slots.size(), a.prev != nullptr, st);
+        rc = launch_edges(e->eb, (int)n, e->W, e->H, e->edge.data(), (int)e->edge.size(), first, a.prev != nullptr, st);
         if (rc) return rc;
     }
     // carry the last frame (scored size) for the next batch
@@ -323,13 +308,11 @@ void psd_engine_destroy(psd_engine* e) {
         if (e->h2d_done[s]) cudaEventDestroy(e->h2d_done[s]);
     }
     cudaFree(e->small); cudaFree(e->d_xofs); cudaFree(e->d_xa); cudaFree(e->d_yofs); cudaFree(e->d_ya);
-    cudaFree(e->carry); cudaFree(e->d_sums); cudaFree(e->d_yhist);
-    for (uint64_t* p : e->d_hash) cudaFree(p);
-    for (HashPlan& p : e->hash) hash_plan_destroy(&p);
-    for (auto& s : e->edge) { cudaFree(s.carry_bits); cudaFree(s.sad); }
-    cudaFree(e->eb.vplane); cudaFree(e->eb.vhist); cudaFree(e->eb.thresholds); cudaFree(e->eb.cand);
-    cudaFree(e->eb.tmp); cudaFree(e->eb.bits_in); cudaFree(e->eb.bits_dil); cudaFree(e->eb.bits_hdil);
-    cudaFree(e->eb.dirty); cudaFree(e->eb.hyst_flags);
+    cudaFree(e->carry);
+    for (FrameRows* r : result_arrays(e, true)) r->release();
+    for (auto& h : e->hash) hash_plan_destroy(&h.plan);
+    for (auto& s : e->edge) cudaFree(s.carry_bits);
+    edge_buffers_destroy(&e->eb);
     for (cudaEvent_t ev : e->ev_pool) cudaEventDestroy(ev);
     if (e->copy_stream) cudaStreamDestroy(e->copy_stream);
     if (e->compute_stream) cudaStreamDestroy(e->compute_stream);
@@ -345,16 +328,39 @@ static int effective_ksize(const psd_engine* e, int k) {
     return k;
 }
 
-#define ENG_CUDA(expr)                                                                          \
-    do {                                                                                        \
-        cudaError_t _e = (expr);                                                                \
-        if (_e != cudaSuccess) {                                                                \
-            psd::set_error("%s failed: %s (%s:%d)", #expr, cudaGetErrorString(_e), __FILE__,    \
-                           __LINE__);                                                           \
-            psd_engine_destroy(e);                                                              \
-            return (_e == cudaErrorMemoryAllocation) ? PSD_ERR_OOM : PSD_ERR_CUDA;              \
-        }                                                                                       \
-    } while (0)
+// a new edge slot of kernel size k: its scratch, its carried edges and its SAD rows (slot 0's are the sums')
+static int add_edge_slot(psd_engine* e, int k) {
+    int rc = edge_dilate_check(e->W, k);
+    if (rc) return rc;
+    rc = e->edge.empty() ? edge_buffers_create(&e->eb, e->W, e->H, e->max_batch, k)
+                         : edge_buffers_add_ksize(&e->eb, e->W, e->H, e->max_batch, k);
+    if (rc) return rc;
+    EdgeSlot s{k, nullptr, FrameRows{nullptr, sizeof(uint64_t)}};
+    PSD_CUDA(cudaMalloc(&s.carry_bits, (size_t)e->H * ((e->W + 31) / 32) * 4));
+    if (e->edge.empty())
+        s.sads = sums_sad_rows(e);
+    else if ((rc = s.sads.grow(e->capacity, 0, e->compute_stream))) {
+        cudaFree(s.carry_bits);
+        return rc;
+    }
+    e->edge.push_back(s);
+    return PSD_OK;
+}
+
+// a new hash slot: its plan and its rows
+static int add_hash_slot(psd_engine* e, int size, int lowpass) {
+    psd_engine::HashSlot h{};
+    int rc = hash_plan_create(&h.plan, e->W, e->H, size, lowpass, e->max_batch);
+    h.rows.row_bytes = (int64_t)h.plan.words * sizeof(uint64_t);
+    if (!rc) rc = h.rows.grow(e->capacity, 0, e->compute_stream);
+    if (rc) {
+        hash_plan_destroy(&h.plan);
+        h.rows.release();
+        return rc;
+    }
+    e->hash.push_back(h);
+    return PSD_OK;
+}
 
 int psd_engine_create(const psd_config* cfg, psd_engine** out) {
     PSD_REQUIRE(cfg && out, "psd_engine_create: null argument");
@@ -382,7 +388,9 @@ int psd_engine_create(const psd_config* cfg, psd_engine** out) {
         return PSD_ERR_NODEVICE;
     }
     PSD_CUDA(cudaSetDevice(cfg->device));
-    psd_engine* e = new (std::nothrow) psd_engine();
+    // the engine is destroyed on every return before it is handed out (psd_engine_destroy takes a partial engine)
+    std::unique_ptr<psd_engine, void (*)(psd_engine*)> guard(new (std::nothrow) psd_engine(), psd_engine_destroy);
+    psd_engine* e = guard.get();
     if (!e) { set_error("out of host memory"); return PSD_ERR_OOM; }
     e->cfg = *cfg;
     e->device = cfg->device;
@@ -394,70 +402,38 @@ int psd_engine_create(const psd_config* cfg, psd_engine** out) {
     e->src_frame_bytes = (int64_t)e->sw * e->sh * 3;
     e->features = cfg->features | ((cfg->features & PSD_F_EDGES) ? PSD_F_HSV : 0);
     e->max_batch = cfg->max_batch;
-    if (e->features & PSD_F_EDGES) {
-        const int k = effective_ksize(e, cfg->edge_kernel_size);
-        if (edge_dilate_check(e->W, k) != PSD_OK) {
-            psd_engine_destroy(e);
-            return PSD_ERR_INVALID;
-        }
-        e->ksize = k;
-        e->edge.push_back({k, nullptr, nullptr});
-    }
-    if (e->features & PSD_F_HASH) {
-        e->hash.emplace_back();
-        e->d_hash.push_back(nullptr);
-        int rc = hash_plan_create(&e->hash[0], e->W, e->H, cfg->hash_size ? cfg->hash_size : 8,
-                                  cfg->hash_lowpass ? cfg->hash_lowpass : 2, e->max_batch);
-        if (rc) { psd_engine_destroy(e); return rc; }
-    }
-    ENG_CUDA(cudaStreamCreateWithFlags(&e->copy_stream, cudaStreamNonBlocking));
-    ENG_CUDA(cudaStreamCreateWithFlags(&e->compute_stream, cudaStreamNonBlocking));
+    PSD_CUDA(cudaStreamCreateWithFlags(&e->copy_stream, cudaStreamNonBlocking));
+    PSD_CUDA(cudaStreamCreateWithFlags(&e->compute_stream, cudaStreamNonBlocking));
     for (int s = 0; s < 2; ++s) {
-        ENG_CUDA(cudaEventCreateWithFlags(&e->slot_free[s], cudaEventDisableTiming));
-        ENG_CUDA(cudaEventCreateWithFlags(&e->h2d_done[s], cudaEventDisableTiming));
+        PSD_CUDA(cudaEventCreateWithFlags(&e->slot_free[s], cudaEventDisableTiming));
+        PSD_CUDA(cudaEventCreateWithFlags(&e->h2d_done[s], cudaEventDisableTiming));
     }
-    ENG_CUDA(cudaMalloc(&e->carry, (size_t)e->frame_bytes));
+    PSD_CUDA(cudaMalloc(&e->carry, (size_t)e->frame_bytes));
     // without resizing, staged batches of a frame size that is not a multiple of 16 bytes are always copied
     // (user device pointers that are not 16-byte aligned allocate it on first use, in run_batch)
     if (e->resize || e->frame_bytes % 16 != 0)
-        ENG_CUDA(cudaMalloc(&e->small, (size_t)e->small_stride * e->max_batch));
+        PSD_CUDA(cudaMalloc(&e->small, (size_t)e->small_stride * e->max_batch));
     if (e->resize) {
         std::vector<int32_t> xo, yo; std::vector<int16_t> xa, ya;
         build_taps(e->sw, e->W, xo, xa);
         build_taps(e->sh, e->H, yo, ya);
-        ENG_CUDA(cudaMalloc(&e->d_xofs, xo.size() * 4)); ENG_CUDA(cudaMalloc(&e->d_xa, xa.size() * 2));
-        ENG_CUDA(cudaMalloc(&e->d_yofs, yo.size() * 4)); ENG_CUDA(cudaMalloc(&e->d_ya, ya.size() * 2));
-        ENG_CUDA(cudaMemcpy(e->d_xofs, xo.data(), xo.size() * 4, cudaMemcpyHostToDevice));
-        ENG_CUDA(cudaMemcpy(e->d_xa, xa.data(), xa.size() * 2, cudaMemcpyHostToDevice));
-        ENG_CUDA(cudaMemcpy(e->d_yofs, yo.data(), yo.size() * 4, cudaMemcpyHostToDevice));
-        ENG_CUDA(cudaMemcpy(e->d_ya, ya.data(), ya.size() * 2, cudaMemcpyHostToDevice));
+        PSD_CUDA(cudaMalloc(&e->d_xofs, xo.size() * 4)); PSD_CUDA(cudaMalloc(&e->d_xa, xa.size() * 2));
+        PSD_CUDA(cudaMalloc(&e->d_yofs, yo.size() * 4)); PSD_CUDA(cudaMalloc(&e->d_ya, ya.size() * 2));
+        PSD_CUDA(cudaMemcpy(e->d_xofs, xo.data(), xo.size() * 4, cudaMemcpyHostToDevice));
+        PSD_CUDA(cudaMemcpy(e->d_xa, xa.data(), xa.size() * 2, cudaMemcpyHostToDevice));
+        PSD_CUDA(cudaMemcpy(e->d_yofs, yo.data(), yo.size() * 4, cudaMemcpyHostToDevice));
+        PSD_CUDA(cudaMemcpy(e->d_ya, ya.data(), ya.size() * 2, cudaMemcpyHostToDevice));
     }
+    int rc = ensure_capacity(e, 4096);
+    if (rc) return rc;
     if (e->features & PSD_F_EDGES) {
-        const size_t plane = (size_t)e->P * e->max_batch;
-        ENG_CUDA(cudaMalloc(&e->eb.vplane, plane));
-        const size_t words = (size_t)e->H * ((e->W + 31) / 32);
-        // the two planes of the hysteresis are tile-major and padded to whole 64 x 32 tiles; the padding is never
-        // written, so it is zeroed once here
-        const size_t tiled = (size_t)edge_tile_words(e->W, e->H) * 4 * e->max_batch;
-        ENG_CUDA(cudaMalloc(&e->eb.cand, tiled));
-        ENG_CUDA(cudaMalloc(&e->eb.bits_in, tiled));
-        ENG_CUDA(cudaMemset(e->eb.cand, 0, tiled));
-        ENG_CUDA(cudaMemset(e->eb.bits_in, 0, tiled));
-        ENG_CUDA(cudaMalloc(&e->eb.tmp, (size_t)e->P));
-        ENG_CUDA(cudaMalloc(&e->eb.bits_dil, words * 4 * e->max_batch));
-        if (edge_dilate_separable(e->ksize)) ENG_CUDA(cudaMalloc(&e->eb.bits_hdil, words * 4 * e->max_batch));
-        ENG_CUDA(cudaMalloc(&e->edge[0].carry_bits, words * 4));
-        ENG_CUDA(cudaMalloc(&e->eb.vhist, (size_t)e->max_batch * 256 * 4));
-        ENG_CUDA(cudaMalloc(&e->eb.thresholds, (size_t)e->max_batch * 2 * 4));
-        ENG_CUDA(cudaMalloc(&e->eb.hyst_flags, 64));
-        const size_t n_tiles = (size_t)e->max_batch * ((e->W + 63) / 64) * ((e->H + 31) / 32);
-        ENG_CUDA(cudaMalloc(&e->eb.dirty, 2 * n_tiles));
+        if ((rc = add_edge_slot(e, effective_ksize(e, cfg->edge_kernel_size)))) return rc;
     }
-    {
-        int rc = ensure_capacity(e, 4096);
-        if (rc) { psd_engine_destroy(e); return rc; }
+    if (e->features & PSD_F_HASH) {
+        rc = add_hash_slot(e, cfg->hash_size ? cfg->hash_size : 8, cfg->hash_lowpass ? cfg->hash_lowpass : 2);
+        if (rc) return rc;
     }
-    *out = e;
+    *out = guard.release();
     return PSD_OK;
 }
 
@@ -529,7 +505,7 @@ int psd_engine_set_halo_device(psd_engine* e, const void* dptr) {
     PSD_REQUIRE(e->n_frames == 0, "halo must be set before the first frame is submitted");
     PSD_CUDA(cudaSetDevice(e->device));
     e->have_carry = false;
-    int rc = run_batch(e, (const uint8_t*)dptr, packed_layout(e, e->src_frame_bytes), 1, 0, true);
+    int rc = run_batch(e, (const uint8_t*)dptr, packed_layout(e, e->src_frame_bytes), 1, -1);
     if (rc) return rc;
     e->halo_scored = true;
     return PSD_OK;
@@ -595,7 +571,7 @@ int psd_engine_submit_device_layout(psd_engine* e, const void* base, int64_t n, 
     int64_t done = 0;
     while (done < n) {
         const int64_t b = (n - done < batch) ? (n - done) : batch;
-        rc = run_batch(e, p + done * l.frame_stride, l, b, e->n_frames + 1, false);
+        rc = run_batch(e, p + done * l.frame_stride, l, b, e->n_frames);
         if (rc) return rc;
         e->n_frames += b;
         done += b;
@@ -622,7 +598,7 @@ int psd_engine_submit_host(psd_engine* e, const uint8_t* bgr, int64_t n, int64_t
         e->next_slot ^= 1;
         rc = stage_host(e, bgr + done * frame_stride, b, frame_stride, row_pitch, flags, slot);
         if (rc) return rc;
-        rc = run_batch(e, e->dev_stage[slot], packed_layout(e, e->src_frame_bytes), b, e->n_frames + 1, false);
+        rc = run_batch(e, e->dev_stage[slot], packed_layout(e, e->src_frame_bytes), b, e->n_frames);
         if (rc) return rc;
         PSD_CUDA(cudaEventRecord(e->slot_free[slot], e->compute_stream));
         e->n_frames += b;
@@ -641,37 +617,33 @@ int psd_engine_sync(psd_engine* e) {
 
 void* psd_engine_compute_stream(psd_engine* e) { return e ? (void*)e->compute_stream : nullptr; }
 int64_t psd_engine_frame_count(const psd_engine* e) { return e ? e->n_frames : -1; }
-int psd_engine_edge_kernel_size(const psd_engine* e) { return e ? e->ksize : -1; }
+int psd_engine_edge_kernel_size(const psd_engine* e) { return e ? (e->edge.empty() ? 0 : e->edge[0].ksize) : -1; }
 
-int psd_engine_read_sums(psd_engine* e, int64_t first, int64_t n, psd_frame_sums* out) {
-    PSD_REQUIRE(e && out, "psd_engine_read_sums: null argument");
+// the rows of stream frames [first, first + n) (first = -1: from the halo frame's) to the host, once the engine is idle
+static int read_rows(psd_engine* e, const FrameRows& r, int64_t first, int64_t n, void* out) {
     PSD_REQUIRE(first >= -1 && n >= 0 && first + n <= e->n_frames, "frame range out of bounds");
     int rc = psd_engine_sync(e);
     if (rc) return rc;
-    if (n) PSD_CUDA(cudaMemcpy(out, e->d_sums + first + 1, (size_t)n * sizeof(psd_frame_sums), cudaMemcpyDeviceToHost));
+    if (n) PSD_CUDA(cudaMemcpy(out, r.at<uint8_t>(first), (size_t)n * r.row_bytes, cudaMemcpyDeviceToHost));
     return PSD_OK;
+}
+
+int psd_engine_read_sums(psd_engine* e, int64_t first, int64_t n, psd_frame_sums* out) {
+    PSD_REQUIRE(e && out, "psd_engine_read_sums: null argument");
+    return read_rows(e, e->sums, first, n, out);
 }
 
 int psd_engine_read_yhist(psd_engine* e, int64_t first, int64_t n, uint32_t* out) {
     PSD_REQUIRE(e && out, "psd_engine_read_yhist: null argument");
     PSD_REQUIRE(e->features & PSD_F_YHIST, "engine was created without PSD_F_YHIST");
-    PSD_REQUIRE(first >= -1 && n >= 0 && first + n <= e->n_frames, "frame range out of bounds");
-    int rc = psd_engine_sync(e);
-    if (rc) return rc;
-    if (n) PSD_CUDA(cudaMemcpy(out, e->d_yhist + (first + 1) * 256, (size_t)n * 256 * 4, cudaMemcpyDeviceToHost));
-    return PSD_OK;
+    return read_rows(e, e->yhist, first, n, out);
 }
 
 int psd_engine_read_hash_at(psd_engine* e, int32_t slot, int64_t first, int64_t n, uint64_t* out) {
     PSD_REQUIRE(e && out, "psd_engine_read_hash: null argument");
     PSD_REQUIRE(e->features & PSD_F_HASH, "engine was created without PSD_F_HASH");
     PSD_REQUIRE(slot >= 0 && slot < (int32_t)e->hash.size(), "hash slot %d out of range (%d)", slot, (int)e->hash.size());
-    PSD_REQUIRE(first >= -1 && n >= 0 && first + n <= e->n_frames, "frame range out of bounds");
-    int rc = psd_engine_sync(e);
-    if (rc) return rc;
-    const int words = e->hash[slot].words;
-    if (n) PSD_CUDA(cudaMemcpy(out, e->d_hash[slot] + (first + 1) * words, (size_t)n * words * 8, cudaMemcpyDeviceToHost));
-    return PSD_OK;
+    return read_rows(e, e->hash[slot].rows, first, n, out);
 }
 
 int psd_engine_read_hash(psd_engine* e, int64_t first, int64_t n, uint64_t* out) {
@@ -682,7 +654,7 @@ int psd_engine_device_hash_at(psd_engine* e, int32_t slot, const uint64_t** hash
     PSD_REQUIRE(e && hashes, "psd_engine_device_hash: null argument");
     if (e->hash.empty() && slot == 0) { *hashes = nullptr; return PSD_OK; }
     PSD_REQUIRE(slot >= 0 && slot < (int32_t)e->hash.size(), "hash slot %d out of range (%d)", slot, (int)e->hash.size());
-    *hashes = e->d_hash[slot] + e->hash[slot].words;
+    *hashes = e->hash[slot].rows.at<uint64_t>(0);
     return PSD_OK;
 }
 
@@ -692,7 +664,7 @@ int psd_engine_device_edge_sads(psd_engine* e, int32_t slot, const uint64_t** sa
     PSD_REQUIRE(e && sad_edges, "psd_engine_device_edge_sads: null argument");
     PSD_REQUIRE(slot == 0 || (slot > 0 && slot < (int32_t)e->edge.size()), "edge slot %d out of range (%d)", slot,
                 (int)e->edge.size());
-    *sad_edges = slot == 0 ? nullptr : e->edge[slot].sad + 1;
+    *sad_edges = slot == 0 ? nullptr : e->edge[slot].sads.at<uint64_t>(0);
     return PSD_OK;
 }
 
@@ -720,16 +692,8 @@ int psd_engine_add_edge_kernel_size(psd_engine* e, int32_t kernel_size, int32_t*
     const int k = effective_ksize(e, kernel_size);
     for (size_t s = 0; s < e->edge.size(); ++s)
         if (e->edge[s].ksize == k) { *slot = (int32_t)s; return PSD_OK; }
-    rc = edge_dilate_check(e->W, k);
-    if (rc) return rc;
     PSD_CUDA(cudaSetDevice(e->device));
-    const size_t words = (size_t)e->H * ((e->W + 31) / 32);
-    if (edge_dilate_separable(k) && !e->eb.bits_hdil)
-        PSD_CUDA(cudaMalloc(&e->eb.bits_hdil, words * 4 * e->max_batch));
-    e->edge.push_back({k, nullptr, nullptr});
-    auto& st = e->edge.back();
-    PSD_CUDA(cudaMalloc(&st.carry_bits, words * 4));
-    rc = grow_array(e, &st.sad, 0, e->capacity, 1);
+    rc = add_edge_slot(e, k);
     if (rc) return rc;
     *slot = (int32_t)(e->edge.size() - 1);
     return PSD_OK;
@@ -743,25 +707,21 @@ int psd_engine_add_hash_geometry(psd_engine* e, int32_t size, int32_t lowpass, i
     if (rc) return rc;
     size = size ? size : 8;
     lowpass = lowpass ? lowpass : 2;
-    for (size_t s = 0; s < e->hash.size(); ++s)
-        if (e->hash[s].size == size && e->hash[s].n == (int64_t)size * lowpass) { *slot = (int32_t)s; return PSD_OK; }
+    for (size_t s = 0; s < e->hash.size(); ++s) {
+        const HashPlan& p = e->hash[s].plan;
+        if (p.size == size && p.n == (int64_t)size * lowpass) { *slot = (int32_t)s; return PSD_OK; }
+    }
     PSD_CUDA(cudaSetDevice(e->device));
-    HashPlan p{};
-    rc = hash_plan_create(&p, e->W, e->H, size, lowpass, e->max_batch);
-    if (rc) { hash_plan_destroy(&p); return rc; }
-    uint64_t* d = nullptr;
-    rc = grow_array(e, &d, 0, e->capacity, p.words);
-    if (rc) { hash_plan_destroy(&p); return rc; }
-    e->hash.push_back(p);
-    e->d_hash.push_back(d);
+    rc = add_hash_slot(e, size, lowpass);
+    if (rc) return rc;
     *slot = (int32_t)(e->hash.size() - 1);
     return PSD_OK;
 }
 
 int psd_engine_device_results(psd_engine* e, const psd_frame_sums** sums, const uint32_t** yhist) {
     PSD_REQUIRE(e, "null engine");
-    if (sums) *sums = e->d_sums + 1;
-    if (yhist) *yhist = e->d_yhist ? e->d_yhist + 256 : nullptr;
+    if (sums) *sums = e->sums.at<psd_frame_sums>(0);
+    if (yhist) *yhist = e->yhist.d ? e->yhist.at<uint32_t>(0) : nullptr;
     return PSD_OK;
 }
 
@@ -800,10 +760,7 @@ int psd_engine_debug_plane(psd_engine* e, int which, int64_t index, uint8_t* out
     PSD_REQUIRE(cap >= (size_t)e->P, "buffer too small");
     PSD_REQUIRE(which >= 1 && which <= 3, "unknown plane %d", which);
     if (which == 2 || which == 3) {  // bit-packed maps -> 0/255 bytes
-        const size_t words = (size_t)e->H * ((e->W + 31) / 32);
-        const uint32_t* bits = which == 3 ? e->eb.bits_dil + index * words
-                                          : e->eb.bits_in + index * (size_t)edge_tile_words(e->W, e->H);
-        rc = edge_unpack(bits, e->eb.tmp, e->W, e->H, which == 2, e->compute_stream);
+        rc = edge_unpack(e->eb, index, which == 2, e->W, e->H, e->compute_stream);
         if (rc) return rc;
         PSD_CUDA(cudaStreamSynchronize(e->compute_stream));
         PSD_CUDA(cudaMemcpy(out, e->eb.tmp, (size_t)e->P, cudaMemcpyDeviceToHost));
@@ -820,6 +777,12 @@ static int scan_to_host(psd_engine* e, double* d_tmp, double* out, size_t count)
     return PSD_OK;
 }
 
+// a host scan's device buffer: allocated per call, freed on every return
+struct ScanBuffer {
+    double* p = nullptr;
+    ~ScanBuffer() { cudaFree(p); }
+};
+
 int psd_engine_scan_content_host_at(psd_engine* e, int32_t edge_slot, int64_t first, int64_t n,
                                     const double weights[4], double weight_abs_sum, double* out_components,
                                     double* out_content_val) {
@@ -829,14 +792,13 @@ int psd_engine_scan_content_host_at(psd_engine* e, int32_t edge_slot, int64_t fi
                 "edge slot %d out of range (%d)", edge_slot, (int)e->edge.size());
     if (n == 0) return PSD_OK;
     PSD_CUDA(cudaSetDevice(e->device));
-    double* tmp = nullptr;
-    PSD_CUDA(cudaMalloc(&tmp, (size_t)n * 5 * sizeof(double)));
-    const uint64_t* sad_edges = edge_slot ? e->edge[edge_slot].sad + 1 + first : nullptr;
-    int rc = psd_scan_content_edges(e->d_sums + 1 + first, sad_edges, n, e->P, weights, weight_abs_sum, tmp + n, tmp,
-                                    e->compute_stream);
-    if (!rc) rc = scan_to_host(e, tmp, out_content_val, (size_t)n);
-    if (!rc && out_components) rc = scan_to_host(e, tmp + n, out_components, (size_t)n * 4);
-    cudaFree(tmp);
+    ScanBuffer tmp;
+    PSD_CUDA(cudaMalloc(&tmp.p, (size_t)n * 5 * sizeof(double)));
+    const uint64_t* sad_edges = edge_slot ? e->edge[edge_slot].sads.at<uint64_t>(first) : nullptr;
+    int rc = psd_scan_content_edges(e->sums.at<psd_frame_sums>(first), sad_edges, n, e->P, weights, weight_abs_sum,
+                                    tmp.p + n, tmp.p, e->compute_stream);
+    if (!rc) rc = scan_to_host(e, tmp.p, out_content_val, (size_t)n);
+    if (!rc && out_components) rc = scan_to_host(e, tmp.p + n, out_components, (size_t)n * 4);
     return rc;
 }
 
@@ -850,16 +812,11 @@ int psd_engine_scan_adaptive_host(psd_engine* e, const double* scores_host, int6
     PSD_REQUIRE(e && scores_host && out_ratio && n >= 0, "psd_engine_scan_adaptive_host: bad argument");
     if (n == 0) return PSD_OK;
     PSD_CUDA(cudaSetDevice(e->device));
-    double* tmp = nullptr;
-    PSD_CUDA(cudaMalloc(&tmp, (size_t)n * 2 * sizeof(double)));
-    int rc = PSD_OK;
-    if (cudaMemcpyAsync(tmp, scores_host, (size_t)n * sizeof(double), cudaMemcpyHostToDevice, e->compute_stream) != cudaSuccess) {
-        set_error("scores upload failed"); rc = PSD_ERR_CUDA;
-    }
-    if (!rc) rc = psd_scan_adaptive(tmp, n, window_width, min_content_val, tmp + n, e->compute_stream);
-    if (!rc) rc = scan_to_host(e, tmp + n, out_ratio, (size_t)n);
-    cudaFree(tmp);
-    return rc;
+    ScanBuffer tmp;
+    PSD_CUDA(cudaMalloc(&tmp.p, (size_t)n * 2 * sizeof(double)));
+    PSD_CUDA(cudaMemcpyAsync(tmp.p, scores_host, (size_t)n * sizeof(double), cudaMemcpyHostToDevice, e->compute_stream));
+    int rc = psd_scan_adaptive(tmp.p, n, window_width, min_content_val, tmp.p + n, e->compute_stream);
+    return rc ? rc : scan_to_host(e, tmp.p + n, out_ratio, (size_t)n);
 }
 
 int psd_engine_scan_average_host(psd_engine* e, int64_t first, int64_t n, double* out_avg) {
@@ -867,12 +824,10 @@ int psd_engine_scan_average_host(psd_engine* e, int64_t first, int64_t n, double
     PSD_REQUIRE(first >= 0 && n >= 0 && first + n <= e->n_frames, "frame range out of bounds");
     if (n == 0) return PSD_OK;
     PSD_CUDA(cudaSetDevice(e->device));
-    double* tmp = nullptr;
-    PSD_CUDA(cudaMalloc(&tmp, (size_t)n * sizeof(double)));
-    int rc = psd_scan_average(e->d_sums + 1 + first, n, e->P * 3, tmp, e->compute_stream);
-    if (!rc) rc = scan_to_host(e, tmp, out_avg, (size_t)n);
-    cudaFree(tmp);
-    return rc;
+    ScanBuffer tmp;
+    PSD_CUDA(cudaMalloc(&tmp.p, (size_t)n * sizeof(double)));
+    int rc = psd_scan_average(e->sums.at<psd_frame_sums>(first), n, e->P * 3, tmp.p, e->compute_stream);
+    return rc ? rc : scan_to_host(e, tmp.p, out_avg, (size_t)n);
 }
 
 int psd_engine_scan_hist_correl_host(psd_engine* e, int64_t first, int64_t n, int32_t bins, double* out) {
@@ -881,14 +836,11 @@ int psd_engine_scan_hist_correl_host(psd_engine* e, int64_t first, int64_t n, in
     PSD_REQUIRE(first >= 0 && n >= 0 && first + n <= e->n_frames, "frame range out of bounds");
     if (n == 0) return PSD_OK;
     PSD_CUDA(cudaSetDevice(e->device));
-    double* tmp = nullptr;
-    PSD_CUDA(cudaMalloc(&tmp, (size_t)n * sizeof(double)));
-    // slot `first` (= stream frame first-1, or the halo slot) precedes slot first+1
-    const uint32_t* prev = (first > 0 || e->halo_scored) ? e->d_yhist + first * 256 : nullptr;
-    int rc = psd_scan_hist_correl(e->d_yhist + (first + 1) * 256, n, bins, prev, tmp, e->compute_stream);
-    if (!rc) rc = scan_to_host(e, tmp, out, (size_t)n);
-    cudaFree(tmp);
-    return rc;
+    ScanBuffer tmp;
+    PSD_CUDA(cudaMalloc(&tmp.p, (size_t)n * sizeof(double)));
+    int rc = psd_scan_hist_correl(e->yhist.at<uint32_t>(first), n, bins, previous_row<uint32_t>(e, e->yhist, first),
+                                  tmp.p, e->compute_stream);
+    return rc ? rc : scan_to_host(e, tmp.p, out, (size_t)n);
 }
 
 int psd_scan_hash_dist(const uint64_t* hashes, int64_t n, int32_t hash_size, const uint64_t* prev_hash, double* out,
@@ -905,16 +857,12 @@ int psd_engine_scan_hash_dist_host_at(psd_engine* e, int32_t hash_slot, int64_t 
     PSD_REQUIRE(first >= 0 && n >= 0 && first + n <= e->n_frames, "frame range out of bounds");
     if (n == 0) return PSD_OK;
     PSD_CUDA(cudaSetDevice(e->device));
-    double* tmp = nullptr;
-    PSD_CUDA(cudaMalloc(&tmp, (size_t)n * sizeof(double)));
-    const HashPlan& p = e->hash[hash_slot];
-    const uint64_t* h = e->d_hash[hash_slot];
-    // slot `first` (= stream frame first-1, or the halo slot) precedes slot first+1
-    const uint64_t* prev = (first > 0 || e->halo_scored) ? h + first * p.words : nullptr;
-    int rc = psd_scan_hash_dist(h + (first + 1) * p.words, n, p.size, prev, tmp, e->compute_stream);
-    if (!rc) rc = scan_to_host(e, tmp, out, (size_t)n);
-    cudaFree(tmp);
-    return rc;
+    ScanBuffer tmp;
+    PSD_CUDA(cudaMalloc(&tmp.p, (size_t)n * sizeof(double)));
+    const auto& h = e->hash[hash_slot];
+    int rc = psd_scan_hash_dist(h.rows.at<uint64_t>(first), n, h.plan.size, previous_row<uint64_t>(e, h.rows, first),
+                                tmp.p, e->compute_stream);
+    return rc ? rc : scan_to_host(e, tmp.p, out, (size_t)n);
 }
 
 int psd_engine_scan_hash_dist_host(psd_engine* e, int64_t first, int64_t n, double* out) {

@@ -82,6 +82,18 @@ inline bool layout_packed_bgr(const psd_frame_layout& l, int w) {
     return l.pixel_stride == 3 && l.channel_stride == 1 && l.row_stride == 3 * (int64_t)w;
 }
 
+// ---- per-frame result arrays of an engine (engine.cu) ----
+// Row 0 belongs to the halo frame, stream frame i sits at row i + 1: at() is the one place that mapping is made.
+struct FrameRows {
+    uint8_t* d = nullptr;
+    int64_t row_bytes = 0;
+    template <class T> T* at(int64_t frame) const { return reinterpret_cast<T*>(d + (frame + 1) * row_bytes); }
+    // cap zeroed rows holding the first `keep` rows of the current array, if there is one
+    int grow(int64_t cap, int64_t keep, cudaStream_t stream);
+    int zero(int64_t first, int64_t n, cudaStream_t stream) const;  // the rows of stream frames [first, first + n)
+    void release() { cudaFree(d); d = nullptr; }
+};
+
 // ---- edge path (edge_kernels.cu) ----
 struct EdgeBuffers {
     uint8_t* vplane;    // [n][P] V of HSV (written by the score pass)
@@ -96,18 +108,22 @@ struct EdgeBuffers {
     uint8_t* dirty;     // [2][n][tiles] hysteresis: tiles to revisit (double-buffered by round parity)
     int32_t* hyst_flags;// [3] hysteresis: "some tile changed" per round (rotating)
 };
+// the Canny scratch of batches of up to max_batch frames, and what the dilation of kernel size ksize needs
+int edge_buffers_create(EdgeBuffers* b, int W, int H, int max_batch, int ksize);
+int edge_buffers_add_ksize(EdgeBuffers* b, int W, int H, int max_batch, int ksize);  // another kernel size's needs
+void edge_buffers_destroy(EdgeBuffers* b);
 struct EdgeSlot {          // one dilation kernel size of an engine
     int ksize;
     uint32_t* carry_bits;  // [H][Wq] this size's dilated edges of the predecessor frame
-    uint64_t* sad;         // the batch's frame f accumulates into sad[f * sad_stride] (pre-zeroed)
-    int64_t sad_stride;    // uint64 words
+    FrameRows sads;        // a frame's SAD accumulates into the first uint64 of its row (pre-zeroed): slot 0's rows are
+                           // the sums' (psd_frame_sums::sad_edges, 8 words apart), every other slot owns one word a row
 };
-// Canny (thresholds, classify, hysteresis) once, then a dilation and a SAD per slot
-int launch_edges(const EdgeBuffers& b, int n, int width, int height, const EdgeSlot* slots, int n_slots,
+// Canny (thresholds, classify, hysteresis) once, then a dilation and a SAD per slot; the batch's frame 0 is stream
+// frame `first` of the slots' SAD rows
+int launch_edges(const EdgeBuffers& b, int n, int width, int height, const EdgeSlot* slots, int n_slots, int64_t first,
                  bool have_prev, cudaStream_t stream);
-int edge_unpack(const uint32_t* bits, uint8_t* out, int W, int H, bool tile_major, cudaStream_t stream);
-int64_t edge_tile_words(int W, int H);   // words per frame of a tile-major bit plane
-bool edge_dilate_separable(int ksize);  // this kernel size dilates in two passes through EdgeBuffers::bits_hdil
+// frame `index` of the last batch's Canny map (canny_map) or dilated map -> 0/255 bytes in b.tmp
+int edge_unpack(const EdgeBuffers& b, int64_t index, bool canny_map, int W, int H, cudaStream_t stream);
 int edge_dilate_check(int W, int ksize); // PSD_OK, or PSD_ERR_INVALID if a row of the separable pass is too wide
 
 // ---- perceptual hash (hash_kernels.cu) ----
