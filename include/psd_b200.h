@@ -286,6 +286,27 @@ int psd_sweep_eval(int64_t* cuts, const int32_t* count, int32_t n_cells, int32_t
                    const int32_t* tolerances, int32_t n_tol, void* workspace, size_t workspace_bytes,
                    int32_t* out_n_pred, int64_t* out_hard, int64_t* out_fades, void* stream);
 
+/* ---- many clips in one engine pass: clips scored back to back into one engine, then every clip's cuts ----
+ * A clip table is a DEVICE int64[n_clips + 1]: offsets[0] = 0, non-decreasing, offsets[n_clips] = n; clip j is
+ * frames [offsets[j], offsets[j+1]) of the pass. */
+/* After the psd_scan_* that filled values[n] over the whole pass: for every clip [b, e), values[i] = fill for i in
+ * [b, min(b + head, e)) and in [max(e - tail, b), e): CUDART_NAN (sign bit set) when fill_nan is 1, else `fill` as
+ * given, bit for bit.  This gives each clip the entries a one-clip engine's scan has there, in the scan's own bits:
+ * content_val head 1, 0.0 (content_detector.py:161-164); adaptive ratio head w, tail w, fill_nan, after the
+ * content_val fix-up (adaptive_detector.py:111-115); hist correl head 1, fill_nan; hash dist head 1, fill = the NaN
+ * with the sign bit clear that psd_scan_hash_dist writes (no predecessor); average_rgb none. */
+int psd_clip_fill(double* values, int64_t n, const int64_t* clip_offsets, int32_t n_clips, int32_t head, int32_t tail,
+                  int32_t fill_nan, double fill, void* stream);
+/* Every (cell, clip) automaton in one pass: cell k over clip j's slice of its metric arrays, with frame numbers from
+ * clip_first_frame[j] and min_frames[k * n_clips + j].  cells is a HOST array (validated as psd_sweep_cuts does,
+ * then copied on `stream`); everything else is DEVICE memory.  cut_offsets[n_cells * n_clips + 1] receives the
+ * exclusive offsets of the (cell, clip) cut lists, cell-major, and their total; cuts[cut_offsets[t] ..] the cuts
+ * of (cell, clip) t in emission order.  When the total exceeds cuts_cap, the offsets and the total are written and
+ * no cut is: grow the cut array and call again. */
+int psd_clip_cuts(const psd_sweep_cell* cells, int32_t n_cells, const int64_t* clip_offsets,
+                  const int64_t* clip_first_frame, int32_t n_clips, const int64_t* min_frames, int64_t* cuts,
+                  int64_t cuts_cap, int64_t* cut_offsets, void* stream);
+
 /* host-convenience wrappers: engine-owned sums -> host arrays (numpy), implies sync */
 int psd_engine_scan_content_host(psd_engine* e, int64_t first, int64_t n, const double weights[4],
                                  double weight_abs_sum, double* out_components,

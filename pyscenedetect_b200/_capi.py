@@ -162,6 +162,8 @@ SIGNATURES = {
     "psd_sweep_cuts": (C.c_int, [_vp, _i32, _i64, _i64, _vp, _vp, _i32, _vp]),
     "psd_sweep_eval": (C.c_int, [_vp, _vp, _i32, _i32, _i64, _vp, _i32, _vp, _i32, _vp, _i32, _vp, C.c_size_t,
                                  _vp, _vp, _vp, _vp]),
+    "psd_clip_fill": (C.c_int, [_vp, _i64, _vp, _i32, _i32, _i32, _i32, _dbl, _vp]),
+    "psd_clip_cuts": (C.c_int, [_vp, _i32, _vp, _vp, _i32, _vp, _vp, _i64, _vp, _vp]),
     "psd_engine_scan_content_host": (C.c_int, [_vp, _i64, _i64, _dp, _dbl, _vp, _vp]),
     "psd_engine_scan_adaptive_host": (C.c_int, [_vp, _vp, _i64, _i32, _dbl, _vp]),
     "psd_engine_scan_average_host": (C.c_int, [_vp, _i64, _i64, _vp]),

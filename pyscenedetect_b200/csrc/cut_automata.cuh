@@ -1,6 +1,7 @@
 // The five cut state machines as device functions: one thread walks one cell's frame sequence.  The
-// single-cell kernels of cut_kernels.cu (psd_cuts_*) and the batched kernel of sweep_kernels.cu
-// (psd_sweep_cuts, one thread per grid cell) both call these, so each automaton exists once.
+// single-cell kernels of cut_kernels.cu (psd_cuts_*) and the batched kernels of sweep_kernels.cu
+// (psd_sweep_cuts, one thread per grid cell) and clip_kernels.cu (psd_clip_cuts, one thread per (cell, clip))
+// all call these, so each automaton exists once.
 //   flash_filter_cuts   detector.py:160-224   (FlashFilter MERGE / SUPPRESS over `above(i)`)
 //   adaptive_cuts       adaptive_detector.py:134-143
 //   histogram_cuts      histogram_detector.py:87-112
@@ -133,6 +134,36 @@ __device__ __forceinline__ void threshold_cuts(const double* __restrict__ avg, i
     // post_process (threshold_detector.py:170-191) with timecode = last frame
     const int64_t last = first_frame + n - 1;
     if (!fade_in && add_final_scene && (last - last_scene_cut) >= min_frames) out.push(fade_frame);
+}
+
+// One psd_sweep_cell's automaton over the n frames of its metric arrays that start at index `base`, the first of
+// them frame `first_frame`.  psd_sweep_cuts (one thread per cell, base 0) and psd_clip_cuts (one thread per (cell,
+// clip), base = the clip's first index) both dispatch through here.
+__device__ __forceinline__ void run_cell(const psd_sweep_cell& c, int64_t base, int64_t n, int64_t first_frame,
+                                         int64_t min_frames, CutSink& out) {
+    const double* __restrict__ metric = c.metric + base;
+    switch (c.kind) {
+        case PSD_SWEEP_CONTENT: {
+            // content_detector.py:210 inside the automaton: no per-cell flag array
+            const double thr = c.threshold;
+            flash_filter_cuts([&](int64_t i) { return metric[i] >= thr; }, n, first_frame, min_frames, c.mode, out);
+            break;
+        }
+        case PSD_SWEEP_ADAPTIVE:
+            adaptive_cuts(metric, c.metric2 + base, n, first_frame, c.window, c.threshold, c.min_content_val,
+                          min_frames, out);
+            break;
+        case PSD_SWEEP_THRESHOLD:
+            threshold_cuts(metric, n, first_frame, c.threshold, c.mode, c.fade_bias, min_frames, c.add_final_scene,
+                           out);
+            break;
+        case PSD_SWEEP_HISTOGRAM:
+            histogram_cuts(metric, n, first_frame, c.threshold, min_frames, out);
+            break;
+        default:  // PSD_SWEEP_HASH (the host rejects any other kind)
+            hash_cuts(metric, n, first_frame, c.threshold, min_frames, out);
+            break;
+    }
 }
 
 }  // namespace psd

@@ -154,6 +154,10 @@ int launch_hash(const HashPlan* plans, int n_plans, const uint8_t* frames, int64
 int launch_hash_dist(const uint64_t* hashes, int64_t n, int size, const uint64_t* prev_hash, double* out,
                      cudaStream_t stream);
 
+// ---- cut automata over grid cells (sweep_kernels.cu) ----
+// the host-side checks of psd_sweep_cuts on an array of cells; `who` prefixes the error message
+int validate_sweep_cells(const psd_sweep_cell* cells, int32_t n_cells, const char* who);
+
 // ---- synthetic generator (synth_kernel.cu) ----
 int launch_synth(uint8_t* out, const int32_t* d_params, int64_t n, int width, int height,
                  int64_t frame_stride, cudaStream_t stream);

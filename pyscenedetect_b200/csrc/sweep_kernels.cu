@@ -20,29 +20,7 @@ __global__ void __launch_bounds__(128) psd_sweep_cuts_kernel(const psd_sweep_cel
     if (k >= n_cells) return;
     const psd_sweep_cell c = cells[k];
     CutSink out{cuts + (int64_t)k * cap, cap, 0};
-    switch (c.kind) {
-        case PSD_SWEEP_CONTENT: {
-            // content_detector.py:210 inside the automaton: no per-cell flag array
-            const double* __restrict__ val = c.metric;
-            const double thr = c.threshold;
-            flash_filter_cuts([&](int64_t i) { return val[i] >= thr; }, n, first_frame, c.min_frames, c.mode, out);
-            break;
-        }
-        case PSD_SWEEP_ADAPTIVE:
-            adaptive_cuts(c.metric, c.metric2, n, first_frame, c.window, c.threshold, c.min_content_val,
-                          c.min_frames, out);
-            break;
-        case PSD_SWEEP_THRESHOLD:
-            threshold_cuts(c.metric, n, first_frame, c.threshold, c.mode, c.fade_bias, c.min_frames,
-                           c.add_final_scene, out);
-            break;
-        case PSD_SWEEP_HISTOGRAM:
-            histogram_cuts(c.metric, n, first_frame, c.threshold, c.min_frames, out);
-            break;
-        default:  // PSD_SWEEP_HASH (the host rejects any other kind)
-            hash_cuts(c.metric, n, first_frame, c.threshold, c.min_frames, out);
-            break;
-    }
+    run_cell(c, 0, n, first_frame, c.min_frames, out);
     count[k] = out.n;
 }
 
@@ -174,6 +152,23 @@ __global__ void __launch_bounds__(128) psd_sweep_eval_kernel(
 
 static inline int32_t words_for(int64_t bits) { return (int32_t)((bits + 31) / 32); }
 
+int validate_sweep_cells(const psd_sweep_cell* cells, int32_t n_cells, const char* who) {
+    PSD_REQUIRE(n_cells == 0 || cells, "%s: no cells", who);
+    for (int32_t k = 0; k < n_cells; ++k) {
+        const psd_sweep_cell& c = cells[k];
+        PSD_REQUIRE(c.kind >= PSD_SWEEP_CONTENT && c.kind <= PSD_SWEEP_HASH, "%s: cell %d: unknown kind %d", who, k,
+                    c.kind);
+        PSD_REQUIRE(c.metric, "%s: cell %d: no metric array", who, k);
+        PSD_REQUIRE(c.mode == 0 || ((c.kind == PSD_SWEEP_CONTENT || c.kind == PSD_SWEEP_THRESHOLD) && c.mode == 1),
+                    "%s: cell %d: bad mode %d", who, k, c.mode);
+        PSD_REQUIRE(c.kind != PSD_SWEEP_ADAPTIVE || (c.metric2 && c.window >= 1),
+                    "%s: cell %d: adaptive cells need metric2 and window >= 1", who, k);
+        PSD_REQUIRE(c.add_final_scene == 0 || (c.kind == PSD_SWEEP_THRESHOLD && c.add_final_scene == 1),
+                    "%s: cell %d: bad add_final_scene", who, k);
+    }
+    return PSD_OK;
+}
+
 }  // namespace psd
 
 using namespace psd;
@@ -183,18 +178,8 @@ extern "C" int psd_sweep_cuts(const psd_sweep_cell* cells, int32_t n_cells, int6
     PSD_REQUIRE(n_cells >= 0 && n >= 0 && cap >= 0, "psd_sweep_cuts: bad args");
     if (n_cells == 0) return PSD_OK;
     PSD_REQUIRE(cells && cuts && count, "psd_sweep_cuts: bad args");
-    for (int32_t k = 0; k < n_cells; ++k) {
-        const psd_sweep_cell& c = cells[k];
-        PSD_REQUIRE(c.kind >= PSD_SWEEP_CONTENT && c.kind <= PSD_SWEEP_HASH, "psd_sweep_cuts: cell %d: unknown kind %d",
-                    k, c.kind);
-        PSD_REQUIRE(c.metric, "psd_sweep_cuts: cell %d: no metric array", k);
-        PSD_REQUIRE(c.mode == 0 || ((c.kind == PSD_SWEEP_CONTENT || c.kind == PSD_SWEEP_THRESHOLD) && c.mode == 1),
-                    "psd_sweep_cuts: cell %d: bad mode %d", k, c.mode);
-        PSD_REQUIRE(c.kind != PSD_SWEEP_ADAPTIVE || (c.metric2 && c.window >= 1),
-                    "psd_sweep_cuts: cell %d: adaptive cells need metric2 and window >= 1", k);
-        PSD_REQUIRE(c.add_final_scene == 0 || (c.kind == PSD_SWEEP_THRESHOLD && c.add_final_scene == 1),
-                    "psd_sweep_cuts: cell %d: bad add_final_scene", k);
-    }
+    const int rc = validate_sweep_cells(cells, n_cells, "psd_sweep_cuts");
+    if (rc != PSD_OK) return rc;
     cudaStream_t s = (cudaStream_t)stream;
     psd_sweep_cell* d_cells = nullptr;
     const size_t bytes = sizeof(psd_sweep_cell) * (size_t)n_cells;

@@ -57,12 +57,38 @@ def min_len_frames(length, fps) -> int:
     raise TypeError("unsupported min_scene_len")
 
 
-def scan_metric(lib, holder, key: tuple, out: int, content_val: int | None = None) -> None:
+def scan_metric(lib, holder, key: tuple, out: int, content_val: int | None = None,
+                clips: tuple[int, int] | None = None) -> None:
     """Launch the psd_scan_* that fills one metric array `out` (float64 per frame) from every frame a result holder
     (an Engine, a `SlotView` of one or `sharding.GatheredResults`) holds, on the holder's stream.  `key` is a
     `ParameterSweep` metric key without its group index: ("content_val", weights), ("adaptive_ratio", weights,
     window_width, min_content_val), which reads `content_val` (that weight vector's array), ("average_rgb",),
-    ("hist_correl", bins) or ("hash_dist",)."""
+    ("hist_correl", bins) or ("hash_dist",).
+
+    `clips` = (device clip table, clip count) when the holder's frames are several clips scored back to back
+    (psd_clip_fill): the scan is followed by the fix-up that gives every clip's first (and, for the adaptive ratio,
+    last) entries the values a one-clip engine's scan has there, so each clip's slice equals that engine's array
+    byte for byte.  An adaptive ratio must read a `content_val` array that was fixed up the same way."""
+    _scan_metric(lib, holder, key, out, content_val)
+    if clips is None or key[0] == "average_rgb":  # average_rgb is per frame: nothing crosses a clip edge
+        return
+    table, n_clips = clips
+    # the value a one-clip scan writes there, in the scan's own bits: psd_scan_adaptive and psd_scan_hist_correl
+    # write CUDART_NAN (fill_nan 1), psd_scan_hash_dist the NaN with the sign bit clear, which is Python's
+    fill = 0.0
+    if key[0] == "content_val":      # the first frame scores 0.0 (content_detector.py:161-164)
+        head, tail, nan = 1, 0, 0
+    elif key[0] == "adaptive_ratio":  # the window is incomplete (adaptive_detector.py:111-115)
+        head, tail, nan = int(key[2]), int(key[2]), 1
+    elif key[0] == "hist_correl":     # no predecessor (histogram_detector.py:98)
+        head, tail, nan = 1, 0, 1
+    else:                             # hash_dist: no predecessor (hash_detector.py:82)
+        head, tail, nan, fill = 1, 0, 0, float("nan")
+    check(lib.psd_clip_fill(out, holder.frame_count, table, n_clips, head, tail, nan, fill, holder.compute_stream),
+          "psd_clip_fill")
+
+
+def _scan_metric(lib, holder, key: tuple, out: int, content_val: int | None) -> None:
     n, st = holder.frame_count, holder.compute_stream
     kind = key[0]
     if kind == "content_val":

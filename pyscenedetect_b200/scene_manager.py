@@ -195,6 +195,12 @@ class FrameBatches:
         self._which ^= 1
         return tcs, batch, (not zero_copy) or bool(getattr(video, "is_pinned", False))
 
+    def resume(self) -> None:
+        """Read on after `next()` returned None, from a stream that reports an end and can then be read past it
+        (clips.py's chain of clips pauses at a clip boundary so that the engine can be emptied).  The buffers are
+        kept: the caller has synchronised every engine that read them."""
+        self._done = False
+
     def close(self) -> None:
         for p in self._pinned:
             if p is not None:
