@@ -306,6 +306,26 @@ int psd_clip_fill(double* values, int64_t n, const int64_t* clip_offsets, int32_
 int psd_clip_cuts(const psd_sweep_cell* cells, int32_t n_cells, const int64_t* clip_offsets,
                   const int64_t* clip_first_frame, int32_t n_clips, const int64_t* min_frames, int64_t* cuts,
                   int64_t cuts_cap, int64_t* cut_offsets, void* stream);
+/* benchmark/evaluator.py:227-331 (score_video) for every (cell, clip, tolerance) on psd_clip_cuts' output, and the
+ * counts summed over the clips (evaluator.py:167-186).  cuts / cut_offsets are psd_clip_cuts' arrays and cuts_total
+ * its total cut_offsets[n_cells * n_clips]; each (cell, clip) list is first turned, in place, into the predicted list
+ * of benchmark/sweep.py:169 (sorted unique cuts followed by clip_end_frame[clip], or nothing when there is no cut) and
+ * out_n_pred[cell * n_clips + clip] is its length (-1: more than max_cuts cuts, not scored).  Clip j's ground truth
+ * is gt_cuts[gt_offsets[j] .. gt_offsets[j+1]) (strictly increasing) and fades[fade_offsets[j] ..
+ * fade_offsets[j+1])[2] (inclusive), matched as psd_sweep_eval matches.  Outputs:
+ *   out_hard[n_cells][n_clips][n_tol][5]  matched, false_positives, missed, offset_sum, offset_count
+ *   out_fades[n_cells][n_clips][3]        matched, false_positives, missed
+ *   out_totals_hard[n_cells][n_tol][5], out_totals_fades[n_cells][3]: the same summed over the clips
+ *   out_over[1]                           the lowest cell * n_clips + clip with more than max_cuts cuts, or -1
+ * tolerances is a HOST array (n_tol <= PSD_SWEEP_MAX_TOLERANCES); every other pointer is a DEVICE pointer.
+ * workspace holds the matching bitmaps: 4 * (n_tol * (n_cells * n_clips + ceil(cuts_total / 32))
+ * + n_cells * n_tol * (2 * n_clips + ceil(n_gt / 32) + ceil(n_fades / 32))) bytes. */
+int psd_clip_eval(int64_t* cuts, const int64_t* cut_offsets, int32_t n_cells, int32_t n_clips, int64_t cuts_total,
+                  int64_t max_cuts, const int64_t* clip_end_frame, const int64_t* gt_offsets, const int64_t* gt_cuts,
+                  int32_t n_gt, const int64_t* fade_offsets, const int64_t* fades, int32_t n_fades,
+                  const int32_t* tolerances, int32_t n_tol, void* workspace, size_t workspace_bytes,
+                  int32_t* out_n_pred, int64_t* out_hard, int64_t* out_fades, int64_t* out_totals_hard,
+                  int64_t* out_totals_fades, int64_t* out_over, void* stream);
 
 /* host-convenience wrappers: engine-owned sums -> host arrays (numpy), implies sync */
 int psd_engine_scan_content_host(psd_engine* e, int64_t first, int64_t n, const double weights[4],

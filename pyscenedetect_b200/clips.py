@@ -154,28 +154,60 @@ class _DeviceClipChain(_ClipChain):
         return None
 
 
-class _Pass:
-    """The device half of a `detect_clips` call: the detectors' cells and metric keys, the metric arrays, clip table
-    and cut buffers (reused pass after pass and group after group; they only grow), and the step that turns an
-    engine's pass into every clip's cut list."""
+@dataclass
+class PassCuts:
+    """One pass's (cell, clip) cut lists in device memory, which this object owns: cell k's cuts in clip j are
+    cuts[offsets[k * n_clips + j] .. offsets[k * n_clips + j + 1]), in emission order.  `table` holds the clip table
+    psd_clip_cuts read: offsets[n_clips + 1], first frames[n_clips], end frames[n_clips] (what
+    `SceneManager.get_scene_list` ends at: the last position + 1), then min_frames[n_cells * n_clips]."""
 
-    def __init__(self, detectors, device: int):
+    clips: list                 # ClipResult of every clip scored, in pass order
+    n_cells: int
+    table: DeviceBuffer
+    offsets: DeviceBuffer       # int64[n_cells * n_clips + 1]: exclusive offsets, then the total
+    cuts: DeviceBuffer
+    total: int
+
+    @property
+    def n_clips(self) -> int:
+        return len(self.clips)
+
+    @property
+    def end_frames(self) -> int:
+        """Device pointer to the int64 end frame of every clip."""
+        return self.table.ptr + (2 * self.n_clips + 1) * 8
+
+    def close(self) -> None:
+        for b in (self.table, self.offsets, self.cuts):
+            b.close()
+
+
+class _Pass:
+    """The device half of a many-clip pass: the cells' metric keys and metric arrays (reused pass after pass and
+    group after group; they only grow), and the step that turns an engine's pass into every (cell, clip) cut list.
+    `cells` are CellPlans over `groups`, the pixel groups whose results each engine holds as slots."""
+
+    def __init__(self, cells, groups, device: int):
         self._lib = _capi.load()
         self.device = device
-        self.groups, gi = [], {}
-        self.cells = []
-        for d in detectors:
-            g = pixel_group_of(d)
-            if g not in gi:
-                gi[g] = len(self.groups)
-                self.groups.append(g)
-            self.cells.append(plan_cell(d, gi[g]))
+        self.cells, self.groups = list(cells), list(groups)
         self.keys = []  # metric keys in order of first use: content_val before the adaptive ratio that reads it
         for c in self.cells:
             for key in (c.metric2, c.metric):
                 if key is not None and key not in self.keys:
                     self.keys.append(key)
         self._bufs = {}
+
+    @classmethod
+    def of_detectors(cls, detectors, device: int) -> _Pass:
+        groups, gi, cells = [], {}, []
+        for d in detectors:
+            g = pixel_group_of(d)
+            if g not in gi:
+                gi[g] = len(groups)
+                groups.append(g)
+            cells.append(plan_cell(d, gi[g]))
+        return cls(cells, groups, device)
 
     def _buf(self, name, nbytes: int) -> DeviceBuffer:
         b = self._bufs.get(name)
@@ -190,14 +222,14 @@ class _Pass:
             b.close()
         self._bufs = {}
 
-    def finish(self, engine, holders, clips: list) -> None:
-        """Every clip of `clips` ((ClipResult, frames scored) of the frames `engine` holds, in order) gets its cut
-        frames."""
+    def cuts(self, engine, holders, clips: list) -> PassCuts | None:
+        """Every (cell, clip) cut list of `clips` ((ClipResult, frames scored) of the frames `engine` holds, in
+        order), left in device memory; None when no clip has a frame.  Only the cut total comes back to the host."""
         lib = self._lib
         scored = [r for r, m in clips if m]
         n = engine.frame_count
         if not scored:
-            return
+            return None
         c, k = len(scored), len(self.cells)
         sizes = np.array([m for _, m in clips if m], dtype=np.int64)
         if int(sizes.sum()) != n:
@@ -205,10 +237,11 @@ class _Pass:
         table = np.concatenate([
             np.concatenate([[0], np.cumsum(sizes)]),
             [r.start.frame_num for r in scored],
+            [r.end.frame_num + 1 for r in scored],
             [cell.min_frames(r.fps) for cell in self.cells for r in scored]]).astype(np.int64)
-        tbuf = self._buf("table", table.nbytes)
+        tbuf = DeviceBuffer(table.nbytes, self.device)
         tbuf.upload(table)
-        offsets, first, min_frames = tbuf.ptr, tbuf.ptr + (c + 1) * 8, tbuf.ptr + (2 * c + 1) * 8
+        offsets, first, min_frames = tbuf.ptr, tbuf.ptr + (c + 1) * 8, tbuf.ptr + (3 * c + 1) * 8
         arrays = {key: self._buf(key, n * 8) for key in self.keys}
         for key in self.keys:
             val = arrays[("content_val",) + key[1:3]].ptr if key[0] == "adaptive_ratio" else None
@@ -220,26 +253,38 @@ class _Pass:
                 metric2=arrays[cell.metric2].ptr if cell.metric2 is not None else None, threshold=cell.threshold,
                 min_content_val=cell.min_content_val, fade_bias=cell.fade_bias, min_frames=0, window=cell.window,
                 add_final_scene=cell.add_final_scene)
-        obuf = self._buf("cut_offsets", (k * c + 1) * 8)
+        obuf = DeviceBuffer((k * c + 1) * 8, self.device)
         cap = max(1, int(n * FIRST_CUTS_PER_FRAME)) if FIRST_CUTS_PER_FRAME > 0 else 0
-        cuts = self._buf("cuts", cap * 8)
+        cuts = DeviceBuffer(max(8, cap * 8), self.device)
         cap = cuts.nbytes // 8
         st = engine.compute_stream
         for attempt in range(2):
             check(lib.psd_clip_cuts(cells, k, offsets, first, c, min_frames, cuts.ptr, cap, obuf.ptr, st),
                   "psd_clip_cuts")
             engine.sync()
-            offs = obuf.download((k * c + 1) * 8).view(np.int64)
-            total = int(offs[-1])
+            total = int(obuf.download(8, offset=k * c * 8).view(np.int64)[0])
             if total <= cap:
                 break
             if attempt:
                 raise RuntimeError(f"psd_clip_cuts needs {total} cuts after growing its buffer to {cap}")
-            cuts = self._buf("cuts", total * 8)
+            cuts.close()
+            cuts = DeviceBuffer(total * 8, self.device)
             cap = cuts.nbytes // 8
-        got = cuts.download(total * 8).view(np.int64).tolist() if total else []
-        offs = offs.tolist()
-        for j, r in enumerate(scored):  # (cell i, clip j) is list i * c + j: SceneManager.get_cut_list per clip
+        return PassCuts(scored, k, tbuf, obuf, cuts, total)
+
+    def finish(self, engine, holders, clips: list) -> None:
+        """Every clip of `clips` ((ClipResult, frames scored) of the frames `engine` holds, in order) gets its cut
+        frames: the union of every cell's cuts, as SceneManager.get_cut_list gives them."""
+        pc = self.cuts(engine, holders, clips)
+        if pc is None:
+            return
+        try:
+            k, c = pc.n_cells, pc.n_clips
+            offs = pc.offsets.download((k * c + 1) * 8).view(np.int64).tolist()
+            got = pc.cuts.download(pc.total * 8).view(np.int64).tolist() if pc.total else []
+        finally:
+            pc.close()
+        for j, r in enumerate(pc.clips):  # (cell i, clip j) is list i * c + j: SceneManager.get_cut_list per clip
             r.cut_frames = sorted({f for i in range(k) for f in got[offs[i * c + j]:offs[i * c + j + 1]]})
 
 
@@ -273,43 +318,55 @@ def detect_clips(videos, detectors, auto_downscale: bool = True, downscale: int 
     geometry = SceneManager(device=device, batch_size=batch_size)
     geometry._auto_downscale, geometry._downscale = bool(auto_downscale), int(downscale)
     videos = list(videos)
-    groups: dict = {}
-    for i, v in enumerate(videos):
-        groups.setdefault(_group_key(v), []).append((i, v))
     results: list = [None] * len(videos)
-    device_pass = _Pass(detectors, device)
+    device_pass = _Pass.of_detectors(detectors, device)
+    passes = clip_passes(videos, device_pass.groups, geometry, batch_size, device)
     try:
-        for (size, on_cuda, views, order), clips in groups.items():
-            box, (w, h), (sw, sh) = geometry._geometry(*size)
-            engine, holders = shared_engine(device_pass.groups, w, h, sw, sh, device=device, max_batch=batch_size)
-            chain = (_DeviceClipChain if views else _ClipChain)(clips, MAX_PASS_FRAMES, on_cuda)
-            gather = FrameBatches(chain, box, (w, h), batch_size)
-            try:
-                while True:
-                    item = gather.next()  # overlaps the GPU's work on the previous batch
-                    engine.sync()         # retire the previous batch before its buffer is reused
-                    if item is None:
-                        device_pass.finish(engine, holders, [(r, m) for _, r, m in chain.done])
-                        for index, r, _ in chain.done:
-                            results[index] = r
-                        if not chain.paused:
-                            break
-                        engine.reset()
-                        chain.resume()
-                        gather.resume()
-                        continue
-                    _tcs, frames, pinned = item
-                    if isinstance(frames, np.ndarray):
-                        engine.submit(frames, pinned=pinned)
-                    else:  # CUDA frames: a view of one clip, or a list of frames from streams without read_batch
-                        for f in (frames if isinstance(frames, list) else [frames]):
-                            engine.submit(f, channel_order=order)
-            finally:
-                gather.close()
-                engine.close()
+        for engine, holders, done in passes:
+            device_pass.finish(engine, holders, [(r, m) for _, r, m in done])
+            for index, r, _ in done:
+                results[index] = r
     finally:
+        passes.close()
         device_pass.close()
     return results
+
+
+def clip_passes(videos, groups, geometry, batch_size: int, device: int):
+    """Score the streams of `videos` pass by pass: clips grouped by `_group_key`, one engine per group built by
+    `shared_engine` with every pixel group of `groups` as a slot and `geometry._geometry` (a SceneManager's), the
+    clips of a group scored back to back.  Yields (engine, holders, done) at the end of every pass, `done` being
+    [(input index, ClipResult, frames scored)] of the clips the engine holds, in order; the engine is reset for the
+    next pass when the consumer asks for it.  Close the generator to release the engine of an unfinished group."""
+    by_key: dict = {}
+    for i, v in enumerate(videos):
+        by_key.setdefault(_group_key(v), []).append((i, v))
+    for (size, on_cuda, views, order), clips in by_key.items():
+        box, (w, h), (sw, sh) = geometry._geometry(*size)
+        engine, holders = shared_engine(groups, w, h, sw, sh, device=device, max_batch=batch_size)
+        chain = (_DeviceClipChain if views else _ClipChain)(clips, MAX_PASS_FRAMES, on_cuda)
+        gather = FrameBatches(chain, box, (w, h), batch_size)
+        try:
+            while True:
+                item = gather.next()  # overlaps the GPU's work on the previous batch
+                engine.sync()         # retire the previous batch before its buffer is reused
+                if item is None:
+                    yield engine, holders, chain.done
+                    if not chain.paused:
+                        break
+                    engine.reset()
+                    chain.resume()
+                    gather.resume()
+                    continue
+                _tcs, frames, pinned = item
+                if isinstance(frames, np.ndarray):
+                    engine.submit(frames, pinned=pinned)
+                else:  # CUDA frames: a view of one clip, or a list of frames from streams without read_batch
+                    for f in (frames if isinstance(frames, list) else [frames]):
+                        engine.submit(f, channel_order=order)
+        finally:
+            gather.close()
+            engine.close()
 
 
 __all__ = ["detect_clips", "ClipResult", "MAX_PASS_FRAMES"]

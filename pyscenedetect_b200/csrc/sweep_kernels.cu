@@ -5,10 +5,12 @@
 //                    each frame's value together (one broadcast load per warp) and take the same branch
 //                    most of the time: they only diverge on the frames where some of them cut.
 //   psd_sweep_eval   benchmark/evaluator.py:227-331 (score_video) per (cell, tolerance): first the
-//                    predicted list of sweep.py:169, then fade matching, then greedy hard-cut matching.
+//                    predicted list of sweep.py:169, then fade matching, then greedy hard-cut matching
+//                    (sweep_eval.cuh, shared with psd_clip_eval).
 // The automata are sequential walks, so the sweep is bounded by one thread's latency per frame (a load, a
 // compare, a few integer ops): G cells cost about as much as one cell until the cells fill the GPU.
 #include "cut_automata.cuh"
+#include "sweep_eval.cuh"
 
 namespace psd {
 
@@ -26,8 +28,6 @@ __global__ void __launch_bounds__(128) psd_sweep_cuts_kernel(const psd_sweep_cel
 
 // Cell k's cut slice -> the predicted list of sweep.py:169, in place: sorted(set(cuts)), then end_frame
 // when there is a cut.  The end is not stored (the slice may be full): entry n_pred - 1 is end_frame.
-// Insertion sort is linear on the strictly increasing lists every automaton but a |fade_bias| > 1
-// ThresholdDetector emits (cut_automata.cuh).
 __global__ void __launch_bounds__(128) psd_sweep_pred_kernel(int64_t* __restrict__ cuts,
                                                              const int32_t* __restrict__ count, int32_t n_cells,
                                                              int32_t cap, int32_t* __restrict__ n_pred) {
@@ -38,48 +38,11 @@ __global__ void __launch_bounds__(128) psd_sweep_pred_kernel(int64_t* __restrict
         n_pred[k] = -1;
         return;
     }
-    int64_t* p = cuts + (int64_t)k * cap;
-    for (int32_t i = 1; i < c; ++i) {
-        const int64_t v = p[i];
-        int32_t j = i - 1;
-        if (p[j] <= v) continue;
-        while (j >= 0 && p[j] > v) {
-            p[j + 1] = p[j];
-            --j;
-        }
-        p[j + 1] = v;
-    }
-    int32_t u = 0;
-    for (int32_t i = 0; i < c; ++i)
-        if (u == 0 || p[i] != p[u - 1]) p[u++] = p[i];
+    const int32_t u = sort_unique(cuts + (int64_t)k * cap, c);
     n_pred[k] = u ? u + 1 : 0;
 }
 
-struct Tolerances {
-    int32_t t[PSD_SWEEP_MAX_TOLERANCES];
-};
-
-__device__ __forceinline__ bool bit_test_set(uint32_t* bits, int32_t i) {
-    const uint32_t m = 1u << (i & 31);
-    const bool was = (bits[i >> 5] & m) != 0;
-    bits[i >> 5] |= m;
-    return was;
-}
-
-__device__ __forceinline__ int32_t find_frame(const int64_t* __restrict__ gt, int32_t n_gt, int64_t g) {
-    int32_t lo = 0, hi = n_gt;  // first index with gt[index] >= g
-    while (lo < hi) {
-        const int32_t mid = (lo + hi) >> 1;
-        if (gt[mid] < g) lo = mid + 1;
-        else hi = mid;
-    }
-    return (lo < n_gt && gt[lo] == g) ? lo : -1;
-}
-
-// One thread per (cell, tolerance).  Hard-cut matching (evaluator.py:227-266) claims (d, i, j) pairs in
-// sorted order.  With strictly increasing ground truth a prediction p_i has at most two partners at
-// distance d, g = p_i - d before g = p_i + d in j order, so the sorted walk is: for d = 0..tol, for i in
-// order, claim (i, p_i - d) else (i, p_i + d) if both sides are unused.  No candidate list is built.
+// One thread per (cell, tolerance): score_predictions (sweep_eval.cuh) on the cell's predicted list.
 __global__ void __launch_bounds__(128) psd_sweep_eval_kernel(
     const int64_t* __restrict__ cuts, const int32_t* __restrict__ n_pred, int32_t n_cells, int32_t cap,
     int64_t end_frame, const int64_t* __restrict__ gt, int32_t n_gt, const int64_t* __restrict__ fades,
@@ -96,61 +59,12 @@ __global__ void __launch_bounds__(128) psd_sweep_eval_kernel(
             for (int r = 0; r < 3; ++r) out_fades[(int64_t)k * 3 + r] = 0;
         return;
     }
-    const int64_t* p = cuts + (int64_t)k * cap;
-    auto pred = [&](int32_t i) { return i < np - 1 ? p[i] : end_frame; };
     uint32_t* used_p = workspace + tid * (int64_t)(words_p + words_g + words_f);
-    uint32_t* used_g = used_p + words_p;
-    uint32_t* used_f = used_g + words_g;
     for (int32_t w = 0; w < words_p + words_g + words_f; ++w) used_p[w] = 0u;
-
-    // fades (evaluator.py:269-304): first interval containing the prediction consumes it
-    int64_t fm = 0, ffp = 0, remaining = np;
-    for (int32_t i = 0; i < np; ++i) {
-        const int64_t v = pred(i);
-        for (int32_t f = 0; f < n_fades; ++f) {
-            if (fades[2 * f] <= v && v <= fades[2 * f + 1]) {
-                bit_test_set(used_p, i);
-                --remaining;
-                if (bit_test_set(used_f, f)) ++ffp;
-                else ++fm;
-                break;
-            }
-        }
-    }
-    // hard cuts on the predictions no fade consumed
-    int32_t tol = 0;  // a select, not tols.t[q]: a dynamic index would copy the array to local memory
-#pragma unroll
-    for (int r = 0; r < PSD_SWEEP_MAX_TOLERANCES; ++r)
-        if (r == q) tol = tols.t[r];
-    int64_t matched = 0, offset_sum = 0;
-    for (int32_t d = 0; d <= tol; ++d) {
-        for (int32_t i = 0; i < np; ++i) {
-            if (used_p[i >> 5] & (1u << (i & 31))) continue;
-            const int64_t v = pred(i);
-            int32_t j = find_frame(gt, n_gt, v - d);
-            if (j < 0 || (used_g[j >> 5] & (1u << (j & 31)))) {
-                j = d ? find_frame(gt, n_gt, v + d) : -1;
-                if (j < 0 || (used_g[j >> 5] & (1u << (j & 31)))) continue;
-            }
-            bit_test_set(used_g, j);
-            bit_test_set(used_p, i);
-            ++matched;
-            offset_sum += d;
-        }
-    }
-    hard[0] = matched;
-    hard[1] = remaining - matched;
-    hard[2] = n_gt - matched;
-    hard[3] = offset_sum;
-    hard[4] = matched;
-    if (q == 0) {
-        out_fades[(int64_t)k * 3 + 0] = fm;
-        out_fades[(int64_t)k * 3 + 1] = ffp;
-        out_fades[(int64_t)k * 3 + 2] = n_fades - fm;
-    }
+    score_predictions(cuts + (int64_t)k * cap, np, end_frame, gt, n_gt, fades, n_fades, tolerance_at(tols, q), used_p,
+                      used_p + words_p, used_p + words_p + words_g, hard,
+                      q == 0 ? out_fades + (int64_t)k * 3 : nullptr);
 }
-
-static inline int32_t words_for(int64_t bits) { return (int32_t)((bits + 31) / 32); }
 
 int validate_sweep_cells(const psd_sweep_cell* cells, int32_t n_cells, const char* who) {
     PSD_REQUIRE(n_cells == 0 || cells, "%s: no cells", who);
@@ -208,7 +122,8 @@ extern "C" int psd_sweep_eval(int64_t* cuts, const int32_t* count, int32_t n_cel
     PSD_REQUIRE(cuts && count && out_n_pred && out_hard && out_fades, "psd_sweep_eval: bad args");
     PSD_REQUIRE(n_gt == 0 || gt_cuts, "psd_sweep_eval: gt_cuts is NULL");
     PSD_REQUIRE(n_fades == 0 || fades, "psd_sweep_eval: fades is NULL");
-    const int32_t wp = words_for((int64_t)cap + 1), wg = words_for(n_gt), wf = words_for(n_fades);
+    const int32_t wp = (int32_t)words_for((int64_t)cap + 1), wg = (int32_t)words_for(n_gt);
+    const int32_t wf = (int32_t)words_for(n_fades);
     const int64_t threads = (int64_t)n_cells * n_tol;
     const size_t need = (size_t)threads * 4u * (size_t)(wp + wg + wf);
     PSD_REQUIRE(workspace && workspace_bytes >= need, "psd_sweep_eval: workspace needs %zu bytes", need);

@@ -200,6 +200,121 @@ class SweepResult:
         return int(f[0]), int(f[1]), int(f[2])
 
 
+def _cell_totals(grid, tolerances, th, tf) -> list[CellTotals]:
+    """CellTotals per cell from summed counts th[cell][tolerance][5] and tf[cell][3], in grid order."""
+    out = []
+    for k, params in enumerate(grid):
+        h, f = th[k], tf[k]
+        out.append(CellTotals(
+            params=params,
+            hard={t: EventCounts(int(h[q, 0]), int(h[q, 1]), int(h[q, 2])) for q, t in enumerate(tolerances)},
+            hard_offset={t: (float(h[q, 3]), int(h[q, 4])) for q, t in enumerate(tolerances)},
+            fades=EventCounts(int(f[0]), int(f[1]), int(f[2]))))
+    return out
+
+
+def clip_eval_workspace_bytes(n_cells: int, n_clips: int, n_tol: int, cuts_total: int, n_gt: int,
+                              n_fades: int) -> int:
+    """The matching bitmaps psd_clip_eval needs (include/psd_b200.h), from sizes the host already has."""
+    words = lambda bits: -(-bits // 32)  # noqa: E731
+    return 4 * (n_tol * (n_cells * n_clips + words(cuts_total))
+                + n_cells * n_tol * (2 * n_clips + words(n_gt) + words(n_fades)))
+
+
+class _ClipPass:
+    """One pass of `run_clips`: psd_clip_cuts' and psd_clip_eval's per-(cell, clip) arrays in device memory, owned
+    here; each array is downloaded once, by the first accessor that reads it."""
+
+    def __init__(self, pc, n_tol, n_pred, hard, fades):
+        self.c, self.n_tol = pc.n_clips, n_tol
+        self._bufs = {"offsets": (pc.offsets, np.int64, (-1,)), "n_pred": (n_pred, np.int32, (-1,)),
+                      "hard": (hard, np.int64, (-1, n_tol, 5)), "fades": (fades, np.int64, (-1, 3))}
+        self.cuts_buf = pc.cuts
+        self._host = {}
+
+    def host(self, name) -> np.ndarray:
+        if name not in self._host:
+            buf, dtype, shape = self._bufs[name]
+            self._host[name] = buf.download(buf.nbytes).view(dtype).reshape(shape)
+        return self._host[name]
+
+
+class ClipSweepResult:
+    """Every (cell, clip) of one `ParameterSweep.run_clips` call.  Per-(cell, clip) counts and cut lists stay in
+    device memory until an accessor reads them; `totals` holds this call's counts summed over its clips."""
+
+    def __init__(self, grid, tolerances, passes, where, end_frames, totals_hard, totals_fades, grid_ms):
+        self.grid = grid
+        self.tolerances = tuple(tolerances)
+        self._passes = passes        # [_ClipPass]
+        self._where = where          # clip -> (pass index, index within the pass)
+        self._end = end_frames
+        self._th, self._tf = totals_hard, totals_fades
+        self.grid_ms = grid_ms       # scans + psd_clip_cuts + psd_clip_eval of every pass, host clock ending in syncs
+
+    def __len__(self) -> int:
+        return len(self.grid)
+
+    @property
+    def n_clips(self) -> int:
+        return len(self._where)
+
+    def _at(self, k: int, j: int):
+        if not 0 <= k < len(self.grid):
+            raise IndexError(f"cell {k} out of range")
+        p, jj = self._where[j]
+        ps = self._passes[p]
+        return ps, k * ps.c + jj
+
+    def _q(self, tol) -> int:
+        try:
+            return self.tolerances.index(tol)
+        except ValueError:
+            raise KeyError(f"tolerance {tol} was not evaluated (tolerances {self.tolerances})") from None
+
+    def end_frame(self, j: int) -> int:
+        """Clip j's end as SceneManager.get_scene_list ends it: its last position + 1 (clip-local frames)."""
+        return self._end[j]
+
+    def cuts(self, k: int, j: int) -> list[int]:
+        """Cell k's predicted list on clip j, as `SweepResult.cuts` gives it: sorted unique cuts, then the clip's
+        end frame; empty when the cell found no cut."""
+        ps, t = self._at(k, j)
+        m = int(ps.host("n_pred")[t])
+        if m <= 0:
+            return []
+        o = int(ps.host("offsets")[t])
+        got = ps.cuts_buf.download((m - 1) * 8, offset=o * 8).view(np.int64).tolist()
+        return got + [self._end[j]]
+
+    def raw_count(self, k: int, j: int) -> int:
+        """How many cuts cell k's automaton emitted on clip j (before de-duplication)."""
+        ps, t = self._at(k, j)
+        o = ps.host("offsets")
+        return int(o[t + 1] - o[t])
+
+    def hard(self, k: int, j: int, tol: int) -> tuple[int, int, int]:
+        """(matched, false_positives, missed) of clip j's hard cuts at tolerance `tol`."""
+        ps, t = self._at(k, j)
+        h = ps.host("hard")[t, self._q(tol)]
+        return int(h[0]), int(h[1]), int(h[2])
+
+    def hard_offset(self, k: int, j: int, tol: int) -> tuple[float, int]:
+        """(sum of |prediction - ground truth|, match count) over clip j's hard-cut matches."""
+        ps, t = self._at(k, j)
+        h = ps.host("hard")[t, self._q(tol)]
+        return float(h[3]), int(h[4])
+
+    def fades(self, k: int, j: int) -> tuple[int, int, int]:
+        ps, t = self._at(k, j)
+        f = ps.host("fades")[t]
+        return int(f[0]), int(f[1]), int(f[2])
+
+    def totals(self) -> list[CellTotals]:
+        """Every cell's counts summed over this call's clips, in grid order."""
+        return _cell_totals(self.grid, self.tolerances, self._th, self._tf)
+
+
 class ParameterSweep:
     """Every cell of `grid` (a list of `detector_cls(**params)` keyword dicts, as the reference harness takes
     them) over each video `run` is given.  `detector_cls` is one of this package's detectors; each cell is
@@ -355,18 +470,104 @@ class ParameterSweep:
         return SweepResult(self.tolerances, self.slot_of, count_h, n_pred_h, hard_h, fades_h, cuts, cap, end_frame,
                            grid_ms)
 
+    # -- many clips per pass --
+    def run_clips(self, videos, ground_truths=None) -> ClipSweepResult:
+        """Every cell over every stream of `videos`: for each (cell, clip), what `run(videos[j], ground_truths[j])`
+        gives on a fresh ParameterSweep with this grid, tolerances and batch size; `totals` and `videos` afterwards
+        are what a loop of `run` leaves.  Streams are anything `detect_clips` reads (host or CUDA `ArrayVideoStream`s
+        of any layout and channel order, reference `VideoStream`s) and may differ in length, frame rate and frame
+        size; each is read from its current position, with SceneManager's default geometry, and its frame numbers
+        are clip-local.
+
+        The clips are scored as `detect_clips` scores them, pass by pass.  Each pass ends with the scans, ONE
+        psd_clip_cuts for every (cell, clip) automaton and ONE psd_clip_eval that scores every (cell, clip,
+        tolerance) against clip j's ground truth and sums the counts over the pass's clips on the device; only
+        those sums and the cut total come back to the host.
+
+        `ground_truths`: None (every count is against an empty truth and `totals` is not updated), or one
+        GroundTruth per video.  ValueError for a length mismatch or a clip without frames, RuntimeError for a
+        (cell, clip) with more than max_cuts_per_cell cuts; `totals` only changes when the call returns."""
+        from .clips import _Pass, clip_passes
+        videos = list(videos)
+        if ground_truths is None:
+            gts = [GroundTruth([])] * len(videos)
+        else:
+            gts = list(ground_truths)
+            if len(gts) != len(videos):
+                raise ValueError(f"{len(videos)} videos need as many ground truths, got {len(gts)}")
+            if not all(isinstance(g, GroundTruth) for g in gts):
+                raise ValueError("every ground truth must be a GroundTruth (GroundTruth([]) for a clip without cuts)")
+        lib = self._lib = self._lib or _capi.load()
+        n_cells, n_tol, dev = len(self.cells), len(self.tolerances), self.device
+        tols = (C.c_int32 * n_tol)(*self.tolerances)
+        th = np.zeros((n_cells, n_tol, 5), dtype=np.int64)
+        tf = np.zeros((n_cells, 3), dtype=np.int64)
+        passes, where, ends = [], [None] * len(videos), [0] * len(videos)
+        grid_ms = 0.0
+        device_pass = _Pass(self.cells, self.groups, dev)
+        scoring = clip_passes(videos, self.groups, SceneManager(device=dev, batch_size=self.batch_size),
+                              self.batch_size, dev)
+        try:
+            for engine, holders, done in scoring:
+                for index, _r, m in done:
+                    if not m:
+                        raise ValueError(f"clip {index} has no frames")
+                t0 = time.perf_counter()
+                pc = device_pass.cuts(engine, holders, [(r, m) for _, r, m in done])
+                indices = [index for index, _r, _m in done]
+                c = pc.n_clips
+                ggt = [gts[i] for i in indices]
+                gt_off = np.concatenate([[0], np.cumsum([len(g.hard_cuts) for g in ggt])]).astype(np.int64)
+                fade_off = np.concatenate([[0], np.cumsum([len(g.fades) for g in ggt])]).astype(np.int64)
+                n_gt, n_fades = int(gt_off[-1]), int(fade_off[-1])
+                gt_table = np.concatenate([gt_off, fade_off, [x for g in ggt for x in g.hard_cuts],
+                                           [x for g in ggt for f in g.fades for x in f]]).astype(np.int64)
+                gbuf = DeviceBuffer(gt_table.nbytes, dev)
+                gbuf.upload(gt_table)
+                m = n_cells * c
+                ws = DeviceBuffer(max(8, clip_eval_workspace_bytes(n_cells, c, n_tol, pc.total, n_gt, n_fades)), dev)
+                n_pred = DeviceBuffer(max(8, m * 4), dev)
+                hard = DeviceBuffer(m * n_tol * 40, dev)
+                fades = DeviceBuffer(m * 24, dev)
+                sums = DeviceBuffer(n_cells * (n_tol * 5 + 3) * 8 + 8, dev)  # totals_hard, totals_fades, over
+                try:
+                    gt_cuts = gbuf.ptr + 2 * (c + 1) * 8
+                    check(lib.psd_clip_eval(
+                        pc.cuts.ptr, pc.offsets.ptr, n_cells, c, pc.total, self.cap, pc.end_frames, gbuf.ptr, gt_cuts,
+                        n_gt, gbuf.ptr + (c + 1) * 8, gt_cuts + n_gt * 8, n_fades, tols, n_tol, ws.ptr, ws.nbytes,
+                        n_pred.ptr, hard.ptr, fades.ptr, sums.ptr, sums.ptr + n_cells * n_tol * 40,
+                        sums.ptr + n_cells * (n_tol * 5 + 3) * 8, engine.compute_stream), "psd_clip_eval")
+                    engine.sync()
+                    grid_ms += (time.perf_counter() - t0) * 1e3
+                    got = sums.download(sums.nbytes).view(np.int64)
+                finally:
+                    for b in (gbuf, ws, sums, pc.table):
+                        b.close()
+                over = int(got[-1])
+                if over >= 0:
+                    k, jj = divmod(over, c)
+                    o = pc.offsets.download(16, offset=over * 8).view(np.int64)
+                    raise RuntimeError(f"cell {k} ({self.grid[k]}) found {int(o[1] - o[0])} cuts in clip "
+                                       f"{indices[jj]}, more than max_cuts_per_cell={self.cap}")
+                th += got[:n_cells * n_tol * 5].reshape(n_cells, n_tol, 5)
+                tf += got[n_cells * n_tol * 5:-1].reshape(n_cells, 3)
+                for jj, (index, r) in enumerate(zip(indices, pc.clips)):
+                    where[index] = (len(passes), jj)
+                    ends[index] = r.end.frame_num + 1
+                passes.append(_ClipPass(pc, n_tol, n_pred, hard, fades))
+        finally:
+            scoring.close()
+            device_pass.close()
+        if ground_truths is not None:
+            self._totals_hard += th
+            self._totals_fades += tf
+            self.videos += len(videos)
+        return ClipSweepResult(self.grid, self.tolerances, passes, where, ends, th, tf, grid_ms)
+
     def totals(self) -> list[CellTotals]:
-        """Every cell's counts summed over the videos run with ground truth so far, in grid order."""
-        out = []
-        for k, params in enumerate(self.grid):
-            h, f = self._totals_hard[k], self._totals_fades[k]
-            out.append(CellTotals(
-                params=params,
-                hard={t: EventCounts(int(h[q, 0]), int(h[q, 1]), int(h[q, 2])) for q, t in enumerate(self.tolerances)},
-                hard_offset={t: (float(h[q, 3]), int(h[q, 4])) for q, t in enumerate(self.tolerances)},
-                fades=EventCounts(int(f[0]), int(f[1]), int(f[2]))))
-        return out
+        """Every cell's counts summed over the videos and clips run with ground truth so far, in grid order."""
+        return _cell_totals(self.grid, self.tolerances, self._totals_hard, self._totals_fades)
 
 
-__all__ = ["ParameterSweep", "SweepResult", "GroundTruth", "EventCounts", "CellTotals", "PixelGroup", "CellPlan",
-           "plan_cell", "pixel_group_of"]
+__all__ = ["ParameterSweep", "SweepResult", "ClipSweepResult", "GroundTruth", "EventCounts", "CellTotals",
+           "PixelGroup", "CellPlan", "plan_cell", "pixel_group_of"]
