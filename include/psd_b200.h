@@ -326,6 +326,26 @@ int psd_clip_eval(int64_t* cuts, const int64_t* cut_offsets, int32_t n_cells, in
                   const int32_t* tolerances, int32_t n_tol, void* workspace, size_t workspace_bytes,
                   int32_t* out_n_pred, int64_t* out_hard, int64_t* out_fades, int64_t* out_totals_hard,
                   int64_t* out_totals_fades, int64_t* out_over, void* stream);
+/* One column of a StatsManager CSV (stats_manager.py:save_to_csv) over a pass: frame i's value is values[i * stride]
+ * (a psd_scan_* output, stride 1, or one component of psd_scan_content's out_components, stride 4).  The first `head`
+ * and the last `tail` frames of every clip have no value there: the cell prints None. */
+typedef struct psd_stats_column {
+    const double* values; /* DEVICE */
+    int64_t stride;
+    int32_t head;
+    int32_t tail;
+} psd_stats_column;
+#define PSD_STATS_MAX_COLUMNS 64
+/* Every clip's StatsManager CSV rows, without the header, in one pass: for each frame of clip j that some column has
+ * a value for, `frame_num + 1,HH:MM:SS.nnn,` then every column's str(value) or None, comma-separated, and "\n"; frame_num
+ * = clip_first_frame[j] + the frame's index in the clip, the timecode FrameTimecode(frame_num, rate).get_timecode()
+ * with rate = clip_rate[j] (float(frame rate)).  columns is a HOST array in CSV order (validated, then copied on
+ * `stream`); everything else is DEVICE memory.  n = clip_offsets[n_clips] frames; row_offsets[n + 1] is workspace.
+ * out receives clip 0's rows, then clip 1's, ...; clip_bytes[n_clips + 1] their exclusive byte offsets and the total.
+ * When the total exceeds out_cap, clip_bytes is written and the text is not: grow out and call again. */
+int psd_clip_stats_csv(const psd_stats_column* columns, int32_t n_columns, const int64_t* clip_offsets,
+                       const int64_t* clip_first_frame, const double* clip_rate, int32_t n_clips, int64_t n,
+                       int64_t* row_offsets, char* out, int64_t out_cap, int64_t* clip_bytes, void* stream);
 
 /* host-convenience wrappers: engine-owned sums -> host arrays (numpy), implies sync */
 int psd_engine_scan_content_host(psd_engine* e, int64_t first, int64_t n, const double weights[4],
@@ -358,6 +378,9 @@ int psd_gather_bgr(int device, const void* base, const psd_frame_layout* layout,
 /* device BGR (n pixels, a multiple of 16) -> H,S,V and Y planes with the device functions the fused pass uses */
 int psd_test_hsv(int device, const uint8_t* bgr_host, int64_t n_pixels, uint8_t* h_out, uint8_t* s_out,
                  uint8_t* v_out, uint8_t* y_out);
+/* str() of n host doubles with the device formatter psd_clip_stats_csv prints values with: text_out[n][32], each
+ * value's text followed by NUL bytes */
+int psd_test_format_f64(int device, const double* values_host, int64_t n, char* text_out);
 /* HashDetector's stages through the engine's hash kernels: n_frames packed BGR24 frames (width x height, frame_stride
  * bytes apart) in DEVICE memory of `device`, and n_geo (1 to 16) geometries {size, lowpass} in geometries[n_geo][2].
  * Builds each geometry's plan for n_frames frames and runs the hash pass once.  Host outputs, geometry g's block

@@ -89,6 +89,22 @@ class PsdSweepCell(C.Structure):
 
 assert C.sizeof(PsdSweepCell) == 64
 
+STATS_MAX_COLUMNS = 64
+F64_TEXT = 32  # bytes per value of psd_test_format_f64
+
+
+class PsdStatsColumn(C.Structure):
+    """psd_stats_column: one column of psd_clip_stats_csv (24 bytes)."""
+    _fields_ = [
+        ("values", C.c_void_p),
+        ("stride", C.c_int64),
+        ("head", C.c_int32),
+        ("tail", C.c_int32),
+    ]
+
+
+assert C.sizeof(PsdStatsColumn) == 24
+
 
 # numpy view of psd_frame_sums (64 bytes)
 SUMS_DTYPE = np.dtype([
@@ -166,6 +182,7 @@ SIGNATURES = {
     "psd_clip_cuts": (C.c_int, [_vp, _i32, _vp, _vp, _i32, _vp, _vp, _i64, _vp, _vp]),
     "psd_clip_eval": (C.c_int, [_vp, _vp, _i32, _i32, _i64, _i64, _vp, _vp, _vp, _i32, _vp, _vp, _i32, _vp, _i32, _vp,
                                 C.c_size_t, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "psd_clip_stats_csv": (C.c_int, [_vp, _i32, _vp, _vp, _vp, _i32, _i64, _vp, _vp, _i64, _vp, _vp]),
     "psd_engine_scan_content_host": (C.c_int, [_vp, _i64, _i64, _dp, _dbl, _vp, _vp]),
     "psd_engine_scan_adaptive_host": (C.c_int, [_vp, _vp, _i64, _i32, _dbl, _vp]),
     "psd_engine_scan_average_host": (C.c_int, [_vp, _i64, _i64, _vp]),
@@ -176,6 +193,7 @@ SIGNATURES = {
     "psd_synth_frames": (C.c_int, [C.c_int, _vp, _vp, _i64, _i32, _i32, _i64, _vp]),
     "psd_gather_bgr": (C.c_int, [C.c_int, _vp, C.POINTER(PsdFrameLayout), _i64, _i32, _i32, _vp, _i64, _vp]),
     "psd_test_hsv": (C.c_int, [C.c_int, _vp, _i64, _vp, _vp, _vp, _vp]),
+    "psd_test_format_f64": (C.c_int, [C.c_int, _vp, _i64, _vp]),
     "psd_test_hash_stages": (C.c_int, [C.c_int, _vp, _i64, _i32, _i32, _i64, _vp, _i32, _vp, _vp, _vp, _vp]),
 }
 

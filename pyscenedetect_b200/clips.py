@@ -24,10 +24,17 @@ per-frame result memory does not grow with the number of clips (a single longer 
 Results are those of a fresh `SceneManager(batch_size=...)` with the same `auto_downscale` / `downscale` and fresh
 detectors, running `detect_scenes` on each clip: cut list, scene lists and frame count.  Frame numbers are
 clip-local, frame-number timecodes at the clip's constant frame rate (as `DeviceCuts` gives them).
+
+With `stats=True` each clip also gets the text a `StatsManager` attached to that SceneManager saves
+(`save_to_csv`): the metric arrays the cuts are made from are already on the device, so psd_clip_stats_csv prints
+every clip's rows there (three launches a pass) and one download per pass brings them back, instead of a
+`set_metrics` per frame and a `str()` per value on the host.
 """
 
 from __future__ import annotations
 
+import csv
+import io
 from dataclasses import dataclass, field
 from fractions import Fraction
 
@@ -36,6 +43,7 @@ import numpy as np
 from . import _capi, _dlpack
 from ._capi import check
 from .compat import FrameTimecode
+from .detectors import ContentDetector, ThresholdDetector
 from .detectors._base import EngineDetector, pixel_group_of
 from .device_cuts import scan_metric
 from .engine import DeviceBuffer
@@ -44,6 +52,7 @@ from .sweep import _KIND, plan_cell
 
 MAX_PASS_FRAMES = 1 << 16     # frames an engine holds before its pass is finished at the next clip boundary
 FIRST_CUTS_PER_FRAME = 0.25   # first cut buffer of a pass, in cuts per frame held; grown once if the cuts need more
+FIRST_STATS_BYTES = (32, 24)  # first CSV text buffer, in bytes per frame held: a + b * columns; grown once if short
 
 
 @dataclass
@@ -55,6 +64,7 @@ class ClipResult:
     cut_frames: list = field(default_factory=list)  # sorted unique cut frame numbers
     start: FrameTimecode | None = None       # position of the first frame scored (None: the clip had no frames)
     end: FrameTimecode | None = None         # the stream's position after the last frame
+    stats_csv: bytes | None = None           # detect_clips(stats=True): what StatsManager.save_to_csv writes
 
     def cut_list(self) -> list:
         return [FrameTimecode(c, self.fps) for c in self.cut_frames]
@@ -197,17 +207,50 @@ class _Pass:
                 if key is not None and key not in self.keys:
                     self.keys.append(key)
         self._bufs = {}
+        self.columns = None         # stats: [(CSV key, metric key, component or None, head, tail)] in CSV order
+        self.components_key = None  # stats: the content_val key whose scan also writes the four components
+        self.header = b""
 
     @classmethod
-    def of_detectors(cls, detectors, device: int) -> _Pass:
+    def of_detectors(cls, detectors, device: int, stats: bool = False) -> _Pass:
         groups, gi, cells = [], {}, []
         for d in detectors:
-            g = pixel_group_of(d)
+            g = pixel_group_of(d, stats)
             if g not in gi:
                 gi[g] = len(groups)
                 groups.append(g)
             cells.append(plan_cell(d, gi[g]))
-        return cls(cells, groups, device)
+        p = cls(cells, groups, device)
+        if stats:
+            p.plan_stats(detectors)
+        return p
+
+    def plan_stats(self, detectors) -> None:
+        """One CSV column per metric key of the detectors, read from the metric array of the last detector that
+        writes the key (SceneManager runs the detectors in order on every batch, so at every frame the last writer's
+        value stands), with the frames of a clip that have no value: head / tail as the detectors skip them."""
+        writers = {}
+        for d, cell in zip(detectors, self.cells):
+            if cell.kind in ("content", "adaptive"):  # content_detector.py:161-164,183-186: frames 1 .. n-1
+                val = cell.metric if cell.kind == "content" else cell.metric2
+                writers[ContentDetector.FRAME_SCORE_KEY] = (val, None, 1, 0)
+                for i, name in enumerate(ContentDetector.Components._fields):
+                    writers[name] = (val, i, 1, 0)
+                if cell.kind == "adaptive":       # adaptive_detector.py:116-128: frames W .. n-1-W
+                    writers[d.get_metrics()[-1]] = (cell.metric, None, cell.window, cell.window)
+            elif cell.kind == "threshold":        # threshold_detector.py:127-129: every frame
+                writers[ThresholdDetector.THRESHOLD_VALUE_KEY] = (cell.metric, None, 0, 0)
+            else:                                 # histogram, hash: every frame with a predecessor
+                writers[d.get_metrics()[0]] = (cell.metric, None, 1, 0)
+        keys = sorted(set().union(*(d.get_metrics() for d in detectors)))
+        assert set(keys) == set(writers), (keys, sorted(writers))
+        if len(keys) > _capi.STATS_MAX_COLUMNS:
+            raise ValueError(f"{len(keys)} metric columns: psd_clip_stats_csv prints at most {_capi.STATS_MAX_COLUMNS}")
+        self.columns = [(k, *writers[k]) for k in keys]
+        self.components_key = next((c[1] for c in self.columns if c[2] is not None), None)
+        text = io.StringIO()
+        csv.writer(text, lineterminator="\n").writerow(["Frame Number", "Timecode", *keys])
+        self.header = text.getvalue().encode()
 
     def _buf(self, name, nbytes: int) -> DeviceBuffer:
         b = self._bufs.get(name)
@@ -243,9 +286,11 @@ class _Pass:
         tbuf.upload(table)
         offsets, first, min_frames = tbuf.ptr, tbuf.ptr + (c + 1) * 8, tbuf.ptr + (3 * c + 1) * 8
         arrays = {key: self._buf(key, n * 8) for key in self.keys}
+        comps = self._buf("components", n * 32).ptr if self.components_key is not None else None
         for key in self.keys:
             val = arrays[("content_val",) + key[1:3]].ptr if key[0] == "adaptive_ratio" else None
-            scan_metric(lib, holders[key[1]], (key[0],) + key[2:], arrays[key].ptr, val, clips=(offsets, c))
+            scan_metric(lib, holders[key[1]], (key[0],) + key[2:], arrays[key].ptr, val, clips=(offsets, c),
+                        components=comps if key == self.components_key else None)
         cells = (_capi.PsdSweepCell * k)()
         for i, cell in enumerate(self.cells):
             cells[i] = _capi.PsdSweepCell(
@@ -272,9 +317,47 @@ class _Pass:
             cap = cuts.nbytes // 8
         return PassCuts(scored, k, tbuf, obuf, cuts, total)
 
+    def stats_csv(self, engine, pc: PassCuts) -> list:
+        """The CSV of every clip of `pc` (header and rows), printed on the device by one psd_clip_stats_csv from the
+        metric arrays `cuts` left, and brought back with one download."""
+        n, c = engine.frame_count, pc.n_clips
+        cols = (_capi.PsdStatsColumn * len(self.columns))()
+        for i, (_, key, comp, head, tail) in enumerate(self.columns):
+            ptr, stride = (self._bufs[key].ptr, 1) if comp is None else (self._bufs["components"].ptr + 8 * comp, 4)
+            cols[i] = _capi.PsdStatsColumn(values=ptr, stride=stride, head=head, tail=tail)
+        rates = np.array([float(r.start.frame_rate) for r in pc.clips], dtype=np.float64)
+        rbuf = DeviceBuffer(rates.nbytes, self.device)
+        cbuf = DeviceBuffer((c + 1) * 8, self.device)
+        try:
+            rbuf.upload(rates)
+            rows = self._buf("stats_rows", (n + 1) * 8)
+            a, b = FIRST_STATS_BYTES
+            text = self._buf("stats_text", n * (a + b * len(cols)))
+            for attempt in range(2):
+                cap = text.nbytes
+                check(self._lib.psd_clip_stats_csv(cols, len(cols), pc.table.ptr, pc.table.ptr + (c + 1) * 8, rbuf.ptr,
+                                                   c, n, rows.ptr, text.ptr, cap, cbuf.ptr, engine.compute_stream),
+                      "psd_clip_stats_csv")
+                engine.sync()
+                offs = cbuf.download((c + 1) * 8).view(np.int64).tolist()
+                if offs[-1] <= cap:
+                    break
+                if attempt:
+                    raise RuntimeError(f"psd_clip_stats_csv needs {offs[-1]} bytes after growing its buffer to {cap}")
+                text = self._buf("stats_text", offs[-1])
+            data = text.download(offs[-1]).tobytes() if offs[-1] else b""
+        finally:
+            rbuf.close()
+            cbuf.close()
+        return [self.header + data[offs[j]:offs[j + 1]] for j in range(c)]
+
     def finish(self, engine, holders, clips: list) -> None:
         """Every clip of `clips` ((ClipResult, frames scored) of the frames `engine` holds, in order) gets its cut
-        frames: the union of every cell's cuts, as SceneManager.get_cut_list gives them."""
+        frames: the union of every cell's cuts, as SceneManager.get_cut_list gives them; and with a stats plan its
+        CSV (the header alone for a clip without frames)."""
+        for r, _ in clips:
+            if self.columns is not None:
+                r.stats_csv = self.header
         pc = self.cuts(engine, holders, clips)
         if pc is None:
             return
@@ -282,10 +365,13 @@ class _Pass:
             k, c = pc.n_cells, pc.n_clips
             offs = pc.offsets.download((k * c + 1) * 8).view(np.int64).tolist()
             got = pc.cuts.download(pc.total * 8).view(np.int64).tolist() if pc.total else []
+            texts = self.stats_csv(engine, pc) if self.columns is not None else None
         finally:
             pc.close()
         for j, r in enumerate(pc.clips):  # (cell i, clip j) is list i * c + j: SceneManager.get_cut_list per clip
             r.cut_frames = sorted({f for i in range(k) for f in got[offs[i * c + j]:offs[i * c + j + 1]]})
+            if texts is not None:
+                r.stats_csv = texts[j]
 
 
 def _group_key(video) -> tuple:
@@ -296,15 +382,22 @@ def _group_key(video) -> tuple:
 
 
 def detect_clips(videos, detectors, auto_downscale: bool = True, downscale: int = 1, device: int = 0,
-                 batch_size: int = 64) -> list[ClipResult]:
+                 batch_size: int = 64, stats: bool = False) -> list[ClipResult]:
     """Detect scenes in every stream of `videos` with every detector of `detectors`: for each clip, in input order,
     what a fresh `SceneManager(device=device, batch_size=batch_size)` with these `auto_downscale` / `downscale` and
     fresh copies of the detectors give from `detect_scenes(video)`.  Streams are anything `detect_scenes` reads
     (`ArrayVideoStream` over numpy or CUDA arrays of any layout and channel order, a reference `VideoStream`) and may
     differ in length, frame rate and frame size; a stream is read from its current position to its end.
 
+    `stats=True`: every result also has `stats_csv`, the bytes `StatsManager.save_to_csv` writes (line terminator
+    "\\n") after that SceneManager, built with a fresh `StatsManager()`, ran `detect_scenes(video)`: the header
+    `Frame Number,Timecode,` and the sorted metric keys of the detectors, then one row per frame that has a metric.
+    As an attached StatsManager does, it turns on ContentDetector's edge component; the cut lists are those of
+    `stats=False`.
+
     The detectors are configuration only: they are not attached to an engine or otherwise changed.  ValueError for
-    an empty detector list or a detector with a `stats_manager` (this path produces no per-frame metric rows)."""
+    an empty detector list or a detector with a `stats_manager` (the detectors take no StatsManager here: ask for
+    `stats` instead)."""
     detectors = list(detectors)
     if not detectors:
         raise ValueError("No detectors added")
@@ -319,7 +412,7 @@ def detect_clips(videos, detectors, auto_downscale: bool = True, downscale: int 
     geometry._auto_downscale, geometry._downscale = bool(auto_downscale), int(downscale)
     videos = list(videos)
     results: list = [None] * len(videos)
-    device_pass = _Pass.of_detectors(detectors, device)
+    device_pass = _Pass.of_detectors(detectors, device, stats=stats)
     passes = clip_passes(videos, device_pass.groups, geometry, batch_size, device)
     try:
         for engine, holders, done in passes:

@@ -10,10 +10,15 @@
 //   psd_clip_eval    the counterpart of psd_sweep_eval for psd_clip_cuts' compact output: every (cell, clip) list
 //                    turned in place into its predicted list, every (cell, clip, tolerance) scored against clip j's
 //                    ground truth with score_predictions (sweep_eval.cuh), and the counts summed over the clips
-// Each is one launch (three for psd_clip_cuts and psd_clip_eval) per pass whatever the number of cells and clips.
+//   psd_clip_stats_csv  every clip's StatsManager CSV rows (stats_csv.cuh formats them): one thread per frame counts
+//                    its row's bytes, an exclusive scan gives the row offsets, and the writing pass prints each row in
+//                    place, so one download carries every clip's text
+// Each is one launch (three for psd_clip_cuts, psd_clip_eval and psd_clip_stats_csv) per pass whatever the number of
+// cells and clips.
 #include <math_constants.h>
 
 #include "cut_automata.cuh"
+#include "stats_csv.cuh"
 #include "sweep_eval.cuh"
 
 namespace psd {
@@ -183,6 +188,86 @@ __global__ void __launch_bounds__(256) clip_totals_kernel(const int64_t* __restr
     }
 }
 
+// The clip that pass frame i belongs to: the last j with offsets[j] <= i (empty clips share their offset with the next
+// clip, so this is the clip that holds i).
+__device__ __forceinline__ int32_t clip_of(const int64_t* __restrict__ offsets, int32_t n_clips, int64_t i) {
+    int32_t lo = 0, hi = n_clips - 1;
+    while (lo < hi) {
+        const int32_t mid = (lo + hi + 1) >> 1;
+        if (offsets[mid] <= i) lo = mid;
+        else hi = mid - 1;
+    }
+    return lo;
+}
+
+// A row's cells.  Counting pass (WRITE = false): row_offsets[i] = the bytes of frame i's row (0: no row).  Writing
+// pass: the row at out + row_offsets[i], after psd_clip_scan_kernel made them offsets; nothing when the total exceeds
+// cap.  The writing pass's threads n .. n + n_clips write the clip byte offsets.
+template <bool WRITE>
+__global__ void __launch_bounds__(128) stats_rows_kernel(const psd_stats_column* __restrict__ cols, int32_t n_cols,
+                                                         const int64_t* __restrict__ offsets,
+                                                         const int64_t* __restrict__ first_frame,
+                                                         const double* __restrict__ rate, int32_t n_clips, int64_t n,
+                                                         int64_t* __restrict__ row_offsets, char* __restrict__ out,
+                                                         int64_t cap, int64_t* __restrict__ clip_bytes) {
+    const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+    if (WRITE && i >= n) {
+        if (i <= n + n_clips) clip_bytes[i - n] = row_offsets[min(max(offsets[i - n], (int64_t)0), n)];
+        return;
+    }
+    if (i >= n) return;
+    const int32_t j = clip_of(offsets, n_clips, i);
+    const int64_t b = offsets[j], local = i - b, len = offsets[j + 1] - b;
+    bool row = false;
+    for (int32_t c = 0; c < n_cols; ++c) row |= local >= cols[c].head && local < len - cols[c].tail;
+    if (WRITE && (!row || row_offsets[n] > cap)) return;
+    if (!row) {
+        row_offsets[i] = 0;
+        return;
+    }
+    const int64_t frame = first_frame[j] + local;
+    const Timecode tc = timecode_of(frame, rate[j]);
+    char* p = WRITE ? out + row_offsets[i] : nullptr;
+    int64_t bytes = uint_len((uint64_t)frame + 1) + 1 + timecode_len(tc);
+    if (WRITE) {
+        p = uint_write((uint64_t)frame + 1, p);
+        *p++ = ',';
+        p = timecode_write(tc, p);
+    }
+    for (int32_t c = 0; c < n_cols; ++c) {
+        const psd_stats_column col = cols[c];
+        const bool has = local >= col.head && local < len - col.tail;
+        if (has) {
+            const Decimal d = f64_decimal(col.values[i * col.stride]);
+            bytes += 1 + f64_len(d);
+            if (WRITE) {
+                *p++ = ',';
+                p = f64_write(d, p);
+            }
+        } else {
+            bytes += 5;
+            if (WRITE) {
+                *p++ = ',';
+                put3(p, 'N', 'o', 'n');
+                p[3] = 'e';
+                p += 4;
+            }
+        }
+    }
+    if (WRITE) *p = '\n';
+    else row_offsets[i] = bytes + 1;
+}
+
+__global__ void __launch_bounds__(128) format_f64_kernel(const double* __restrict__ v, int64_t n, char* __restrict__ out) {
+    const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    char* p = out + i * 32;
+    const Decimal d = f64_decimal(v[i]);
+    const int len = f64_len(d);
+    f64_write(d, p);
+    for (int k = len; k < 32; ++k) p[k] = 0;
+}
+
 }  // namespace psd
 
 using namespace psd;
@@ -288,5 +373,62 @@ extern "C" int psd_clip_eval(int64_t* cuts, const int64_t* cut_offsets, int32_t 
                                                                      out_totals_hard, out_totals_fades);
     PSD_CHECK_LAUNCH();
     count_launch(3);
+    return PSD_OK;
+}
+
+extern "C" int psd_clip_stats_csv(const psd_stats_column* columns, int32_t n_columns, const int64_t* clip_offsets,
+                                  const int64_t* clip_first_frame, const double* clip_rate, int32_t n_clips, int64_t n,
+                                  int64_t* row_offsets, char* out, int64_t out_cap, int64_t* clip_bytes,
+                                  void* stream) {
+    PSD_REQUIRE(clip_offsets && clip_bytes, "psd_clip_stats_csv: no clip table / clip_bytes");
+    PSD_REQUIRE(n >= 0 && n_clips >= 0 && out_cap >= 0, "psd_clip_stats_csv: bad args");
+    PSD_REQUIRE(columns && n_columns >= 1 && n_columns <= PSD_STATS_MAX_COLUMNS,
+                "psd_clip_stats_csv: 1 to %d columns", PSD_STATS_MAX_COLUMNS);
+    for (int32_t c = 0; c < n_columns; ++c)
+        PSD_REQUIRE(columns[c].values && columns[c].stride >= 1 && columns[c].head >= 0 && columns[c].tail >= 0,
+                    "psd_clip_stats_csv: column %d: no values, or a stride < 1, or a negative head / tail", c);
+    cudaStream_t s = (cudaStream_t)stream;
+    if (n == 0 || n_clips == 0) {
+        PSD_CUDA(cudaMemsetAsync(clip_bytes, 0, sizeof(int64_t) * ((size_t)n_clips + 1), s));
+        return PSD_OK;
+    }
+    PSD_REQUIRE(clip_first_frame && clip_rate && row_offsets, "psd_clip_stats_csv: no first frames / rates / row_offsets");
+    PSD_REQUIRE(out || out_cap == 0, "psd_clip_stats_csv: no output buffer");
+    psd_stats_column* d_cols = nullptr;
+    const size_t bytes = sizeof(psd_stats_column) * (size_t)n_columns;
+    PSD_CUDA(cudaMallocAsync((void**)&d_cols, bytes, s));
+    PSD_CUDA(cudaMemcpyAsync(d_cols, columns, bytes, cudaMemcpyHostToDevice, s));  // pageable: staged before return
+    stats_rows_kernel<false><<<(unsigned)((n + 127) / 128), 128, 0, s>>>(
+        d_cols, n_columns, clip_offsets, clip_first_frame, clip_rate, n_clips, n, row_offsets, out, out_cap, clip_bytes);
+    PSD_CHECK_LAUNCH();
+    psd_clip_scan_kernel<<<1, 1024, 0, s>>>(row_offsets, n);
+    PSD_CHECK_LAUNCH();
+    const int64_t threads = n + n_clips + 1;
+    stats_rows_kernel<true><<<(unsigned)((threads + 127) / 128), 128, 0, s>>>(
+        d_cols, n_columns, clip_offsets, clip_first_frame, clip_rate, n_clips, n, row_offsets, out, out_cap, clip_bytes);
+    PSD_CHECK_LAUNCH();
+    count_launch(3);
+    PSD_CUDA(cudaFreeAsync(d_cols, s));
+    return PSD_OK;
+}
+
+extern "C" int psd_test_format_f64(int device, const double* values_host, int64_t n, char* text_out) {
+    PSD_REQUIRE(n >= 0 && (n == 0 || (values_host && text_out)), "psd_test_format_f64: bad args");
+    if (n == 0) return PSD_OK;
+    PSD_CUDA(cudaSetDevice(device));
+    double* d_v = nullptr;
+    char* d_text = nullptr;
+    cudaError_t e = cudaMalloc((void**)&d_v, sizeof(double) * (size_t)n);
+    if (e == cudaSuccess) e = cudaMalloc((void**)&d_text, 32 * (size_t)n);
+    if (e == cudaSuccess) e = cudaMemcpy(d_v, values_host, sizeof(double) * (size_t)n, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) {
+        format_f64_kernel<<<(unsigned)((n + 127) / 128), 128>>>(d_v, n, d_text);
+        e = cudaGetLastError();
+        count_launch();
+    }
+    if (e == cudaSuccess) e = cudaMemcpy(text_out, d_text, 32 * (size_t)n, cudaMemcpyDeviceToHost);
+    cudaFree(d_v);
+    cudaFree(d_text);
+    PSD_CUDA(e);
     return PSD_OK;
 }

@@ -28,10 +28,11 @@ class PixelGroup:
                       max_batch=max_batch, edge_kernel_size=self.edge_kernel_size, **dict(self.engine_kwargs))
 
 
-def pixel_group_of(detector) -> PixelGroup:
+def pixel_group_of(detector, stats: bool = False) -> PixelGroup:
     """The features a detector needs, its dilation kernel size argument when it uses the edge component
-    (content_detector.py:135-138; 0 otherwise) and its extra Engine arguments (the hash geometry)."""
-    feats = detector.required_features()
+    (content_detector.py:135-138; 0 otherwise) and its extra Engine arguments (the hash geometry).  `stats`: as if a
+    StatsManager were attached (the detector itself is not changed)."""
+    feats = detector.required_features(stats)
     return PixelGroup(feats, detector.edge_kernel_size_arg() if feats & F_EDGES else 0,
                       tuple(sorted(detector.engine_kwargs().items())))
 
@@ -66,7 +67,8 @@ class EngineDetector(SceneDetector):
         self._base_index = 0  # engine frame index of this detector's first frame
 
     # -- configuration hooks used by SceneManager's batched fast path --
-    def required_features(self) -> int:
+    def required_features(self, stats: bool = False) -> int:
+        """PSD_F_* bits of the fused pass; `stats`: also what the per-frame metrics of a StatsManager need."""
         return self.FEATURES
 
     def edge_kernel_size_arg(self) -> int:

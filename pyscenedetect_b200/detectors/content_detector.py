@@ -56,9 +56,9 @@ class ContentDetector(EngineDetector):
     def get_metrics(self):
         return ContentDetector.METRIC_KEYS
 
-    def required_features(self) -> int:
+    def required_features(self, stats: bool = False) -> int:
         # content_detector.py:158: edges are computed when weighted OR a StatsManager is attached
-        calculate_edges = (self._weights.delta_edges > 0.0) or self.stats_manager is not None
+        calculate_edges = (self._weights.delta_edges > 0.0) or self.stats_manager is not None or stats
         return F_HSV | (F_EDGES if calculate_edges else 0)
 
     def edge_kernel_size_arg(self) -> int:

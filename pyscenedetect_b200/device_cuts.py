@@ -58,7 +58,7 @@ def min_len_frames(length, fps) -> int:
 
 
 def scan_metric(lib, holder, key: tuple, out: int, content_val: int | None = None,
-                clips: tuple[int, int] | None = None) -> None:
+                clips: tuple[int, int] | None = None, components: int | None = None) -> None:
     """Launch the psd_scan_* that fills one metric array `out` (float64 per frame) from every frame a result holder
     (an Engine, a `SlotView` of one or `sharding.GatheredResults`) holds, on the holder's stream.  `key` is a
     `ParameterSweep` metric key without its group index: ("content_val", weights), ("adaptive_ratio", weights,
@@ -68,8 +68,11 @@ def scan_metric(lib, holder, key: tuple, out: int, content_val: int | None = Non
     `clips` = (device clip table, clip count) when the holder's frames are several clips scored back to back
     (psd_clip_fill): the scan is followed by the fix-up that gives every clip's first (and, for the adaptive ratio,
     last) entries the values a one-clip engine's scan has there, so each clip's slice equals that engine's array
-    byte for byte.  An adaptive ratio must read a `content_val` array that was fixed up the same way."""
-    _scan_metric(lib, holder, key, out, content_val)
+    byte for byte.  An adaptive ratio must read a `content_val` array that was fixed up the same way.
+
+    `components`: for content_val, a float64[n][4] device array that also receives psd_scan_content's components
+    (content_detector.py:166-176); the clip fix-up leaves them as scanned."""
+    _scan_metric(lib, holder, key, out, content_val, components)
     if clips is None or key[0] == "average_rgb":  # average_rgb is per frame: nothing crosses a clip edge
         return
     table, n_clips = clips
@@ -88,7 +91,7 @@ def scan_metric(lib, holder, key: tuple, out: int, content_val: int | None = Non
           "psd_clip_fill")
 
 
-def _scan_metric(lib, holder, key: tuple, out: int, content_val: int | None) -> None:
+def _scan_metric(lib, holder, key: tuple, out: int, content_val: int | None, components: int | None = None) -> None:
     n, st = holder.frame_count, holder.compute_stream
     kind = key[0]
     if kind == "content_val":
@@ -96,8 +99,8 @@ def _scan_metric(lib, holder, key: tuple, out: int, content_val: int | None) -> 
         w = (C.c_double * 4)(*[float(x) for x in key[1]])
         wsum = float(sum(abs(x) for x in key[1]))  # same expression as content_detector.py:180
         # NULL edge SADs: the sums' own sad_edges (edge slot 0)
-        check(lib.psd_scan_content_edges(sums, holder.device_edge_sads(), n, holder.n_pixels, w, wsum, None, out, st),
-              "psd_scan_content_edges")
+        check(lib.psd_scan_content_edges(sums, holder.device_edge_sads(), n, holder.n_pixels, w, wsum, components, out,
+                                         st), "psd_scan_content_edges")
     elif kind == "adaptive_ratio":
         check(lib.psd_scan_adaptive(content_val, n, int(key[2]), float(key[3]), out, st), "psd_scan_adaptive")
     elif kind == "average_rgb":
