@@ -306,6 +306,20 @@ int psd_clip_fill(double* values, int64_t n, const int64_t* clip_offsets, int32_
 int psd_clip_cuts(const psd_sweep_cell* cells, int32_t n_cells, const int64_t* clip_offsets,
                   const int64_t* clip_first_frame, int32_t n_clips, const int64_t* min_frames, int64_t* cuts,
                   int64_t cuts_cap, int64_t* cut_offsets, void* stream);
+/* psd_clip_cuts for clips read with SceneManager.detect_scenes(frame_skip = frame_step - 1): the per-frame loop
+ * processes every frame_step-th frame and reads the frames between them without processing them
+ * (scene_manager.py:682-685), so element i of clip j's slice is frame clip_first_frame[j] + i * frame_step, and the
+ * automata (detector.py:160-224, adaptive_detector.py:134-143, histogram_detector.py:87-112,
+ * hash_detector.py:79-109, threshold_detector.py:113-168) compare those true frame numbers with min_frames, which
+ * stays in frames.  ThresholdDetector's post_process (threshold_detector.py:170-191) gets the stream's position after
+ * the loop (scene_manager.py:618-621), which is past the last processed frame when skipped frames were read behind
+ * it: clip_end_frame[j] - 1, clip_end_frame being the DEVICE int64[n_clips] end frames psd_clip_eval takes (that
+ * position + 1), or NULL for the last processed frame.  frame_step >= 1; frame_step 1 and a NULL clip_end_frame give
+ * psd_clip_cuts' results bit for bit.  Same kernels and launches as psd_clip_cuts. */
+int psd_clip_cuts_step(const psd_sweep_cell* cells, int32_t n_cells, const int64_t* clip_offsets,
+                       const int64_t* clip_first_frame, int32_t n_clips, const int64_t* min_frames, int64_t* cuts,
+                       int64_t cuts_cap, int64_t* cut_offsets, int64_t frame_step, const int64_t* clip_end_frame,
+                       void* stream);
 /* benchmark/evaluator.py:227-331 (score_video) for every (cell, clip, tolerance) on psd_clip_cuts' output, and the
  * counts summed over the clips (evaluator.py:167-186).  cuts / cut_offsets are psd_clip_cuts' arrays and cuts_total
  * its total cut_offsets[n_cells * n_clips]; each (cell, clip) list is first turned, in place, into the predicted list

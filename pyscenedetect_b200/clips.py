@@ -21,9 +21,12 @@ stream, as SceneManager reads them: at least one submission per clip.
 A pass is finished, and the engine reset, once it holds `MAX_PASS_FRAMES` frames, at the next clip boundary; so the
 per-frame result memory does not grow with the number of clips (a single longer clip is held whole).
 
-Results are those of a fresh `SceneManager(batch_size=...)` with the same `auto_downscale` / `downscale` and fresh
-detectors, running `detect_scenes` on each clip: cut list, scene lists and frame count.  Frame numbers are
-clip-local, frame-number timecodes at the clip's constant frame rate (as `DeviceCuts` gives them).
+Results are those of a fresh `SceneManager(batch_size=...)` with the same `auto_downscale` / `downscale` / `crop`
+and fresh detectors, running `detect_scenes(video, duration=, end_time=, frame_skip=)` on each clip: cut list, scene
+lists and frame count.  Frame numbers are clip-local, frame-number timecodes at the clip's constant frame rate (as
+`DeviceCuts` gives them).  Each clip is read through its own `StreamWindow`, the one detect_scenes reads a stream
+through; with a frame skip, element i of a clip's metric slice is frame first + i * (frame_skip + 1), which
+psd_clip_cuts_step's automata walk.
 
 With `stats=True` each clip also gets the text a `StatsManager` attached to that SceneManager saves
 (`save_to_csv`): the metric arrays the cuts are made from are already on the device, so psd_clip_stats_csv prints
@@ -47,7 +50,8 @@ from .detectors import ContentDetector, ThresholdDetector
 from .detectors._base import EngineDetector, pixel_group_of
 from .device_cuts import scan_metric
 from .engine import DeviceBuffer
-from .scene_manager import FrameBatches, SceneManager, get_scenes_from_cuts, shared_engine
+from .scene_manager import (FrameBatches, SceneManager, StreamWindow, base_timecode_of, check_window,
+                            get_scenes_from_cuts, shared_engine, window_end_frame)
 from .sweep import _KIND, plan_cell
 
 MAX_PASS_FRAMES = 1 << 16     # frames an engine holds before its pass is finished at the next clip boundary
@@ -79,28 +83,28 @@ class ClipResult:
 
 
 class _ClipChain:
-    """A group's streams read one after the other as one stream, for `FrameBatches`: `read()` moves on to the next
-    clip when one ends, and records each clip's positions and frame count.  At a clip boundary, once the pass holds
-    `bound` frames, it reports an end (`paused`) until `resume()`."""
+    """A group's streams read one after the other as one stream, for `FrameBatches`: `read()` gives the next frame to
+    process of the current clip's `StreamWindow` (with `frame_skip` and the clip's own end frame of `duration` /
+    `end_time`, as detect_scenes reads one stream) and moves on to the next clip when that window ends, recording each
+    clip's positions and frame count.  At a clip boundary, once the pass holds `bound` frames, it reports an end
+    (`paused`) until `resume()`."""
 
-    def __init__(self, clips, bound: int, on_cuda: bool):
+    def __init__(self, clips, bound: int, on_cuda: bool, frame_skip: int = 0, duration=None, end_time=None):
         self._clips = clips       # [(input index, stream)]
         self._k = -1
         self._on_cuda = on_cuda
+        self._frame_skip, self._duration, self._end_time = frame_skip, duration, end_time
         self.bound = bound
         self.paused = False
-        self.held = 0             # frames read in this pass
+        self.held = 0             # frames processed in this pass
         self.done = []            # (input index, ClipResult, frames scored) of every clip finished in this pass
-        self._result = None
+        self._result = self._window = self._pos = None
         self._start_num = self._scored = 0
         self._next()
 
     frame_number = property(lambda self: self.held)   # FrameBatches only reads positions relative to its start
     frame_rate = property(lambda self: self._result.fps if self._result else Fraction(30))
-
-    @property
-    def position(self):
-        return self._clips[self._k][1].position if self._k < len(self._clips) else None
+    position = property(lambda self: self._pos)       # of the last frame processed
 
     def _next(self):
         self._k += 1
@@ -109,6 +113,8 @@ class _ClipChain:
             self._start_num = video.frame_number
             self._result = ClipResult(fps=video.frame_rate)
             self._scored = 0
+            end = window_end_frame(base_timecode_of(video), self._start_num, self._duration, self._end_time)
+            self._window = StreamWindow(video, self._frame_skip, end)
 
     def _end_clip(self) -> None:
         """Close the current clip; pause if the pass holds enough frames and another clip follows."""
@@ -116,7 +122,7 @@ class _ClipChain:
         r = self._result
         r.frames = video.frame_number - self._start_num
         if r.start is not None:
-            r.end = video.position
+            r.end = video.position  # past the last frame processed when frame_skip read frames behind it
         self.done.append((index, r, self._scored))
         self._next()
         if self.held >= self.bound and self._k < len(self._clips):
@@ -130,12 +136,12 @@ class _ClipChain:
 
     def read(self, decode: bool = True):
         while not self.paused and self._k < len(self._clips):
-            video = self._clips[self._k][1]
-            frame = video.read()
+            frame = self._window.read()
             if frame is not False:
                 if _dlpack.is_dlpack(frame) != self._on_cuda:
                     raise ValueError("a stream's frames are not where its group's are (host or CUDA)")
-                self._took(1, video.position)
+                self._pos = self._window.position
+                self._took(1, self._pos)
                 return frame
             self._end_clip()
         return False
@@ -147,19 +153,19 @@ class _ClipChain:
 
 
 class _DeviceClipChain(_ClipChain):
-    """The chain over CUDA streams with `read_batch`: views of one clip at a time, as SceneManager reads them."""
+    """The chain over CUDA streams with `read_batch`: views `chunk[skip::step]` of one clip at a time, as SceneManager
+    reads them (FrameBatches crops them)."""
 
     def __dlpack_device__(self):
         return self._clips[min(self._k, len(self._clips) - 1)][1].__dlpack_device__()
 
     def read_batch(self, max_frames: int):
         while not self.paused and self._k < len(self._clips):
-            video = self._clips[self._k][1]
-            pos0 = video.frame_number
-            chunk = video.read_batch(max_frames)
-            if chunk is not None:
-                self._took(int(chunk.shape[0]), FrameTimecode(pos0, video.frame_rate))
-                return chunk
+            got = self._window.read_views(max_frames)
+            if got is not None:
+                first, k, view = got
+                self._took(k, FrameTimecode(first, self._result.fps))
+                return view
             self._end_clip()
         return None
 
@@ -207,6 +213,7 @@ class _Pass:
                 if key is not None and key not in self.keys:
                     self.keys.append(key)
         self._bufs = {}
+        self.frame_step = 1         # frame_skip + 1 of the clips' windows: element i of a clip is frame first + i * step
         self.columns = None         # stats: [(CSV key, metric key, component or None, head, tail)] in CSV order
         self.components_key = None  # stats: the content_val key whose scan also writes the four components
         self.header = b""
@@ -304,8 +311,12 @@ class _Pass:
         cap = cuts.nbytes // 8
         st = engine.compute_stream
         for attempt in range(2):
-            check(lib.psd_clip_cuts(cells, k, offsets, first, c, min_frames, cuts.ptr, cap, obuf.ptr, st),
-                  "psd_clip_cuts")
+            if self.frame_step == 1:
+                check(lib.psd_clip_cuts(cells, k, offsets, first, c, min_frames, cuts.ptr, cap, obuf.ptr, st),
+                      "psd_clip_cuts")
+            else:  # post_process sees each clip's end position, past its last processed frame after skipped reads
+                check(lib.psd_clip_cuts_step(cells, k, offsets, first, c, min_frames, cuts.ptr, cap, obuf.ptr,
+                                             self.frame_step, first + c * 8, st), "psd_clip_cuts_step")
             engine.sync()
             total = int(obuf.download(8, offset=k * c * 8).view(np.int64)[0])
             if total <= cap:
@@ -382,12 +393,19 @@ def _group_key(video) -> tuple:
 
 
 def detect_clips(videos, detectors, auto_downscale: bool = True, downscale: int = 1, device: int = 0,
-                 batch_size: int = 64, stats: bool = False) -> list[ClipResult]:
+                 batch_size: int = 64, stats: bool = False, crop=None, duration=None, end_time=None,
+                 frame_skip: int = 0) -> list[ClipResult]:
     """Detect scenes in every stream of `videos` with every detector of `detectors`: for each clip, in input order,
-    what a fresh `SceneManager(device=device, batch_size=batch_size)` with these `auto_downscale` / `downscale` and
-    fresh copies of the detectors give from `detect_scenes(video)`.  Streams are anything `detect_scenes` reads
-    (`ArrayVideoStream` over numpy or CUDA arrays of any layout and channel order, a reference `VideoStream`) and may
-    differ in length, frame rate and frame size; a stream is read from its current position to its end.
+    what a fresh `SceneManager(device=device, batch_size=batch_size)` with these `auto_downscale` / `downscale` /
+    `crop` and fresh copies of the detectors give from `detect_scenes(video, duration=duration, end_time=end_time,
+    frame_skip=frame_skip)`.  Streams are anything `detect_scenes` reads (`ArrayVideoStream` over numpy or CUDA
+    arrays of any layout and channel order, a reference `VideoStream`) and may differ in length, frame rate and frame
+    size; a stream is read from its current position.
+
+    Every clip gets the same window, applied to it as detect_scenes applies it to one stream: `duration` counts from
+    the clip's own position, `end_time` from its base timecode, both at its own frame rate; the first frame is always
+    processed; `frame_skip` frames are read and not processed after each processed one, and `ClipResult.frames`
+    counts them.  `crop` is SceneManager.crop's (X0, Y0, X1, Y1), inclusive, in every clip.
 
     `stats=True`: every result also has `stats_csv`, the bytes `StatsManager.save_to_csv` writes (line terminator
     "\\n") after that SceneManager, built with a fresh `StatsManager()`, ran `detect_scenes(video)`: the header
@@ -397,7 +415,9 @@ def detect_clips(videos, detectors, auto_downscale: bool = True, downscale: int 
 
     The detectors are configuration only: they are not attached to an engine or otherwise changed.  ValueError for
     an empty detector list or a detector with a `stats_manager` (the detectors take no StatsManager here: ask for
-    `stats` instead)."""
+    `stats` instead), for the window arguments detect_scenes refuses (with its messages; `frame_skip` with `stats`
+    included), and, before any frame is read, for a crop that starts outside some clip's frame; TypeError for a
+    malformed crop."""
     detectors = list(detectors)
     if not detectors:
         raise ValueError("No detectors added")
@@ -406,14 +426,24 @@ def detect_clips(videos, detectors, auto_downscale: bool = True, downscale: int 
             raise TypeError("detect_clips drives the GPU detectors of this package")
         if d.stats_manager is not None:
             raise ValueError("detect_clips produces no per-frame metrics: detectors must not have a stats_manager")
+    check_window(duration, end_time, frame_skip, stats)
     if downscale < 1:
         raise ValueError("Downscale factor must be a positive integer >= 1!")
     geometry = SceneManager(device=device, batch_size=batch_size)
     geometry._auto_downscale, geometry._downscale = bool(auto_downscale), int(downscale)
+    geometry.crop = crop
     videos = list(videos)
+    if crop is not None:
+        for i, v in enumerate(videos):
+            fw, fh = v.frame_size
+            x0, y0 = geometry._crop[:2]
+            if x0 >= fw or y0 >= fh:
+                raise ValueError(f"crop starts outside video boundary of clip {i} ({fw}x{fh})")
     results: list = [None] * len(videos)
     device_pass = _Pass.of_detectors(detectors, device, stats=stats)
-    passes = clip_passes(videos, device_pass.groups, geometry, batch_size, device)
+    device_pass.frame_step = int(frame_skip) + 1
+    passes = clip_passes(videos, device_pass.groups, geometry, batch_size, device, frame_skip=frame_skip,
+                         duration=duration, end_time=end_time)
     try:
         for engine, holders, done in passes:
             device_pass.finish(engine, holders, [(r, m) for _, r, m in done])
@@ -425,10 +455,12 @@ def detect_clips(videos, detectors, auto_downscale: bool = True, downscale: int 
     return results
 
 
-def clip_passes(videos, groups, geometry, batch_size: int, device: int):
+def clip_passes(videos, groups, geometry, batch_size: int, device: int, frame_skip: int = 0, duration=None,
+                end_time=None):
     """Score the streams of `videos` pass by pass: clips grouped by `_group_key`, one engine per group built by
-    `shared_engine` with every pixel group of `groups` as a slot and `geometry._geometry` (a SceneManager's), the
-    clips of a group scored back to back.  Yields (engine, holders, done) at the end of every pass, `done` being
+    `shared_engine` with every pixel group of `groups` as a slot and `geometry._geometry` (a SceneManager's: its crop
+    and scored size), the clips of a group scored back to back, each through its own window of `frame_skip` /
+    `duration` / `end_time` (`_ClipChain`).  Frames scored are frames processed.  Yields (engine, holders, done) at the end of every pass, `done` being
     [(input index, ClipResult, frames scored)] of the clips the engine holds, in order; the engine is reset for the
     next pass when the consumer asks for it.  Close the generator to release the engine of an unfinished group."""
     by_key: dict = {}
@@ -437,7 +469,8 @@ def clip_passes(videos, groups, geometry, batch_size: int, device: int):
     for (size, on_cuda, views, order), clips in by_key.items():
         box, (w, h), (sw, sh) = geometry._geometry(*size)
         engine, holders = shared_engine(groups, w, h, sw, sh, device=device, max_batch=batch_size)
-        chain = (_DeviceClipChain if views else _ClipChain)(clips, MAX_PASS_FRAMES, on_cuda)
+        chain = (_DeviceClipChain if views else _ClipChain)(clips, MAX_PASS_FRAMES, on_cuda, frame_skip, duration,
+                                                           end_time)
         gather = FrameBatches(chain, box, (w, h), batch_size)
         try:
             while True:

@@ -6,7 +6,9 @@
 //                    NaN for an incomplete adaptive window or a frame without a predecessor)
 //   psd_clip_cuts    one thread per (cell, clip) runs the cell's automaton (cut_automata.cuh) over the clip's slice
 //                    of the metric arrays, with the clip's first frame number and min_frames: a counting pass, an
-//                    exclusive scan of the counts, then a writing pass into one compact cut array
+//                    exclusive scan of the counts, then a writing pass into one compact cut array.
+//                    psd_clip_cuts_step runs the same kernels on clips read with a frame skip: slice element i is
+//                    frame first + i * step, and post_process sees each clip's end position
 //   psd_clip_eval    the counterpart of psd_sweep_eval for psd_clip_cuts' compact output: every (cell, clip) list
 //                    turned in place into its predicted list, every (cell, clip, tolerance) scored against clip j's
 //                    ground truth with score_predictions (sweep_eval.cuh), and the counts summed over the clips
@@ -39,12 +41,15 @@ __global__ void __launch_bounds__(256) psd_clip_fill_kernel(double* __restrict__
 
 // Counting pass (WRITE = false): cut_offsets[t] = how many cuts (cell, clip) t emits.  Writing pass: the cuts of t
 // at cuts[cut_offsets[t] ..], after psd_clip_scan_kernel turned the counts into offsets; nothing when the total
-// exceeds cap.  t = cell * n_clips + clip, so one cell's clips are adjacent threads.
+// exceeds cap.  t = cell * n_clips + clip, so one cell's clips are adjacent threads.  Element i of clip j is frame
+// first_frame[j] + i * step; post_process's position is end_frame[j] - 1, or the last element's frame when end_frame
+// is NULL.
 template <bool WRITE>
 __global__ void __launch_bounds__(128) psd_clip_cuts_kernel(const psd_sweep_cell* __restrict__ cells, int32_t n_cells,
                                                             const int64_t* __restrict__ offsets,
                                                             const int64_t* __restrict__ first_frame, int32_t n_clips,
-                                                            const int64_t* __restrict__ min_frames,
+                                                            const int64_t* __restrict__ min_frames, int64_t step,
+                                                            const int64_t* __restrict__ end_frame,
                                                             int64_t* __restrict__ cuts, int64_t cap,
                                                             int64_t* __restrict__ cut_offsets) {
     const int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
@@ -59,7 +64,9 @@ __global__ void __launch_bounds__(128) psd_clip_cuts_kernel(const psd_sweep_cell
         out.cuts = cuts + o;
         out.cap = (int32_t)(cut_offsets[t + 1] - o);
     }
-    run_cell(cells[k], b, e - b, first_frame[j], min_frames[t], out);
+    const int64_t first = first_frame[j];
+    const int64_t last = end_frame ? end_frame[j] - 1 : first + (e - b - 1) * step;
+    run_cell(cells[k], b, e - b, first, step, last, min_frames[t], out);
     if (!WRITE) cut_offsets[t] = out.n;
 }
 
@@ -287,13 +294,15 @@ extern "C" int psd_clip_fill(double* values, int64_t n, const int64_t* clip_offs
     return PSD_OK;
 }
 
-extern "C" int psd_clip_cuts(const psd_sweep_cell* cells, int32_t n_cells, const int64_t* clip_offsets,
-                             const int64_t* clip_first_frame, int32_t n_clips, const int64_t* min_frames, int64_t* cuts,
-                             int64_t cuts_cap, int64_t* cut_offsets, void* stream) {
-    PSD_REQUIRE(clip_offsets, "psd_clip_cuts: no clip table");
-    PSD_REQUIRE(n_cells >= 0 && n_clips >= 0 && cuts_cap >= 0, "psd_clip_cuts: bad args");
-    PSD_REQUIRE(cut_offsets, "psd_clip_cuts: no cut_offsets array");
-    const int rc = validate_sweep_cells(cells, n_cells, "psd_clip_cuts");
+static int clip_cuts(const char* name, const psd_sweep_cell* cells, int32_t n_cells, const int64_t* clip_offsets,
+                     const int64_t* clip_first_frame, int32_t n_clips, const int64_t* min_frames, int64_t* cuts,
+                     int64_t cuts_cap, int64_t* cut_offsets, int64_t frame_step, const int64_t* clip_end_frame,
+                     void* stream) {
+    PSD_REQUIRE(clip_offsets, "%s: no clip table", name);
+    PSD_REQUIRE(n_cells >= 0 && n_clips >= 0 && cuts_cap >= 0, "%s: bad args", name);
+    PSD_REQUIRE(frame_step >= 1, "%s: frame_step must be >= 1", name);
+    PSD_REQUIRE(cut_offsets, "%s: no cut_offsets array", name);
+    const int rc = validate_sweep_cells(cells, n_cells, name);
     if (rc != PSD_OK) return rc;
     const int64_t m = (int64_t)n_cells * n_clips;
     cudaStream_t s = (cudaStream_t)stream;
@@ -301,24 +310,41 @@ extern "C" int psd_clip_cuts(const psd_sweep_cell* cells, int32_t n_cells, const
         PSD_CUDA(cudaMemsetAsync(cut_offsets, 0, sizeof(int64_t), s));
         return PSD_OK;
     }
-    PSD_REQUIRE(clip_first_frame && min_frames, "psd_clip_cuts: no clip first frames / min_frames");
-    PSD_REQUIRE(cuts || cuts_cap == 0, "psd_clip_cuts: no cut array");
+    PSD_REQUIRE(clip_first_frame && min_frames, "%s: no clip first frames / min_frames", name);
+    PSD_REQUIRE(cuts || cuts_cap == 0, "%s: no cut array", name);
     psd_sweep_cell* d_cells = nullptr;
     const size_t bytes = sizeof(psd_sweep_cell) * (size_t)n_cells;
     PSD_CUDA(cudaMallocAsync((void**)&d_cells, bytes, s));
     PSD_CUDA(cudaMemcpyAsync(d_cells, cells, bytes, cudaMemcpyHostToDevice, s));  // pageable: staged before return
     const unsigned blocks = (unsigned)((m + 127) / 128);
     psd_clip_cuts_kernel<false><<<blocks, 128, 0, s>>>(d_cells, n_cells, clip_offsets, clip_first_frame, n_clips,
-                                                       min_frames, cuts, cuts_cap, cut_offsets);
+                                                       min_frames, frame_step, clip_end_frame, cuts, cuts_cap,
+                                                       cut_offsets);
     PSD_CHECK_LAUNCH();
     psd_clip_scan_kernel<<<1, 1024, 0, s>>>(cut_offsets, m);
     PSD_CHECK_LAUNCH();
     psd_clip_cuts_kernel<true><<<blocks, 128, 0, s>>>(d_cells, n_cells, clip_offsets, clip_first_frame, n_clips,
-                                                      min_frames, cuts, cuts_cap, cut_offsets);
+                                                      min_frames, frame_step, clip_end_frame, cuts, cuts_cap,
+                                                      cut_offsets);
     PSD_CHECK_LAUNCH();
     count_launch(3);
     PSD_CUDA(cudaFreeAsync(d_cells, s));
     return PSD_OK;
+}
+
+extern "C" int psd_clip_cuts(const psd_sweep_cell* cells, int32_t n_cells, const int64_t* clip_offsets,
+                             const int64_t* clip_first_frame, int32_t n_clips, const int64_t* min_frames, int64_t* cuts,
+                             int64_t cuts_cap, int64_t* cut_offsets, void* stream) {
+    return clip_cuts("psd_clip_cuts", cells, n_cells, clip_offsets, clip_first_frame, n_clips, min_frames, cuts,
+                     cuts_cap, cut_offsets, 1, nullptr, stream);
+}
+
+extern "C" int psd_clip_cuts_step(const psd_sweep_cell* cells, int32_t n_cells, const int64_t* clip_offsets,
+                                  const int64_t* clip_first_frame, int32_t n_clips, const int64_t* min_frames,
+                                  int64_t* cuts, int64_t cuts_cap, int64_t* cut_offsets, int64_t frame_step,
+                                  const int64_t* clip_end_frame, void* stream) {
+    return clip_cuts("psd_clip_cuts_step", cells, n_cells, clip_offsets, clip_first_frame, n_clips, min_frames, cuts,
+                     cuts_cap, cut_offsets, frame_step, clip_end_frame, stream);
 }
 
 extern "C" int psd_clip_eval(int64_t* cuts, const int64_t* cut_offsets, int32_t n_cells, int32_t n_clips,

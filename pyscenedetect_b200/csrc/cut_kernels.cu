@@ -19,7 +19,7 @@ __global__ void psd_cuts_flash_filter_kernel(const uint8_t* __restrict__ above, 
                                              int32_t cap) {
     if (blockIdx.x != 0 || threadIdx.x != 0) return;
     CutSink out{cuts, cap, 0};
-    flash_filter_cuts([&](int64_t i) { return above[i] != 0; }, n, first_frame, min_frames, mode, out);
+    flash_filter_cuts([&](int64_t i) { return above[i] != 0; }, n, first_frame, 1, min_frames, mode, out);
     *count = out.n;
 }
 
@@ -29,7 +29,7 @@ __global__ void psd_cuts_adaptive_kernel(const double* __restrict__ ratio, const
                                          int32_t* count, int32_t cap) {
     if (blockIdx.x != 0 || threadIdx.x != 0) return;
     CutSink out{cuts, cap, 0};
-    adaptive_cuts(ratio, score, n, first_frame, window, adaptive_threshold, min_content_val, min_frames, out);
+    adaptive_cuts(ratio, score, n, first_frame, 1, window, adaptive_threshold, min_content_val, min_frames, out);
     *count = out.n;
 }
 
@@ -38,7 +38,7 @@ __global__ void psd_cuts_histogram_kernel(const double* __restrict__ correl, int
                                           int32_t cap) {
     if (blockIdx.x != 0 || threadIdx.x != 0) return;
     CutSink out{cuts, cap, 0};
-    histogram_cuts(correl, n, first_frame, threshold, min_frames, out);
+    histogram_cuts(correl, n, first_frame, 1, threshold, min_frames, out);
     *count = out.n;
 }
 
@@ -47,7 +47,7 @@ __global__ void psd_cuts_hash_kernel(const double* __restrict__ dist, int64_t n,
                                      int32_t cap) {
     if (blockIdx.x != 0 || threadIdx.x != 0) return;
     CutSink out{cuts, cap, 0};
-    hash_cuts(dist, n, first_frame, threshold, min_frames, out);
+    hash_cuts(dist, n, first_frame, 1, threshold, min_frames, out);
     *count = out.n;
 }
 
@@ -57,7 +57,8 @@ __global__ void psd_cuts_threshold_kernel(const double* __restrict__ avg, int64_
                                           int32_t* count, int32_t cap) {
     if (blockIdx.x != 0 || threadIdx.x != 0) return;
     CutSink out{cuts, cap, 0};
-    threshold_cuts(avg, n, first_frame, threshold, method_ceiling, fade_bias, min_frames, add_final_scene, out);
+    threshold_cuts(avg, n, first_frame, 1, first_frame + n - 1, threshold, method_ceiling, fade_bias, min_frames,
+                   add_final_scene, out);
     *count = out.n;
 }
 

@@ -22,7 +22,7 @@ __global__ void __launch_bounds__(128) psd_sweep_cuts_kernel(const psd_sweep_cel
     if (k >= n_cells) return;
     const psd_sweep_cell c = cells[k];
     CutSink out{cuts + (int64_t)k * cap, cap, 0};
-    run_cell(c, 0, n, first_frame, c.min_frames, out);
+    run_cell(c, 0, n, first_frame, 1, first_frame + n - 1, c.min_frames, out);
     count[k] = out.n;
 }
 

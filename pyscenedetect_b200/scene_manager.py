@@ -83,10 +83,97 @@ def shared_engine(groups, src_width: int, src_height: int, width: int, height: i
     return engine, holders
 
 
+def check_window(duration=None, end_time=None, frame_skip: int = 0, stats: bool = False) -> None:
+    """The argument checks of detect_scenes (scene_manager.py:500-515)."""
+    if frame_skip > 0 and stats:
+        raise ValueError("frame_skip must be 0 when using a StatsManager.")
+    if duration is not None and end_time is not None:
+        raise ValueError("duration and end_time cannot be set at the same time!")
+    if duration is not None and isinstance(duration, (int, float)) and duration < 0:
+        raise ValueError("duration must be greater than or equal to 0!")
+    if end_time is not None and isinstance(end_time, (int, float)) and end_time < 0:
+        raise ValueError("end_time must be greater than or equal to 0!")
+
+
+def base_timecode_of(video) -> FrameTimecode:
+    """The stream's base timecode, or frame 0 at its rate."""
+    base = getattr(video, "base_timecode", None)
+    return base if base is not None else FrameTimecode(0, video.frame_rate)
+
+
+def window_end_frame(base, start_frame: int, duration=None, end_time=None) -> int | None:
+    """scene_manager.py:543-547: end_time is absolute, duration is relative to the position the loop starts at
+    (`start_frame`); frames with position + 1 >= the result are the last ones processed (scene_manager.py:686-689).
+    None: read to the end."""
+    if end_time is not None:
+        return (base + end_time).frame_num
+    if duration is not None:
+        return ((base + duration) + start_frame).frame_num
+    return None
+
+
+class StreamWindow:
+    """Which frames of one stream the detection loop processes (scene_manager.py:650-689), from the stream's position
+    when the window is made: every (frame_skip + 1)-th frame, each followed by the frame_skip frames it skips (read,
+    not decoded), until a processed frame leaves the position + 1 >= `end_frame`; the first frame is processed in
+    any case.  `read()` for a stream read frame by frame, `read_views()` for a stream read with `read_batch`; a window
+    is read one way only."""
+
+    def __init__(self, video, frame_skip: int = 0, end_frame: int | None = None):
+        self.video = video
+        self.step = int(frame_skip) + 1
+        self.end_frame = end_frame
+        self.start = video.frame_number
+        self.processed = 0
+        self.done = False
+        self.position = None  # read(): the position of the last frame processed
+
+    def read(self):
+        """The next frame to process, after which the frames it skips are read; False at the end."""
+        if self.done:
+            return False
+        video = self.video
+        frame = video.read()
+        if frame is False:
+            self.done = True
+            return False
+        self.position = video.position
+        self.processed += 1
+        for _ in range(self.step - 1):  # scene_manager.py:682-685
+            if not video.read(decode=False):
+                break
+        if self.end_frame is not None and not (video.position.frame_num + 1) < self.end_frame:
+            self.done = True
+        return frame
+
+    def read_views(self, max_frames: int):
+        """Up to `max_frames` frames to process from one `read_batch`, with the frames each skips (and those still to
+        skip after the previous call's last one): (frame number of the first, count, view `chunk[skip::step]`), or
+        None at the end."""
+        video, end_frame, step = self.video, self.end_frame, self.step
+        while not self.done:
+            pos = video.frame_number
+            skip = (self.start - pos) % step   # frames still to skip after the last processed one
+            count = max_frames
+            if end_frame is not None:
+                count = min(count, max(-(-(end_frame - pos - skip) // step), 1 if self.processed == 0 else 0))
+            want = skip + count * step
+            chunk = video.read_batch(want) if want > 0 else None
+            if chunk is None:
+                self.done = True
+                return None
+            k = len(range(skip, chunk.shape[0], step))
+            if k == 0:
+                continue
+            self.processed += k
+            return pos + skip, k, (chunk if step == 1 else chunk[skip::step])
+        return None
+
+
 class FrameBatches:
     """The frame-gathering half of the detection loop (scene_manager.py:650-689): reads `video` in batches of
-    up to `batch_size` frames, cropped to `box` = (x0, y0, x1, y1) of size `size` = (w, h).  A stream with
-    `read_batch` and no crop / frame skip is read zero-copy; otherwise frames are copied into one of two
+    up to `batch_size` frames, cropped to `box` = (x0, y0, x1, y1) of size `size` = (w, h), through a `StreamWindow`.
+    A stream with `read_batch` and no crop / frame skip is read zero-copy; otherwise frames are copied into one of two
     page-locked buffers, so that a batch can be gathered while the GPU scores the previous one.
 
     Frames on the GPU (the stream's or the frames' `__dlpack_device__` says CUDA) never go through the host.  A
@@ -106,100 +193,70 @@ class FrameBatches:
         self._video = video
         self._box, self._size = box, size
         self._batch_size = int(batch_size)
-        self._frame_skip = frame_skip
-        self._end_frame = end_frame
+        self._window = StreamWindow(video, frame_skip, end_frame)
         self._device_views = hasattr(video, "read_batch") and _dlpack.on_cuda(video)
         self._zero_copy = hasattr(video, "read_batch") and not cropped and frame_skip == 0 and not self._device_views
-        self._start = video.frame_number
         self._pinned = [None, None]
         self._which = 0
         self._done = False
-        self._processed = 0
 
     def _next_views(self):
-        """The next batch of a CUDA stream with `read_batch`: frames start + j * step (step = frame_skip + 1) are
-        processed, each followed by the frame_skip frames it skips; with an end frame, those before it (and the
-        first frame in any case), as the host loop reads them."""
-        video, end_frame, step = self._video, self._end_frame, self._frame_skip + 1
+        """The next batch of a stream read with `read_batch`: CUDA views, or a zero-copy host view."""
+        got = self._window.read_views(self._batch_size)
+        if got is None:
+            self._done = True
+            return None
+        first, k, chunk = got
+        fps, step = self._video.frame_rate, self._window.step
+        tcs = [FrameTimecode(first + j * step, fps) for j in range(k)]
+        if self._zero_copy:
+            return tcs, chunk, bool(getattr(self._video, "is_pinned", False))
         x0, y0, x1, y1 = self._box
-        while True:
-            pos = video.frame_number
-            skip = (self._start - pos) % step   # frames still to skip after the last processed one
-            count = self._batch_size
-            if end_frame is not None:
-                count = min(count, max(-(-(end_frame - pos - skip) // step), 1 if self._processed == 0 else 0))
-            want = skip + count * step
-            chunk = video.read_batch(want) if want > 0 else None
-            if chunk is None:
-                self._done = True
-                return None
-            k = len(range(skip, chunk.shape[0], step))
-            if k == 0:
-                continue
-            self._processed += k
-            tcs = [FrameTimecode(pos + skip + j * step, video.frame_rate) for j in range(k)]
-            return tcs, chunk[skip::step, y0:y1, x0:x1], False
+        return tcs, chunk[:, y0:y1, x0:x1], False
 
     def next(self):
         if self._done:
             return None
-        if self._device_views:
+        if self._device_views or self._zero_copy:
             return self._next_views()
-        video, end_frame, zero_copy = self._video, self._end_frame, self._zero_copy
+        window = self._window
         x0, y0, x1, y1 = self._box
         w, h = self._size
-        fps = video.frame_rate
         tcs, batch = [], None
-        want = self._batch_size
-        if end_frame is not None and zero_copy:
-            # the frame at position p is processed, then the loop stops unless p + 1 < end; the first
-            # frame is always processed (the check follows the put, scene_manager.py:680-689)
-            want = min(want, max(end_frame - video.frame_number, 1 if self._processed == 0 else 0))
-        if want > 0:
-            if zero_copy:
-                pos0 = video.frame_number
-                view = video.read_batch(want)
-                if view is not None:
-                    batch = view
-                    tcs = [FrameTimecode(pos0 + i, fps) for i in range(view.shape[0])]
+        which = self._which
+        buf, views = None, []
+        k = 0
+        while k < self._batch_size:
+            frame = window.read()
+            if frame is False:
+                self._done = True
+                break
+            if _dlpack.is_dlpack(frame):
+                views.append(frame[y0:y1, x0:x1])
             else:
-                which = self._which
-                buf, views = None, []
-                k = 0
-                while k < want:
-                    frame = video.read()
-                    if frame is False:
-                        self._done = True
-                        break
-                    if _dlpack.is_dlpack(frame):
-                        views.append(frame[y0:y1, x0:x1])
-                    else:
-                        if buf is None:
-                            if self._pinned[which] is None:
-                                self._pinned[which] = PinnedBuffer(self._batch_size * w * h * 3)
-                            buf = self._pinned[which].array.reshape(self._batch_size, h, w, 3)
-                        np.copyto(buf[k], frame[y0:y1, x0:x1])
-                    tcs.append(video.position)
-                    k += 1
-                    for _ in range(self._frame_skip):  # scene_manager.py:682-685
-                        if not video.read(decode=False):
-                            break
-                    if end_frame is not None and not (video.position.frame_num + 1) < end_frame:
-                        self._done = True
-                        break
-                batch = (views if buf is None else buf[:k]) if k else None
+                if buf is None:
+                    if self._pinned[which] is None:
+                        self._pinned[which] = PinnedBuffer(self._batch_size * w * h * 3)
+                    buf = self._pinned[which].array.reshape(self._batch_size, h, w, 3)
+                np.copyto(buf[k], frame[y0:y1, x0:x1])
+            tcs.append(window.position)
+            k += 1
+            if window.done:
+                self._done = True
+                break
+        batch = (views if buf is None else buf[:k]) if k else None
         if batch is None:
             self._done = True
             return None
-        self._processed += len(tcs)
         self._which ^= 1
-        return tcs, batch, (not zero_copy) or bool(getattr(video, "is_pinned", False))
+        return tcs, batch, True
 
     def resume(self) -> None:
         """Read on after `next()` returned None, from a stream that reports an end and can then be read past it
         (clips.py's chain of clips pauses at a clip boundary so that the engine can be emptied).  The buffers are
         kept: the caller has synchronised every engine that read them."""
         self._done = False
+        self._window.done = False
 
     def close(self) -> None:
         for p in self._pinned:
@@ -338,14 +395,7 @@ class SceneManager:
                       show_progress: bool = False, callback=None) -> int:
         if not self._detector_list:
             raise ValueError("No detectors added")
-        if frame_skip > 0 and self._stats_manager is not None:
-            raise ValueError("frame_skip must be 0 when using a StatsManager.")
-        if duration is not None and end_time is not None:
-            raise ValueError("duration and end_time cannot be set at the same time!")
-        if duration is not None and isinstance(duration, (int, float)) and duration < 0:
-            raise ValueError("duration must be greater than or equal to 0!")
-        if end_time is not None and isinstance(end_time, (int, float)) and end_time < 0:
-            raise ValueError("end_time must be greater than or equal to 0!")
+        check_window(duration, end_time, frame_skip, self._stats_manager is not None)
         self.clear()
         self._frame_tail = []
         fw, fh = video.frame_size
@@ -354,18 +404,11 @@ class SceneManager:
                                               device=self._device, max_batch=self._batch_size)
         for d, holder in zip(self._detector_list, holders):
             d.attach_engine(holder)
-        fps = video.frame_rate
-        base = getattr(video, "base_timecode", None)
-        self._base_timecode = base if base is not None else FrameTimecode(0, fps)
+        self._base_timecode = base_timecode_of(video)
         if self._stats_manager is not None and hasattr(self._stats_manager, "_base_timecode"):
             self._stats_manager._base_timecode = self._base_timecode
-        # scene_manager.py:543-547: end_time is absolute, duration is relative to the current position
         start_frame_num = video.frame_number
-        end_frame = None  # frames with position + 1 >= end are the last ones processed (scene_manager.py:686-689)
-        if end_time is not None:
-            end_frame = (self._base_timecode + end_time).frame_num
-        elif duration is not None:
-            end_frame = ((self._base_timecode + duration) + start_frame_num).frame_num
+        end_frame = window_end_frame(self._base_timecode, start_frame_num, duration, end_time)
         self._channel_order = getattr(video, "channel_order", "bgr")
         gather = FrameBatches(video, (x0, y0, x1, y1), (w, h), self._batch_size, cropped=self._crop is not None,
                               frame_skip=frame_skip, end_frame=end_frame)
