@@ -340,6 +340,37 @@ int psd_clip_eval(int64_t* cuts, const int64_t* cut_offsets, int32_t n_cells, in
                   const int32_t* tolerances, int32_t n_tol, void* workspace, size_t workspace_bytes,
                   int32_t* out_n_pred, int64_t* out_hard, int64_t* out_fades, int64_t* out_totals_hard,
                   int64_t* out_totals_fades, int64_t* out_over, void* stream);
+/* ---- several clip tables in one launch: the same clips scored under several settings (crop, downscale, frame
+ * step), each setting's engine with its own pass layout ----
+ * One table (32 bytes) describes how one setting's engine holds the clips: clip j is elements [offsets[j],
+ * offsets[j+1]) of that setting's metric arrays, element i of it is frame first_frame[j] + i * frame_step, and
+ * end_frame[j] is the clip's end (the stream's position after that setting's reads + 1).  Every pointer is DEVICE
+ * memory; every table has the same n_clips.  psd_clip_cuts / psd_clip_cuts_step / psd_clip_eval are the one-table
+ * calls of these entries' kernels. */
+typedef struct psd_clip_table {
+    const int64_t* offsets;     /* int64[n_clips + 1] */
+    const int64_t* first_frame; /* int64[n_clips] (psd_clip_cuts_tables) */
+    const int64_t* end_frame;   /* int64[n_clips]; NULL for psd_clip_cuts_tables: post_process gets the last element */
+    int64_t frame_step;         /* >= 1 */
+} psd_clip_table;
+/* psd_clip_cuts_step with a table per cell: cell k runs over tables[cell_table[k]] (cell_table NULL: every cell over
+ * tables[0]), reading its own metric arrays, with min_frames[k * n_clips + j].  tables[n_tables] and
+ * cell_table[n_cells] are HOST arrays (validated, then copied on `stream` with the cells).  Output as psd_clip_cuts.
+ * Same kernels and launches as psd_clip_cuts. */
+int psd_clip_cuts_tables(const psd_sweep_cell* cells, int32_t n_cells, const psd_clip_table* tables, int32_t n_tables,
+                         const int32_t* cell_table, int32_t n_clips, const int64_t* min_frames, int64_t* cuts,
+                         int64_t cuts_cap, int64_t* cut_offsets, void* stream);
+/* psd_clip_eval with a table per cell: (cell k, clip j)'s predicted list ends at tables[cell_table[k]].end_frame[j]
+ * (cell_table NULL: tables[0]); only end_frame is read.  tables and cell_table are HOST arrays, copied on `stream`.
+ * Ground truth, outputs and workspace as psd_clip_eval: the ground truth is per clip, shared by every table.  Same
+ * kernels and launches as psd_clip_eval. */
+int psd_clip_eval_tables(int64_t* cuts, const int64_t* cut_offsets, int32_t n_cells, int32_t n_clips,
+                         int64_t cuts_total, int64_t max_cuts, const psd_clip_table* tables, int32_t n_tables,
+                         const int32_t* cell_table, const int64_t* gt_offsets, const int64_t* gt_cuts, int32_t n_gt,
+                         const int64_t* fade_offsets, const int64_t* fades, int32_t n_fades, const int32_t* tolerances,
+                         int32_t n_tol, void* workspace, size_t workspace_bytes, int32_t* out_n_pred,
+                         int64_t* out_hard, int64_t* out_fades, int64_t* out_totals_hard, int64_t* out_totals_fades,
+                         int64_t* out_over, void* stream);
 /* One column of a StatsManager CSV (stats_manager.py:save_to_csv) over a pass: frame i's value is values[i * stride]
  * (a psd_scan_* output, stride 1, or one component of psd_scan_content's out_components, stride 4).  The first `head`
  * and the last `tail` frames of every clip have no value there: the cell prints None. */

@@ -89,6 +89,18 @@ class PsdSweepCell(C.Structure):
 
 assert C.sizeof(PsdSweepCell) == 64
 
+class PsdClipTable(C.Structure):
+    """psd_clip_table: how one setting's engine holds the clips of a pass (32 bytes, DEVICE pointers)."""
+    _fields_ = [
+        ("offsets", C.c_void_p),
+        ("first_frame", C.c_void_p),
+        ("end_frame", C.c_void_p),
+        ("frame_step", C.c_int64),
+    ]
+
+
+assert C.sizeof(PsdClipTable) == 32
+
 STATS_MAX_COLUMNS = 64
 F64_TEXT = 32  # bytes per value of psd_test_format_f64
 
@@ -183,6 +195,9 @@ SIGNATURES = {
     "psd_clip_cuts_step": (C.c_int, [_vp, _i32, _vp, _vp, _i32, _vp, _vp, _i64, _vp, _i64, _vp, _vp]),
     "psd_clip_eval": (C.c_int, [_vp, _vp, _i32, _i32, _i64, _i64, _vp, _vp, _vp, _i32, _vp, _vp, _i32, _vp, _i32, _vp,
                                 C.c_size_t, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "psd_clip_cuts_tables": (C.c_int, [_vp, _i32, _vp, _i32, _vp, _i32, _vp, _vp, _i64, _vp, _vp]),
+    "psd_clip_eval_tables": (C.c_int, [_vp, _vp, _i32, _i32, _i64, _i64, _vp, _i32, _vp, _vp, _vp, _i32, _vp, _vp,
+                                       _i32, _vp, _i32, _vp, C.c_size_t, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "psd_clip_stats_csv": (C.c_int, [_vp, _i32, _vp, _vp, _vp, _i32, _i64, _vp, _vp, _i64, _vp, _vp]),
     "psd_engine_scan_content_host": (C.c_int, [_vp, _i64, _i64, _dp, _dbl, _vp, _vp]),
     "psd_engine_scan_adaptive_host": (C.c_int, [_vp, _vp, _i64, _i32, _dbl, _vp]),

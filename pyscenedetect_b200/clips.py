@@ -37,6 +37,7 @@ every clip's rows there (three launches a pass) and one download per pass brings
 from __future__ import annotations
 
 import csv
+import ctypes as C
 import io
 from dataclasses import dataclass, field
 from fractions import Fraction
@@ -183,6 +184,8 @@ class PassCuts:
     offsets: DeviceBuffer       # int64[n_cells * n_clips + 1]: exclusive offsets, then the total
     cuts: DeviceBuffer
     total: int
+    tables: object = None       # cuts_tables: every setting's psd_clip_table (HOST), for psd_clip_eval_tables
+    cell_table: object = None   # cuts_tables: the setting of every cell (HOST int32)
 
     @property
     def n_clips(self) -> int:
@@ -272,6 +275,52 @@ class _Pass:
             b.close()
         self._bufs = {}
 
+    def _scan(self, holders, offsets: int, c: int, n: int, tag=None) -> dict:
+        """Every metric array of the cells over the n frames `holders` hold, clips at the device table `offsets` of c
+        clips: one psd_scan_* (and its psd_clip_fill) per key.  `tag` keeps one setting's arrays apart from
+        another's."""
+        arrays = {key: self._buf(key if tag is None else (tag, key), n * 8) for key in self.keys}
+        comps = self._buf("components", n * 32).ptr if self.components_key is not None else None
+        for key in self.keys:
+            val = arrays[("content_val",) + key[1:3]].ptr if key[0] == "adaptive_ratio" else None
+            scan_metric(self._lib, holders[key[1]], (key[0],) + key[2:], arrays[key].ptr, val, clips=(offsets, c),
+                        components=comps if key == self.components_key else None)
+        return arrays
+
+    def _cells(self, arrays_of) -> C.Array:
+        """The psd_sweep_cell of every cell for each metric-array set of `arrays_of`, set-major."""
+        k = len(self.cells)
+        cells = (_capi.PsdSweepCell * (k * len(arrays_of)))()
+        for s, arrays in enumerate(arrays_of):
+            for i, cell in enumerate(self.cells):
+                cells[s * k + i] = _capi.PsdSweepCell(
+                    kind=_KIND[cell.kind], mode=cell.mode, metric=arrays[cell.metric].ptr,
+                    metric2=arrays[cell.metric2].ptr if cell.metric2 is not None else None, threshold=cell.threshold,
+                    min_content_val=cell.min_content_val, fade_bias=cell.fade_bias, min_frames=0, window=cell.window,
+                    add_final_scene=cell.add_final_scene)
+        return cells
+
+    def _cut_lists(self, engine, m: int, n: int, launch, name: str):
+        """The compact cut lists of m (cell, clip) automata over a pass of n frames: `launch(cuts, cap, offsets)`
+        queues the cut entry on the engine's stream; the buffer is grown once if the total needs more.
+        -> (offsets buffer, cuts buffer, total)."""
+        obuf = DeviceBuffer((m + 1) * 8, self.device)
+        cap = max(1, int(n * FIRST_CUTS_PER_FRAME)) if FIRST_CUTS_PER_FRAME > 0 else 0
+        cuts = DeviceBuffer(max(8, cap * 8), self.device)
+        cap = cuts.nbytes // 8
+        for attempt in range(2):
+            launch(cuts.ptr, cap, obuf.ptr)
+            engine.sync()
+            total = int(obuf.download(8, offset=m * 8).view(np.int64)[0])
+            if total <= cap:
+                break
+            if attempt:
+                raise RuntimeError(f"{name} needs {total} cuts after growing its buffer to {cap}")
+            cuts.close()
+            cuts = DeviceBuffer(total * 8, self.device)
+            cap = cuts.nbytes // 8
+        return obuf, cuts, total
+
     def cuts(self, engine, holders, clips: list) -> PassCuts | None:
         """Every (cell, clip) cut list of `clips` ((ClipResult, frames scored) of the frames `engine` holds, in
         order), left in device memory; None when no clip has a frame.  Only the cut total comes back to the host."""
@@ -292,41 +341,62 @@ class _Pass:
         tbuf = DeviceBuffer(table.nbytes, self.device)
         tbuf.upload(table)
         offsets, first, min_frames = tbuf.ptr, tbuf.ptr + (c + 1) * 8, tbuf.ptr + (3 * c + 1) * 8
-        arrays = {key: self._buf(key, n * 8) for key in self.keys}
-        comps = self._buf("components", n * 32).ptr if self.components_key is not None else None
-        for key in self.keys:
-            val = arrays[("content_val",) + key[1:3]].ptr if key[0] == "adaptive_ratio" else None
-            scan_metric(lib, holders[key[1]], (key[0],) + key[2:], arrays[key].ptr, val, clips=(offsets, c),
-                        components=comps if key == self.components_key else None)
-        cells = (_capi.PsdSweepCell * k)()
-        for i, cell in enumerate(self.cells):
-            cells[i] = _capi.PsdSweepCell(
-                kind=_KIND[cell.kind], mode=cell.mode, metric=arrays[cell.metric].ptr,
-                metric2=arrays[cell.metric2].ptr if cell.metric2 is not None else None, threshold=cell.threshold,
-                min_content_val=cell.min_content_val, fade_bias=cell.fade_bias, min_frames=0, window=cell.window,
-                add_final_scene=cell.add_final_scene)
-        obuf = DeviceBuffer((k * c + 1) * 8, self.device)
-        cap = max(1, int(n * FIRST_CUTS_PER_FRAME)) if FIRST_CUTS_PER_FRAME > 0 else 0
-        cuts = DeviceBuffer(max(8, cap * 8), self.device)
-        cap = cuts.nbytes // 8
+        cells = self._cells([self._scan(holders, offsets, c, n)])
         st = engine.compute_stream
-        for attempt in range(2):
+
+        def launch(cuts, cap, obuf):
             if self.frame_step == 1:
-                check(lib.psd_clip_cuts(cells, k, offsets, first, c, min_frames, cuts.ptr, cap, obuf.ptr, st),
-                      "psd_clip_cuts")
+                check(lib.psd_clip_cuts(cells, k, offsets, first, c, min_frames, cuts, cap, obuf, st), "psd_clip_cuts")
             else:  # post_process sees each clip's end position, past its last processed frame after skipped reads
-                check(lib.psd_clip_cuts_step(cells, k, offsets, first, c, min_frames, cuts.ptr, cap, obuf.ptr,
+                check(lib.psd_clip_cuts_step(cells, k, offsets, first, c, min_frames, cuts, cap, obuf,
                                              self.frame_step, first + c * 8, st), "psd_clip_cuts_step")
-            engine.sync()
-            total = int(obuf.download(8, offset=k * c * 8).view(np.int64)[0])
-            if total <= cap:
-                break
-            if attempt:
-                raise RuntimeError(f"psd_clip_cuts needs {total} cuts after growing its buffer to {cap}")
-            cuts.close()
-            cuts = DeviceBuffer(total * 8, self.device)
-            cap = cuts.nbytes // 8
+
+        obuf, cuts, total = self._cut_lists(engine, k * c, n, launch, "psd_clip_cuts")
         return PassCuts(scored, k, tbuf, obuf, cuts, total)
+
+    def cuts_tables(self, engines, holders, clips: list, steps: list) -> PassCuts:
+        """`cuts` for the same clips scored under several settings: setting s's engine `engines[s]` holds clip j's
+        clips[s][j] = (ClipResult, frames scored), element i of which is frame start + i * steps[s].  Each setting's
+        scans run on its engine with its own clip table; then ONE psd_clip_cuts_tables runs every (setting, cell, clip)
+        automaton, cell index s * len(cells) + k.  Every clip must have frames.  The result's `tables` hold each
+        setting's table, its `clips` are setting 0's."""
+        lib = self._lib
+        n_set, k, c = len(engines), len(self.cells), len(clips[0])
+        parts, lens = [], []
+        for s, e in enumerate(engines):
+            sizes = np.array([m for _, m in clips[s]], dtype=np.int64)
+            if not sizes.all() or int(sizes.sum()) != e.frame_count:
+                raise RuntimeError(f"setting {s}: the engine holds {e.frame_count} frames, the clips "
+                                   f"{sizes.tolist()}")
+            parts += [np.concatenate([[0], np.cumsum(sizes)]), [r.start.frame_num for r, _ in clips[s]],
+                      [r.end.frame_num + 1 for r, _ in clips[s]]]
+            lens.append(e.frame_count)
+        parts.append(np.tile([cell.min_frames(r.fps) for cell in self.cells for r, _ in clips[0]], n_set))
+        table = np.concatenate(parts).astype(np.int64)
+        tbuf = DeviceBuffer(table.nbytes, self.device)
+        tbuf.upload(table)
+        per = (3 * c + 1) * 8  # bytes of one setting's offsets, first frames and end frames
+        tables = (_capi.PsdClipTable * n_set)()
+        for s in range(n_set):
+            base = tbuf.ptr + s * per
+            tables[s] = _capi.PsdClipTable(offsets=base, first_frame=base + (c + 1) * 8,
+                                           end_frame=base + (2 * c + 1) * 8, frame_step=steps[s])
+        min_frames = tbuf.ptr + n_set * per
+        arrays = [self._scan(holders[s], tables[s].offsets, c, lens[s], tag=s if s else None) for s in range(n_set)]
+        for e in engines[1:]:  # the automata read every setting's arrays: order them after every engine's scans
+            e.sync()
+        cells = self._cells(arrays)
+        cell_table = (C.c_int32 * (n_set * k))(*[s for s in range(n_set) for _ in range(k)])
+        st = engines[0].compute_stream
+
+        def launch(cuts, cap, obuf):
+            check(lib.psd_clip_cuts_tables(cells, n_set * k, tables, n_set, cell_table, c, min_frames, cuts, cap, obuf,
+                                           st), "psd_clip_cuts_tables")
+
+        obuf, cuts, total = self._cut_lists(engines[0], n_set * k * c, sum(lens), launch, "psd_clip_cuts_tables")
+        pc = PassCuts([r for r, _ in clips[0]], n_set * k, tbuf, obuf, cuts, total)
+        pc.tables, pc.cell_table = tables, cell_table
+        return pc
 
     def stats_csv(self, engine, pc: PassCuts) -> list:
         """The CSV of every clip of `pc` (header and rows), printed on the device by one psd_clip_stats_csv from the

@@ -8,10 +8,13 @@
 //                    of the metric arrays, with the clip's first frame number and min_frames: a counting pass, an
 //                    exclusive scan of the counts, then a writing pass into one compact cut array.
 //                    psd_clip_cuts_step runs the same kernels on clips read with a frame skip: slice element i is
-//                    frame first + i * step, and post_process sees each clip's end position
+//                    frame first + i * step, and post_process sees each clip's end position; psd_clip_cuts_tables
+//                    gives each cell its own clip table (one per setting of a sweep over settings), and the other two
+//                    are its one-table calls
 //   psd_clip_eval    the counterpart of psd_sweep_eval for psd_clip_cuts' compact output: every (cell, clip) list
 //                    turned in place into its predicted list, every (cell, clip, tolerance) scored against clip j's
-//                    ground truth with score_predictions (sweep_eval.cuh), and the counts summed over the clips
+//                    ground truth with score_predictions (sweep_eval.cuh), and the counts summed over the clips;
+//                    psd_clip_eval_tables ends each cell's lists at the end frames of the cell's clip table
 //   psd_clip_stats_csv  every clip's StatsManager CSV rows (stats_csv.cuh formats them): one thread per frame counts
 //                    its row's bytes, an exclusive scan gives the row offsets, and the writing pass prints each row in
 //                    place, so one download carries every clip's text
@@ -19,11 +22,25 @@
 // cells and clips.
 #include <math_constants.h>
 
+#include <cstddef>
+
 #include "cut_automata.cuh"
 #include "stats_csv.cuh"
 #include "sweep_eval.cuh"
 
 namespace psd {
+
+// A psd_clip_table as the kernels read it, under a name of this namespace: every symbol that starts psd_clip_ is then
+// a clip_kernels.cu kernel or entry, never a parameter type.
+struct ClipTable {
+    const int64_t* offsets;
+    const int64_t* first_frame;
+    const int64_t* end_frame;
+    int64_t frame_step;
+};
+static_assert(sizeof(ClipTable) == sizeof(psd_clip_table) && offsetof(ClipTable, end_frame) ==
+                  offsetof(psd_clip_table, end_frame) && offsetof(ClipTable, frame_step) ==
+                  offsetof(psd_clip_table, frame_step), "ClipTable must be laid out as psd_clip_table");
 
 __global__ void __launch_bounds__(256) psd_clip_fill_kernel(double* __restrict__ values, int64_t n,
                                                             const int64_t* __restrict__ offsets, int32_t n_clips,
@@ -41,22 +58,22 @@ __global__ void __launch_bounds__(256) psd_clip_fill_kernel(double* __restrict__
 
 // Counting pass (WRITE = false): cut_offsets[t] = how many cuts (cell, clip) t emits.  Writing pass: the cuts of t
 // at cuts[cut_offsets[t] ..], after psd_clip_scan_kernel turned the counts into offsets; nothing when the total
-// exceeds cap.  t = cell * n_clips + clip, so one cell's clips are adjacent threads.  Element i of clip j is frame
-// first_frame[j] + i * step; post_process's position is end_frame[j] - 1, or the last element's frame when end_frame
-// is NULL.
+// exceeds cap.  t = cell * n_clips + clip, so one cell's clips are adjacent threads.  Cell k reads clip table
+// tables[cell_table[k]] (tables[0] when cell_table is NULL): element i of clip j is frame first_frame[j] + i * step;
+// post_process's position is end_frame[j] - 1, or the last element's frame when end_frame is NULL.
 template <bool WRITE>
 __global__ void __launch_bounds__(128) psd_clip_cuts_kernel(const psd_sweep_cell* __restrict__ cells, int32_t n_cells,
-                                                            const int64_t* __restrict__ offsets,
-                                                            const int64_t* __restrict__ first_frame, int32_t n_clips,
-                                                            const int64_t* __restrict__ min_frames, int64_t step,
-                                                            const int64_t* __restrict__ end_frame,
+                                                            const ClipTable* __restrict__ tables,
+                                                            const int32_t* __restrict__ cell_table, int32_t n_clips,
+                                                            const int64_t* __restrict__ min_frames,
                                                             int64_t* __restrict__ cuts, int64_t cap,
                                                             int64_t* __restrict__ cut_offsets) {
     const int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
     const int64_t m = (int64_t)n_cells * n_clips;
     if (t >= m) return;
     const int64_t k = t / n_clips, j = t % n_clips;
-    const int64_t b = max(offsets[j], (int64_t)0), e = max(offsets[j + 1], b);
+    const ClipTable tb = tables[cell_table ? cell_table[k] : 0];
+    const int64_t b = max(tb.offsets[j], (int64_t)0), e = max(tb.offsets[j + 1], b);
     CutSink out{nullptr, 0, 0};  // cap 0: counts only
     if (WRITE) {
         if (cut_offsets[m] > cap) return;
@@ -64,8 +81,8 @@ __global__ void __launch_bounds__(128) psd_clip_cuts_kernel(const psd_sweep_cell
         out.cuts = cuts + o;
         out.cap = (int32_t)(cut_offsets[t + 1] - o);
     }
-    const int64_t first = first_frame[j];
-    const int64_t last = end_frame ? end_frame[j] - 1 : first + (e - b - 1) * step;
+    const int64_t first = tb.first_frame[j], step = tb.frame_step;
+    const int64_t last = tb.end_frame ? tb.end_frame[j] - 1 : first + (e - b - 1) * step;
     run_cell(cells[k], b, e - b, first, step, last, min_frames[t], out);
     if (!WRITE) cut_offsets[t] = out.n;
 }
@@ -133,14 +150,16 @@ __global__ void __launch_bounds__(128) clip_pred_kernel(int64_t* __restrict__ cu
     n_pred[t] = u ? u + 1 : 0;
 }
 
-// One thread per (cell k, clip j, tolerance q), tid = (k * n_clips + j) * n_tol + q.  The matching bitmaps are laid
+// One thread per (cell k, clip j, tolerance q), tid = (k * n_clips + j) * n_tol + q; clip j ends at end_frame[j] of
+// cell k's clip table (as in psd_clip_cuts_kernel).  The matching bitmaps are laid
 // out so that their offsets follow from the CSR offsets alone: list t's bits start at word t + floor(o_t / 32) of
 // tolerance q's block of words_p, clip j's ground-truth bits at word j + floor(gb_j / 32) of the (k, q) block of
 // words_g (likewise the fades).  Segment t needs floor(c_t / 32) + 1 words, and t + 1 starts at least that far on.
 __global__ void __launch_bounds__(128) clip_eval_kernel(
     const int64_t* __restrict__ cuts, const int64_t* __restrict__ cut_offsets, const int32_t* __restrict__ n_pred,
-    int32_t n_cells, int32_t n_clips, int64_t cuts_total, const int64_t* __restrict__ end_frame,
-    const int64_t* __restrict__ gt_offsets, const int64_t* __restrict__ gt, int32_t n_gt,
+    int32_t n_cells, int32_t n_clips, int64_t cuts_total, const ClipTable* __restrict__ tables,
+    const int32_t* __restrict__ cell_table, const int64_t* __restrict__ gt_offsets, const int64_t* __restrict__ gt,
+    int32_t n_gt,
     const int64_t* __restrict__ fade_offsets, const int64_t* __restrict__ fades, int32_t n_fades, Tolerances tols,
     int32_t n_tol, uint32_t* __restrict__ workspace, int64_t words_p, int64_t words_g, int64_t words_f,
     int64_t* __restrict__ out_hard, int64_t* __restrict__ out_fades) {
@@ -169,7 +188,8 @@ __global__ void __launch_bounds__(128) clip_eval_kernel(
     for (int64_t w = 0; w < words_for(np); ++w) used_p[w] = 0u;
     for (int64_t w = 0; w < words_for(ge - gb); ++w) used_g[w] = 0u;
     for (int64_t w = 0; w < words_for(fe - fb); ++w) used_f[w] = 0u;
-    score_predictions(cuts + b, np, end_frame[j], gt + gb, (int32_t)(ge - gb), fades + 2 * fb, (int32_t)(fe - fb),
+    const int64_t end_frame = tables[cell_table ? cell_table[k] : 0].end_frame[j];
+    score_predictions(cuts + b, np, end_frame, gt + gb, (int32_t)(ge - gb), fades + 2 * fb, (int32_t)(fe - fb),
                       tolerance_at(tols, q), used_p, used_g, used_f, hard, fade_counts);
 }
 
@@ -294,15 +314,46 @@ extern "C" int psd_clip_fill(double* values, int64_t n, const int64_t* clip_offs
     return PSD_OK;
 }
 
-static int clip_cuts(const char* name, const psd_sweep_cell* cells, int32_t n_cells, const int64_t* clip_offsets,
-                     const int64_t* clip_first_frame, int32_t n_clips, const int64_t* min_frames, int64_t* cuts,
-                     int64_t cuts_cap, int64_t* cut_offsets, int64_t frame_step, const int64_t* clip_end_frame,
-                     void* stream) {
-    PSD_REQUIRE(clip_offsets, "%s: no clip table", name);
+// The cells, the clip tables and the cells' table indices, copied in one device allocation on `s` (pageable: staged
+// before return); *d_cells NULL when the copy failed.
+static int copy_tables(const psd_sweep_cell* cells, int32_t n_cells, const psd_clip_table* tables, int32_t n_tables,
+                       const int32_t* cell_table, cudaStream_t s, psd_sweep_cell** d_cells, ClipTable** d_tables,
+                       int32_t** d_cell_table) {
+    const size_t cb = sizeof(psd_sweep_cell) * (size_t)(cells ? n_cells : 0);
+    const size_t tb = sizeof(psd_clip_table) * (size_t)n_tables;
+    const size_t ib = cell_table ? sizeof(int32_t) * (size_t)n_cells : 0;
+    char* d = nullptr;
+    *d_cells = nullptr;
+    PSD_CUDA(cudaMallocAsync((void**)&d, cb + tb + ib, s));
+    if (cb) PSD_CUDA(cudaMemcpyAsync(d, cells, cb, cudaMemcpyHostToDevice, s));
+    PSD_CUDA(cudaMemcpyAsync(d + cb, tables, tb, cudaMemcpyHostToDevice, s));
+    if (ib) PSD_CUDA(cudaMemcpyAsync(d + cb + tb, cell_table, ib, cudaMemcpyHostToDevice, s));
+    *d_cells = (psd_sweep_cell*)d;
+    *d_tables = (ClipTable*)(d + cb);
+    *d_cell_table = ib ? (int32_t*)(d + cb + tb) : nullptr;
+    return PSD_OK;
+}
+
+// Every cell's table index in [0, n_tables).
+static int check_tables(const char* name, int32_t n_tables, const int32_t* cell_table, int32_t n_cells) {
+    if (cell_table)
+        for (int32_t k = 0; k < n_cells; ++k)
+            PSD_REQUIRE(cell_table[k] >= 0 && cell_table[k] < n_tables, "%s: cell %d names table %d of %d", name, k,
+                        cell_table[k], n_tables);
+    return PSD_OK;
+}
+
+static int clip_cuts(const char* name, const psd_sweep_cell* cells, int32_t n_cells, const psd_clip_table* tables,
+                     int32_t n_tables, const int32_t* cell_table, int32_t n_clips, const int64_t* min_frames,
+                     int64_t* cuts, int64_t cuts_cap, int64_t* cut_offsets, void* stream) {
+    PSD_REQUIRE(tables && n_tables >= 1, "%s: no clip table", name);
+    for (int32_t i = 0; i < n_tables; ++i) PSD_REQUIRE(tables[i].offsets, "%s: no clip table", name);
     PSD_REQUIRE(n_cells >= 0 && n_clips >= 0 && cuts_cap >= 0, "%s: bad args", name);
-    PSD_REQUIRE(frame_step >= 1, "%s: frame_step must be >= 1", name);
+    for (int32_t i = 0; i < n_tables; ++i) PSD_REQUIRE(tables[i].frame_step >= 1, "%s: frame_step must be >= 1", name);
     PSD_REQUIRE(cut_offsets, "%s: no cut_offsets array", name);
-    const int rc = validate_sweep_cells(cells, n_cells, name);
+    int rc = check_tables(name, n_tables, cell_table, n_cells);
+    if (rc != PSD_OK) return rc;
+    rc = validate_sweep_cells(cells, n_cells, name);
     if (rc != PSD_OK) return rc;
     const int64_t m = (int64_t)n_cells * n_clips;
     cudaStream_t s = (cudaStream_t)stream;
@@ -310,22 +361,22 @@ static int clip_cuts(const char* name, const psd_sweep_cell* cells, int32_t n_ce
         PSD_CUDA(cudaMemsetAsync(cut_offsets, 0, sizeof(int64_t), s));
         return PSD_OK;
     }
-    PSD_REQUIRE(clip_first_frame && min_frames, "%s: no clip first frames / min_frames", name);
+    for (int32_t i = 0; i < n_tables; ++i)
+        PSD_REQUIRE(tables[i].first_frame && min_frames, "%s: no clip first frames / min_frames", name);
     PSD_REQUIRE(cuts || cuts_cap == 0, "%s: no cut array", name);
-    psd_sweep_cell* d_cells = nullptr;
-    const size_t bytes = sizeof(psd_sweep_cell) * (size_t)n_cells;
-    PSD_CUDA(cudaMallocAsync((void**)&d_cells, bytes, s));
-    PSD_CUDA(cudaMemcpyAsync(d_cells, cells, bytes, cudaMemcpyHostToDevice, s));  // pageable: staged before return
+    psd_sweep_cell* d_cells;
+    ClipTable* d_tables;
+    int32_t* d_cell_table;
+    rc = copy_tables(cells, n_cells, tables, n_tables, cell_table, s, &d_cells, &d_tables, &d_cell_table);
+    if (rc != PSD_OK) return rc;
     const unsigned blocks = (unsigned)((m + 127) / 128);
-    psd_clip_cuts_kernel<false><<<blocks, 128, 0, s>>>(d_cells, n_cells, clip_offsets, clip_first_frame, n_clips,
-                                                       min_frames, frame_step, clip_end_frame, cuts, cuts_cap,
-                                                       cut_offsets);
+    psd_clip_cuts_kernel<false><<<blocks, 128, 0, s>>>(d_cells, n_cells, d_tables, d_cell_table, n_clips, min_frames,
+                                                       cuts, cuts_cap, cut_offsets);
     PSD_CHECK_LAUNCH();
     psd_clip_scan_kernel<<<1, 1024, 0, s>>>(cut_offsets, m);
     PSD_CHECK_LAUNCH();
-    psd_clip_cuts_kernel<true><<<blocks, 128, 0, s>>>(d_cells, n_cells, clip_offsets, clip_first_frame, n_clips,
-                                                      min_frames, frame_step, clip_end_frame, cuts, cuts_cap,
-                                                      cut_offsets);
+    psd_clip_cuts_kernel<true><<<blocks, 128, 0, s>>>(d_cells, n_cells, d_tables, d_cell_table, n_clips, min_frames,
+                                                      cuts, cuts_cap, cut_offsets);
     PSD_CHECK_LAUNCH();
     count_launch(3);
     PSD_CUDA(cudaFreeAsync(d_cells, s));
@@ -335,48 +386,61 @@ static int clip_cuts(const char* name, const psd_sweep_cell* cells, int32_t n_ce
 extern "C" int psd_clip_cuts(const psd_sweep_cell* cells, int32_t n_cells, const int64_t* clip_offsets,
                              const int64_t* clip_first_frame, int32_t n_clips, const int64_t* min_frames, int64_t* cuts,
                              int64_t cuts_cap, int64_t* cut_offsets, void* stream) {
-    return clip_cuts("psd_clip_cuts", cells, n_cells, clip_offsets, clip_first_frame, n_clips, min_frames, cuts,
-                     cuts_cap, cut_offsets, 1, nullptr, stream);
+    const psd_clip_table table{clip_offsets, clip_first_frame, nullptr, 1};
+    return clip_cuts("psd_clip_cuts", cells, n_cells, &table, 1, nullptr, n_clips, min_frames, cuts, cuts_cap,
+                     cut_offsets, stream);
 }
 
 extern "C" int psd_clip_cuts_step(const psd_sweep_cell* cells, int32_t n_cells, const int64_t* clip_offsets,
                                   const int64_t* clip_first_frame, int32_t n_clips, const int64_t* min_frames,
                                   int64_t* cuts, int64_t cuts_cap, int64_t* cut_offsets, int64_t frame_step,
                                   const int64_t* clip_end_frame, void* stream) {
-    return clip_cuts("psd_clip_cuts_step", cells, n_cells, clip_offsets, clip_first_frame, n_clips, min_frames, cuts,
-                     cuts_cap, cut_offsets, frame_step, clip_end_frame, stream);
+    const psd_clip_table table{clip_offsets, clip_first_frame, clip_end_frame, frame_step};
+    return clip_cuts("psd_clip_cuts_step", cells, n_cells, &table, 1, nullptr, n_clips, min_frames, cuts, cuts_cap,
+                     cut_offsets, stream);
 }
 
-extern "C" int psd_clip_eval(int64_t* cuts, const int64_t* cut_offsets, int32_t n_cells, int32_t n_clips,
-                             int64_t cuts_total, int64_t max_cuts, const int64_t* clip_end_frame,
-                             const int64_t* gt_offsets, const int64_t* gt_cuts, int32_t n_gt,
-                             const int64_t* fade_offsets, const int64_t* fades, int32_t n_fades,
-                             const int32_t* tolerances, int32_t n_tol, void* workspace, size_t workspace_bytes,
-                             int32_t* out_n_pred, int64_t* out_hard, int64_t* out_fades, int64_t* out_totals_hard,
-                             int64_t* out_totals_fades, int64_t* out_over, void* stream) {
-    PSD_REQUIRE(n_cells >= 0 && n_clips >= 0 && cuts_total >= 0 && n_gt >= 0 && n_fades >= 0,
-                "psd_clip_eval: bad args");
-    PSD_REQUIRE(max_cuts >= 0 && max_cuts <= INT32_MAX, "psd_clip_eval: max_cuts must be 0 to %d", INT32_MAX);
-    PSD_REQUIRE(tolerances && n_tol >= 1 && n_tol <= PSD_SWEEP_MAX_TOLERANCES, "psd_clip_eval: 1 to %d tolerances",
+extern "C" int psd_clip_cuts_tables(const psd_sweep_cell* cells, int32_t n_cells, const psd_clip_table* tables,
+                                    int32_t n_tables, const int32_t* cell_table, int32_t n_clips,
+                                    const int64_t* min_frames, int64_t* cuts, int64_t cuts_cap, int64_t* cut_offsets,
+                                    void* stream) {
+    return clip_cuts("psd_clip_cuts_tables", cells, n_cells, tables, n_tables, cell_table, n_clips, min_frames, cuts,
+                     cuts_cap, cut_offsets, stream);
+}
+
+static int clip_eval(const char* name, int64_t* cuts, const int64_t* cut_offsets, int32_t n_cells, int32_t n_clips,
+                     int64_t cuts_total, int64_t max_cuts, const psd_clip_table* tables, int32_t n_tables,
+                     const int32_t* cell_table, const int64_t* gt_offsets, const int64_t* gt_cuts, int32_t n_gt,
+                     const int64_t* fade_offsets, const int64_t* fades, int32_t n_fades, const int32_t* tolerances,
+                     int32_t n_tol, void* workspace, size_t workspace_bytes, int32_t* out_n_pred, int64_t* out_hard,
+                     int64_t* out_fades, int64_t* out_totals_hard, int64_t* out_totals_fades, int64_t* out_over,
+                     void* stream) {
+    PSD_REQUIRE(n_cells >= 0 && n_clips >= 0 && cuts_total >= 0 && n_gt >= 0 && n_fades >= 0, "%s: bad args", name);
+    PSD_REQUIRE(max_cuts >= 0 && max_cuts <= INT32_MAX, "%s: max_cuts must be 0 to %d", name, INT32_MAX);
+    PSD_REQUIRE(tolerances && n_tol >= 1 && n_tol <= PSD_SWEEP_MAX_TOLERANCES, "%s: 1 to %d tolerances", name,
                 PSD_SWEEP_MAX_TOLERANCES);
     Tolerances tols{};
     for (int32_t q = 0; q < n_tol; ++q) {
-        PSD_REQUIRE(tolerances[q] >= 0, "psd_clip_eval: tolerance %d is negative", tolerances[q]);
+        PSD_REQUIRE(tolerances[q] >= 0, "%s: tolerance %d is negative", name, tolerances[q]);
         tols.t[q] = tolerances[q];
     }
-    PSD_REQUIRE(out_over, "psd_clip_eval: no out_over");
+    PSD_REQUIRE(out_over, "%s: no out_over", name);
     const int64_t m = (int64_t)n_cells * n_clips;
-    PSD_REQUIRE(n_cells == 0 || (out_totals_hard && out_totals_fades), "psd_clip_eval: no totals arrays");
+    PSD_REQUIRE(n_cells == 0 || (out_totals_hard && out_totals_fades), "%s: no totals arrays", name);
     if (m > 0) {
-        PSD_REQUIRE(cut_offsets && clip_end_frame && gt_offsets && fade_offsets, "psd_clip_eval: no clip tables");
-        PSD_REQUIRE(cuts || cuts_total == 0, "psd_clip_eval: cuts is NULL");
-        PSD_REQUIRE(n_gt == 0 || gt_cuts, "psd_clip_eval: gt_cuts is NULL");
-        PSD_REQUIRE(n_fades == 0 || fades, "psd_clip_eval: fades is NULL");
-        PSD_REQUIRE(out_n_pred && out_hard && out_fades, "psd_clip_eval: no output arrays");
+        bool ends = tables && n_tables >= 1;
+        for (int32_t i = 0; ends && i < n_tables; ++i) ends = tables[i].end_frame != nullptr;
+        PSD_REQUIRE(cut_offsets && ends && gt_offsets && fade_offsets, "%s: no clip tables", name);
+        PSD_REQUIRE(cuts || cuts_total == 0, "%s: cuts is NULL", name);
+        PSD_REQUIRE(n_gt == 0 || gt_cuts, "%s: gt_cuts is NULL", name);
+        PSD_REQUIRE(n_fades == 0 || fades, "%s: fades is NULL", name);
+        PSD_REQUIRE(out_n_pred && out_hard && out_fades, "%s: no output arrays", name);
+        const int rc = check_tables(name, n_tables, cell_table, n_cells);
+        if (rc != PSD_OK) return rc;
     }
     const int64_t wp = m + words_for(cuts_total), wg = n_clips + words_for(n_gt), wf = n_clips + words_for(n_fades);
     const size_t need = 4u * ((size_t)n_tol * (size_t)wp + (size_t)n_cells * (size_t)n_tol * (size_t)(wg + wf));
-    PSD_REQUIRE(m == 0 || (workspace && workspace_bytes >= need), "psd_clip_eval: workspace needs %zu bytes", need);
+    PSD_REQUIRE(m == 0 || (workspace && workspace_bytes >= need), "%s: workspace needs %zu bytes", name, need);
     cudaStream_t s = (cudaStream_t)stream;
     PSD_CUDA(cudaMemsetAsync(out_over, 0xFF, sizeof(int64_t), s));  // -1: no list longer than max_cuts
     if (m == 0) {  // no clip: every total is 0
@@ -386,12 +450,17 @@ extern "C" int psd_clip_eval(int64_t* cuts, const int64_t* cut_offsets, int32_t 
         }
         return PSD_OK;
     }
+    psd_sweep_cell* d_alloc;
+    ClipTable* d_tables;
+    int32_t* d_cell_table;
+    int rc = copy_tables(nullptr, n_cells, tables, n_tables, cell_table, s, &d_alloc, &d_tables, &d_cell_table);
+    if (rc != PSD_OK) return rc;
     clip_pred_kernel<<<(unsigned)((m + 127) / 128), 128, 0, s>>>(cuts, cut_offsets, m, cuts_total, max_cuts,
                                                                   out_n_pred, (unsigned long long*)out_over);
     PSD_CHECK_LAUNCH();
     const int64_t threads = m * n_tol;
     clip_eval_kernel<<<(unsigned)((threads + 127) / 128), 128, 0, s>>>(
-        cuts, cut_offsets, out_n_pred, n_cells, n_clips, cuts_total, clip_end_frame, gt_offsets, gt_cuts, n_gt,
+        cuts, cut_offsets, out_n_pred, n_cells, n_clips, cuts_total, d_tables, d_cell_table, gt_offsets, gt_cuts, n_gt,
         fade_offsets, fades, n_fades, tols, n_tol, (uint32_t*)workspace, wp, wg, wf, out_hard, out_fades);
     PSD_CHECK_LAUNCH();
     const int64_t sums = (int64_t)n_cells * ((int64_t)n_tol * 5 + 3);
@@ -399,7 +468,36 @@ extern "C" int psd_clip_eval(int64_t* cuts, const int64_t* cut_offsets, int32_t 
                                                                      out_totals_hard, out_totals_fades);
     PSD_CHECK_LAUNCH();
     count_launch(3);
+    PSD_CUDA(cudaFreeAsync(d_alloc, s));
     return PSD_OK;
+}
+
+extern "C" int psd_clip_eval(int64_t* cuts, const int64_t* cut_offsets, int32_t n_cells, int32_t n_clips,
+                             int64_t cuts_total, int64_t max_cuts, const int64_t* clip_end_frame,
+                             const int64_t* gt_offsets, const int64_t* gt_cuts, int32_t n_gt,
+                             const int64_t* fade_offsets, const int64_t* fades, int32_t n_fades,
+                             const int32_t* tolerances, int32_t n_tol, void* workspace, size_t workspace_bytes,
+                             int32_t* out_n_pred, int64_t* out_hard, int64_t* out_fades, int64_t* out_totals_hard,
+                             int64_t* out_totals_fades, int64_t* out_over, void* stream) {
+    const psd_clip_table table{nullptr, nullptr, clip_end_frame, 1};
+    return clip_eval("psd_clip_eval", cuts, cut_offsets, n_cells, n_clips, cuts_total, max_cuts, &table, 1, nullptr,
+                     gt_offsets, gt_cuts, n_gt, fade_offsets, fades, n_fades, tolerances, n_tol, workspace,
+                     workspace_bytes, out_n_pred, out_hard, out_fades, out_totals_hard, out_totals_fades, out_over,
+                     stream);
+}
+
+extern "C" int psd_clip_eval_tables(int64_t* cuts, const int64_t* cut_offsets, int32_t n_cells, int32_t n_clips,
+                                    int64_t cuts_total, int64_t max_cuts, const psd_clip_table* tables,
+                                    int32_t n_tables, const int32_t* cell_table, const int64_t* gt_offsets,
+                                    const int64_t* gt_cuts, int32_t n_gt, const int64_t* fade_offsets,
+                                    const int64_t* fades, int32_t n_fades, const int32_t* tolerances, int32_t n_tol,
+                                    void* workspace, size_t workspace_bytes, int32_t* out_n_pred, int64_t* out_hard,
+                                    int64_t* out_fades, int64_t* out_totals_hard, int64_t* out_totals_fades,
+                                    int64_t* out_over, void* stream) {
+    return clip_eval("psd_clip_eval_tables", cuts, cut_offsets, n_cells, n_clips, cuts_total, max_cuts, tables,
+                     n_tables, cell_table, gt_offsets, gt_cuts, n_gt, fade_offsets, fades, n_fades, tolerances, n_tol,
+                     workspace, workspace_bytes, out_n_pred, out_hard, out_fades, out_totals_hard, out_totals_fades,
+                     out_over, stream);
 }
 
 extern "C" int psd_clip_stats_csv(const psd_stats_column* columns, int32_t n_columns, const int64_t* clip_offsets,

@@ -178,6 +178,14 @@ class Engine:
                                                _capi.SUBMIT_PINNED if pinned else 0),
               "psd_engine_submit_host")
 
+    def submit_layout(self, base: int, n_frames: int, layout: tuple):
+        """Score n_frames BGR frames at device pointer `base` (channel B of pixel (0, 0) of the first), laid out as
+        `layout` = (frame, row, pixel, channel) byte strides, of this engine's source size.  The memory is the
+        caller's: it must stay unchanged until the engine has synchronised."""
+        lay = _capi.PsdFrameLayout(*layout)
+        check(self._lib.psd_engine_submit_device_layout(self._h, int(base), int(n_frames), C.byref(lay)),
+              "psd_engine_submit_device_layout")
+
     def submit_device(self, dptr: int, n_frames: int, frame_stride: int | None = None):
         check(self._lib.psd_engine_submit_device(self._h, dptr, int(n_frames),
                                                  int(frame_stride or self.src_frame_bytes)),

@@ -128,6 +128,15 @@ class StreamWindow:
         self.done = False
         self.position = None  # read(): the position of the last frame processed
 
+    @staticmethod
+    def frames_read(step: int, start: int, end_frame: int | None) -> int | None:
+        """How many frames a window of `step` made at frame number `start` reads, if the stream does not end first:
+        frames start + i * step for every i with that frame < end_frame (and i = 0 in any case) are processed, each
+        followed by its step - 1 skipped reads.  None without an end frame: the window reads to the end."""
+        if end_frame is None:
+            return None
+        return step * max(1, -(-(end_frame - start) // step))
+
     def read(self):
         """The next frame to process, after which the frames it skips are read; False at the end."""
         if self.done:

@@ -23,6 +23,11 @@ Usage::
     r = sw.run(video, ground_truth=GroundTruth(hard_cuts=[...], fades=[(start, end), ...]))
     r.cuts(k); r.hard(k, 1); r.hard_offset(k, 1); r.fades(k)
     sw.totals()   # counts summed over every video run so far, with precision / recall / F1
+
+`settings` adds how frames are read and scored (auto_downscale, downscale, crop, frame_skip) as a second axis:
+`ParameterSweep(..., settings=[{}, {"frame_skip": 1}, {"crop": (0, 60, 1279, 659)}]).run_clips(videos, gts,
+duration="30s")` reads each clip once for every setting (fan_out.py) and evaluates every (setting, cell, clip) with
+one psd_clip_cuts_tables and one psd_clip_eval_tables per pass.
 """
 
 from __future__ import annotations
@@ -38,7 +43,7 @@ from ._capi import check
 from .detectors._base import EngineDetector, PixelGroup, pixel_group_of
 from .device_cuts import automaton_args, flash_filter_frames, histogram_threshold, min_len_frames, scan_metric
 from .engine import DeviceBuffer
-from .scene_manager import FrameBatches, SceneManager, shared_engine
+from .scene_manager import FrameBatches, SceneManager, check_window, shared_engine
 
 _KIND = {"content": _capi.SWEEP_CONTENT, "adaptive": _capi.SWEEP_ADAPTIVE, "threshold": _capi.SWEEP_THRESHOLD,
          "histogram": _capi.SWEEP_HISTOGRAM, "hash": _capi.SWEEP_HASH}
@@ -160,6 +165,7 @@ class SweepResult:
         self._hard, self._fades = hard, fades
         self._cuts_buf, self._cap = cuts_buf, cap
         self.end_frame = end_frame
+        self.end_frames = [end_frame]  # one per setting; `end_frame` is setting 0's
         self.grid_ms = grid_ms  # scans + psd_sweep_cuts + psd_sweep_eval, host clock ending in a sync
 
     def __len__(self) -> int:
@@ -198,6 +204,36 @@ class SweepResult:
     def fades(self, k: int) -> tuple[int, int, int]:
         f = self._fades[self._slot[k]]
         return int(f[0]), int(f[1]), int(f[2])
+
+
+class _OneClipResult(SweepResult):
+    """`run`'s result when the video went through the clip path (settings or a window): clip 0 of a
+    ClipSweepResult, with the accessors of SweepResult."""
+
+    def __init__(self, r: ClipSweepResult):
+        self._r = r
+        self.tolerances = r.tolerances
+        self.end_frames = [r.end_frame(0, setting=s) for s in range(r.n_settings)]
+        self.end_frame = self.end_frames[0]
+        self.grid_ms = r.grid_ms
+
+    def __len__(self) -> int:
+        return len(self._r)
+
+    def cuts(self, k: int) -> list[int]:
+        return self._r.cuts(k, 0)
+
+    def raw_count(self, k: int) -> int:
+        return self._r.raw_count(k, 0)
+
+    def hard(self, k: int, tol: int) -> tuple[int, int, int]:
+        return self._r.hard(k, 0, tol)
+
+    def hard_offset(self, k: int, tol: int) -> tuple[float, int]:
+        return self._r.hard_offset(k, 0, tol)
+
+    def fades(self, k: int) -> tuple[int, int, int]:
+        return self._r.fades(k, 0)
 
 
 def _cell_totals(grid, tolerances, th, tf) -> list[CellTotals]:
@@ -241,16 +277,21 @@ class _ClipPass:
 
 class ClipSweepResult:
     """Every (cell, clip) of one `ParameterSweep.run_clips` call.  Per-(cell, clip) counts and cut lists stay in
-    device memory until an accessor reads them; `totals` holds this call's counts summed over its clips."""
+    device memory until an accessor reads them; `totals` holds this call's counts summed over its clips.  Cells are
+    settings x grid, settings-major: cell k is setting k // n_grid's run of grid cell k % n_grid; `grid` holds every
+    cell's params ({**setting, **grid cell})."""
 
-    def __init__(self, grid, tolerances, passes, where, end_frames, totals_hard, totals_fades, grid_ms):
+    def __init__(self, grid, tolerances, passes, where, end_frames, totals_hard, totals_fades, grid_ms,
+                 n_grid: int | None = None, upload_bytes: int | None = None):
         self.grid = grid
         self.tolerances = tuple(tolerances)
         self._passes = passes        # [_ClipPass]
         self._where = where          # clip -> (pass index, index within the pass)
-        self._end = end_frames
+        self._end = end_frames       # [setting][clip]
+        self._n_grid = n_grid or len(grid)
         self._th, self._tf = totals_hard, totals_fades
-        self.grid_ms = grid_ms       # scans + psd_clip_cuts + psd_clip_eval of every pass, host clock ending in syncs
+        self.grid_ms = grid_ms       # scans + cut and eval entries of every pass, host clock ending in syncs
+        self.upload_bytes = upload_bytes  # host frame bytes copied to the device (settings path; None otherwise)
 
     def __len__(self) -> int:
         return len(self.grid)
@@ -258,6 +299,10 @@ class ClipSweepResult:
     @property
     def n_clips(self) -> int:
         return len(self._where)
+
+    @property
+    def n_settings(self) -> int:
+        return len(self._end)
 
     def _at(self, k: int, j: int):
         if not 0 <= k < len(self.grid):
@@ -272,9 +317,10 @@ class ClipSweepResult:
         except ValueError:
             raise KeyError(f"tolerance {tol} was not evaluated (tolerances {self.tolerances})") from None
 
-    def end_frame(self, j: int) -> int:
-        """Clip j's end as SceneManager.get_scene_list ends it: its last position + 1 (clip-local frames)."""
-        return self._end[j]
+    def end_frame(self, j: int, setting: int = 0) -> int:
+        """Clip j's end under setting `setting` as SceneManager.get_scene_list ends it: its last position + 1
+        (clip-local frames).  Settings differ when their frame skips read past the window differently."""
+        return self._end[setting][j]
 
     def cuts(self, k: int, j: int) -> list[int]:
         """Cell k's predicted list on clip j, as `SweepResult.cuts` gives it: sorted unique cuts, then the clip's
@@ -285,7 +331,7 @@ class ClipSweepResult:
             return []
         o = int(ps.host("offsets")[t])
         got = ps.cuts_buf.download((m - 1) * 8, offset=o * 8).view(np.int64).tolist()
-        return got + [self._end[j]]
+        return got + [self._end[k // self._n_grid][j]]
 
     def raw_count(self, k: int, j: int) -> int:
         """How many cuts cell k's automaton emitted on clip j (before de-duplication)."""
@@ -315,19 +361,56 @@ class ClipSweepResult:
         return _cell_totals(self.grid, self.tolerances, self._th, self._tf)
 
 
+SETTING_KEYS = ("auto_downscale", "downscale", "crop", "frame_skip")
+
+
+def _setting_geometry(setting: dict, device: int, batch_size: int) -> SceneManager:
+    """A SceneManager configured with one setting's `auto_downscale`, `downscale` and `crop` through its own setters
+    (their checks, messages and warnings: `downscale` is ignored while `auto_downscale` is on), whose `_geometry`
+    the setting's engines are built with."""
+    unknown = sorted(set(setting) - set(SETTING_KEYS))
+    if unknown:
+        raise TypeError(f"unknown setting key(s) {unknown}: a setting takes {', '.join(SETTING_KEYS)}")
+    sm = SceneManager(device=device, batch_size=batch_size)
+    if "auto_downscale" in setting:
+        sm.auto_downscale = setting["auto_downscale"]
+    if "downscale" in setting:
+        sm.downscale = setting["downscale"]
+    if "crop" in setting:
+        sm.crop = setting["crop"]
+    skip = setting.get("frame_skip", 0)
+    if isinstance(skip, bool) or not isinstance(skip, (int, np.integer)):
+        raise TypeError("frame_skip must be an integer")
+    if skip < 0:
+        raise ValueError("frame_skip must be >= 0")
+    return sm
+
+
 class ParameterSweep:
     """Every cell of `grid` (a list of `detector_cls(**params)` keyword dicts, as the reference harness takes
     them) over each video `run` is given.  `detector_cls` is one of this package's detectors; each cell is
     built by its constructor, so defaults, validation, `luma_only` and the histogram's threshold map are the
-    constructor's own."""
+    constructor's own.
+
+    `settings` sweeps how the frames are read and scored as well: a list of dicts with the keys `auto_downscale`,
+    `downscale`, `crop` (SceneManager's properties) and `frame_skip` (detect_scenes'), each checked as those check
+    it.  The cells are settings x grid, settings-major (cell s * len(grid) + g, params {**settings[s], **grid[g]}).
+    None means [{}]: one setting, SceneManager's defaults, and the cells of the grid alone."""
 
     def __init__(self, detector_cls, grid, tolerances=(0, 1), device: int = 0, batch_size: int = 64,
-                 max_cuts_per_cell: int = 4096):
+                 max_cuts_per_cell: int = 4096, settings=None):
         if not (isinstance(detector_cls, type) and issubclass(detector_cls, EngineDetector)):
             raise TypeError("ParameterSweep sweeps the detectors of this package")
         self.grid = [dict(p) for p in grid]
         if not self.grid:
             raise ValueError("the grid has no cells")
+        self.settings = [{}] if settings is None else [dict(x) for x in settings]
+        if not self.settings:
+            raise ValueError("settings is empty (None means one setting with SceneManager's defaults)")
+        self._geometries = [_setting_geometry(x, int(device), int(batch_size)) for x in self.settings]
+        self._frame_skips = [int(x.get("frame_skip", 0)) for x in self.settings]
+        self._default_settings = self.settings == [{}]
+        self.params = [{**x, **g} for x in self.settings for g in self.grid]
         tols = tuple(int(t) for t in tolerances)
         if not 1 <= len(tols) <= _capi.SWEEP_MAX_TOLERANCES or any(t < 0 for t in tols) or len(set(tols)) != len(tols):
             raise ValueError(f"tolerances must be 1 to {_capi.SWEEP_MAX_TOLERANCES} distinct non-negative frame counts")
@@ -361,16 +444,23 @@ class ParameterSweep:
         for s, k in enumerate(self.order):
             self.slot_of[k] = s
         self._lib = None
-        self._totals_hard = np.zeros((len(self.cells), len(tols), 5), dtype=np.int64)
-        self._totals_fades = np.zeros((len(self.cells), 3), dtype=np.int64)
+        self._totals_hard = np.zeros((len(self.params), len(tols), 5), dtype=np.int64)
+        self._totals_fades = np.zeros((len(self.params), 3), dtype=np.int64)
         self.videos = 0
 
     # -- the whole pass --
-    def run(self, video, ground_truth: GroundTruth | None = None) -> SweepResult:
+    def run(self, video, ground_truth: GroundTruth | None = None, duration=None, end_time=None) -> SweepResult:
         """Decode `video` once, score it with one Engine (SceneManager's default geometry: auto-downscale, no
         crop) that holds every pixel group's kernel size and hash geometry as a slot, then evaluate every cell.
         Without ground truth nothing is scored (every count is against an empty truth) and `totals` is not
-        updated."""
+        updated.
+
+        With settings other than the default, or a window (`duration` / `end_time`, as detect_scenes takes them),
+        the video goes through `run_clips` as its one clip: cell k's results are run_clips' (k, 0), `end_frames`
+        holds every setting's end frame and `end_frame` setting 0's."""
+        if not self._default_settings or duration is not None or end_time is not None:
+            gts = None if ground_truth is None else [ground_truth]
+            return _OneClipResult(self._run_clips([video], gts, duration, end_time, "the video"))
         fw, fh = video.frame_size
         box, (w, h), (sw, sh) = SceneManager()._geometry(fw, fh)
         engine, holders = shared_engine(self.groups, w, h, sw, sh, device=self.device, max_batch=self.batch_size)
@@ -471,23 +561,36 @@ class ParameterSweep:
                            grid_ms)
 
     # -- many clips per pass --
-    def run_clips(self, videos, ground_truths=None) -> ClipSweepResult:
+    def run_clips(self, videos, ground_truths=None, duration=None, end_time=None) -> ClipSweepResult:
         """Every cell over every stream of `videos`: for each (cell, clip), what `run(videos[j], ground_truths[j])`
         gives on a fresh ParameterSweep with this grid, tolerances and batch size; `totals` and `videos` afterwards
         are what a loop of `run` leaves.  Streams are anything `detect_clips` reads (host or CUDA `ArrayVideoStream`s
         of any layout and channel order, reference `VideoStream`s) and may differ in length, frame rate and frame
-        size; each is read from its current position, with SceneManager's default geometry, and its frame numbers
-        are clip-local.
+        size; each is read from its current position and its frame numbers are clip-local.
 
-        The clips are scored as `detect_clips` scores them, pass by pass.  Each pass ends with the scans, ONE
-        psd_clip_cuts for every (cell, clip) automaton and ONE psd_clip_eval that scores every (cell, clip,
-        tolerance) against clip j's ground truth and sums the counts over the pass's clips on the device; only
-        those sums and the cut total come back to the host.
+        With settings, cell (s, g) on clip j is what a fresh SceneManager with setting s's `auto_downscale`,
+        `downscale` and `crop` finds with `detector_cls(**grid[g])` in `detect_scenes(videos[j], duration=,
+        end_time=, frame_skip=)`: its sorted unique cuts followed by its end position + 1, scored against
+        ground_truths[j].  `duration` / `end_time` give every setting and clip the same window, as in
+        `detect_clips`.  Each stream is read once for every setting (fan_out.py): afterwards it stands at the end of
+        the union of the settings' windows, which a frame skip can put past some settings' own ends.
+
+        The clips are scored as `detect_clips` scores them, pass by pass.  Each pass ends with every setting's
+        scans, ONE cut entry (psd_clip_cuts; psd_clip_cuts_tables for settings) for every (cell, clip) automaton and
+        ONE eval entry (psd_clip_eval / psd_clip_eval_tables) that scores every (cell, clip, tolerance) against clip
+        j's ground truth and sums the counts over the pass's clips on the device; only those sums and the cut total
+        come back to the host.
 
         `ground_truths`: None (every count is against an empty truth and `totals` is not updated), or one
-        GroundTruth per video.  ValueError for a length mismatch or a clip without frames, RuntimeError for a
-        (cell, clip) with more than max_cuts_per_cell cuts; `totals` only changes when the call returns."""
+        GroundTruth per video.  ValueError for a length mismatch, a clip without frames, a window detect_scenes
+        refuses (its messages) or, before any frame is read, a crop that starts outside some clip's frame (naming
+        the clip and the setting); RuntimeError for a (cell, clip) with more than max_cuts_per_cell cuts; `totals`
+        only changes when the call returns."""
+        return self._run_clips(videos, ground_truths, duration, end_time, "clip {}")
+
+    def _run_clips(self, videos, ground_truths, duration, end_time, clip_name: str) -> ClipSweepResult:
         from .clips import _Pass, clip_passes
+        from .fan_out import settings_passes
         videos = list(videos)
         if ground_truths is None:
             gts = [GroundTruth([])] * len(videos)
@@ -497,24 +600,47 @@ class ParameterSweep:
                 raise ValueError(f"{len(videos)} videos need as many ground truths, got {len(gts)}")
             if not all(isinstance(g, GroundTruth) for g in gts):
                 raise ValueError("every ground truth must be a GroundTruth (GroundTruth([]) for a clip without cuts)")
+        check_window(duration, end_time)
+        for s, g in enumerate(self._geometries):
+            if g._crop is not None:
+                x0, y0 = g._crop[:2]
+                for i, v in enumerate(videos):
+                    fw, fh = v.frame_size
+                    if x0 >= fw or y0 >= fh:
+                        raise ValueError(f"crop starts outside video boundary of clip {i} ({fw}x{fh}) in setting {s} "
+                                         f"({self.settings[s]})")
         lib = self._lib = self._lib or _capi.load()
-        n_cells, n_tol, dev = len(self.cells), len(self.tolerances), self.device
+        n_grid, n_set, n_tol, dev = len(self.cells), len(self.settings), len(self.tolerances), self.device
+        n_cells = n_set * n_grid
         tols = (C.c_int32 * n_tol)(*self.tolerances)
         th = np.zeros((n_cells, n_tol, 5), dtype=np.int64)
         tf = np.zeros((n_cells, 3), dtype=np.int64)
-        passes, where, ends = [], [None] * len(videos), [0] * len(videos)
+        passes, where, ends = [], [None] * len(videos), [[0] * len(videos) for _ in range(n_set)]
         grid_ms = 0.0
+        counters = {}
         device_pass = _Pass(self.cells, self.groups, dev)
-        scoring = clip_passes(videos, self.groups, SceneManager(device=dev, batch_size=self.batch_size),
-                              self.batch_size, dev)
+        if self._default_settings:
+            scoring = clip_passes(videos, self.groups, SceneManager(device=dev, batch_size=self.batch_size),
+                                  self.batch_size, dev, duration=duration, end_time=end_time)
+        else:
+            scoring = settings_passes(videos, self.groups, self._geometries, self._frame_skips, self.batch_size, dev,
+                                      duration=duration, end_time=end_time, counters=counters)
+        steps = [f + 1 for f in self._frame_skips]
         try:
             for engine, holders, done in scoring:
-                for index, _r, m in done:
-                    if not m:
-                        raise ValueError(f"clip {index} has no frames")
+                if self._default_settings:
+                    done = [(index, [r], [m]) for index, r, m in done]
+                for index, _rs, ms in done:
+                    if not ms[0]:
+                        raise ValueError(f"{clip_name.format(index)} has no frames")
                 t0 = time.perf_counter()
-                pc = device_pass.cuts(engine, holders, [(r, m) for _, r, m in done])
-                indices = [index for index, _r, _m in done]
+                if self._default_settings:
+                    pc = device_pass.cuts(engine, holders, [(rs[0], ms[0]) for _, rs, ms in done])
+                else:
+                    pc = device_pass.cuts_tables(engine, holders, [[(rs[s], ms[s]) for _, rs, ms in done]
+                                                                   for s in range(n_set)], steps)
+                    engine = engine[0]
+                indices = [index for index, _rs, _ms in done]
                 c = pc.n_clips
                 ggt = [gts[i] for i in indices]
                 gt_off = np.concatenate([[0], np.cumsum([len(g.hard_cuts) for g in ggt])]).astype(np.int64)
@@ -532,11 +658,16 @@ class ParameterSweep:
                 sums = DeviceBuffer(n_cells * (n_tol * 5 + 3) * 8 + 8, dev)  # totals_hard, totals_fades, over
                 try:
                     gt_cuts = gbuf.ptr + 2 * (c + 1) * 8
-                    check(lib.psd_clip_eval(
-                        pc.cuts.ptr, pc.offsets.ptr, n_cells, c, pc.total, self.cap, pc.end_frames, gbuf.ptr, gt_cuts,
-                        n_gt, gbuf.ptr + (c + 1) * 8, gt_cuts + n_gt * 8, n_fades, tols, n_tol, ws.ptr, ws.nbytes,
-                        n_pred.ptr, hard.ptr, fades.ptr, sums.ptr, sums.ptr + n_cells * n_tol * 40,
-                        sums.ptr + n_cells * (n_tol * 5 + 3) * 8, engine.compute_stream), "psd_clip_eval")
+                    truth = (gbuf.ptr, gt_cuts, n_gt, gbuf.ptr + (c + 1) * 8, gt_cuts + n_gt * 8, n_fades, tols, n_tol,
+                             ws.ptr, ws.nbytes, n_pred.ptr, hard.ptr, fades.ptr, sums.ptr,
+                             sums.ptr + n_cells * n_tol * 40, sums.ptr + n_cells * (n_tol * 5 + 3) * 8,
+                             engine.compute_stream)
+                    if pc.tables is None:
+                        check(lib.psd_clip_eval(pc.cuts.ptr, pc.offsets.ptr, n_cells, c, pc.total, self.cap,
+                                                pc.end_frames, *truth), "psd_clip_eval")
+                    else:
+                        check(lib.psd_clip_eval_tables(pc.cuts.ptr, pc.offsets.ptr, n_cells, c, pc.total, self.cap,
+                                                       pc.tables, n_set, pc.cell_table, *truth), "psd_clip_eval_tables")
                     engine.sync()
                     grid_ms += (time.perf_counter() - t0) * 1e3
                     got = sums.download(sums.nbytes).view(np.int64)
@@ -547,13 +678,16 @@ class ParameterSweep:
                 if over >= 0:
                     k, jj = divmod(over, c)
                     o = pc.offsets.download(16, offset=over * 8).view(np.int64)
-                    raise RuntimeError(f"cell {k} ({self.grid[k]}) found {int(o[1] - o[0])} cuts in clip "
+                    where_k = f"({self.grid[k]})" if self._default_settings else \
+                        f"({self.grid[k % n_grid]}) of setting {k // n_grid} ({self.settings[k // n_grid]})"
+                    raise RuntimeError(f"cell {k} {where_k} found {int(o[1] - o[0])} cuts in clip "
                                        f"{indices[jj]}, more than max_cuts_per_cell={self.cap}")
                 th += got[:n_cells * n_tol * 5].reshape(n_cells, n_tol, 5)
                 tf += got[n_cells * n_tol * 5:-1].reshape(n_cells, 3)
-                for jj, (index, r) in enumerate(zip(indices, pc.clips)):
+                for jj, (index, rs, _ms) in enumerate(done):
                     where[index] = (len(passes), jj)
-                    ends[index] = r.end.frame_num + 1
+                    for s in range(n_set):
+                        ends[s][index] = rs[s].end.frame_num + 1
                 passes.append(_ClipPass(pc, n_tol, n_pred, hard, fades))
         finally:
             scoring.close()
@@ -562,11 +696,12 @@ class ParameterSweep:
             self._totals_hard += th
             self._totals_fades += tf
             self.videos += len(videos)
-        return ClipSweepResult(self.grid, self.tolerances, passes, where, ends, th, tf, grid_ms)
+        return ClipSweepResult(self.params, self.tolerances, passes, where, ends, th, tf, grid_ms, n_grid=n_grid,
+                               upload_bytes=None if self._default_settings else counters.get("uploaded", 0))
 
     def totals(self) -> list[CellTotals]:
         """Every cell's counts summed over the videos and clips run with ground truth so far, in grid order."""
-        return _cell_totals(self.grid, self.tolerances, self._totals_hard, self._totals_fades)
+        return _cell_totals(self.params, self.tolerances, self._totals_hard, self._totals_fades)
 
 
 __all__ = ["ParameterSweep", "SweepResult", "ClipSweepResult", "GroundTruth", "EventCounts", "CellTotals",
