@@ -371,6 +371,26 @@ int psd_clip_eval_tables(int64_t* cuts, const int64_t* cut_offsets, int32_t n_ce
                          int32_t n_tol, void* workspace, size_t workspace_bytes, int32_t* out_n_pred,
                          int64_t* out_hard, int64_t* out_fades, int64_t* out_totals_hard, int64_t* out_totals_fades,
                          int64_t* out_over, void* stream);
+/* ---- cells that are sets of detectors: one SceneManager with several detectors cuts at the sorted union of their
+ * cuts (scene_manager.py:403-408) ---- */
+#define PSD_SWEEP_MAX_MEMBERS 16 /* lists per cell of psd_clip_union */
+/* Every (cell, clip) union of psd_clip_cuts' (list, clip) cut lists, in two calls with the same arguments.  cuts /
+ * cut_offsets are psd_clip_cuts' output over n_lists cells (here: lists) and n_clips clips, cuts_total its total.
+ * Cell k is the set of lists cell_lists[cell_offsets[k] .. cell_offsets[k + 1]): 1 to PSD_SWEEP_MAX_MEMBERS indices
+ * in [0, n_lists), repeats allowed; cell_offsets[n_cells + 1] (cell_offsets[0] = 0) and cell_lists are HOST int32
+ * arrays (validated, then copied on `stream`).  unique is a DEVICE int32[n_lists * n_clips] workspace kept between
+ * the two calls; everything else but the cell table is DEVICE memory.
+ *   Counting call (out_cuts NULL, out_cap 0; three launches): every list is sorted and de-duplicated in place (the
+ *   lists are read by many cells) and its length stored in unique; a list with more than max_cuts cuts counts as
+ *   empty and out_over[0] receives the lowest such list * n_clips + clip, or -1.  out_offsets[n_cells * n_clips + 1]
+ *   receives the exclusive offsets of the (cell, clip) unions, cell-major, and their total.
+ *   Writing call (out_cuts of out_cap entries; one launch): out_cuts[out_offsets[t] ..] receives the strictly
+ *   increasing union of (cell, clip) t, from the lists, unique and out_offsets the counting call left; nothing when
+ *   the total exceeds out_cap.  out_over is not written. */
+int psd_clip_union(int64_t* cuts, const int64_t* cut_offsets, int32_t n_lists, int32_t n_clips, int64_t cuts_total,
+                   int64_t max_cuts, const int32_t* cell_offsets, const int32_t* cell_lists, int32_t n_cells,
+                   int32_t* unique, int64_t* out_cuts, int64_t out_cap, int64_t* out_offsets, int64_t* out_over,
+                   void* stream);
 /* One column of a StatsManager CSV (stats_manager.py:save_to_csv) over a pass: frame i's value is values[i * stride]
  * (a psd_scan_* output, stride 1, or one component of psd_scan_content's out_components, stride 4).  The first `head`
  * and the last `tail` frames of every clip have no value there: the cell prints None. */

@@ -69,6 +69,7 @@ SWEEP_THRESHOLD = 2
 SWEEP_HISTOGRAM = 3
 SWEEP_HASH = 4
 SWEEP_MAX_TOLERANCES = 8
+SWEEP_MAX_MEMBERS = 16  # detectors per set of a sweep over detector sets (PSD_SWEEP_MAX_MEMBERS, psd_clip_union)
 
 
 class PsdSweepCell(C.Structure):
@@ -198,6 +199,8 @@ SIGNATURES = {
     "psd_clip_cuts_tables": (C.c_int, [_vp, _i32, _vp, _i32, _vp, _i32, _vp, _vp, _i64, _vp, _vp]),
     "psd_clip_eval_tables": (C.c_int, [_vp, _vp, _i32, _i32, _i64, _i64, _vp, _i32, _vp, _vp, _vp, _i32, _vp, _vp,
                                        _i32, _vp, _i32, _vp, C.c_size_t, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "psd_clip_union": (C.c_int, [_vp, _vp, _i32, _i32, _i64, _i64, _vp, _vp, _i32, _vp, _vp, _i64, _vp, _vp,
+                                 _vp]),
     "psd_clip_stats_csv": (C.c_int, [_vp, _i32, _vp, _vp, _vp, _i32, _i64, _vp, _vp, _i64, _vp, _vp]),
     "psd_engine_scan_content_host": (C.c_int, [_vp, _i64, _i64, _dp, _dbl, _vp, _vp]),
     "psd_engine_scan_adaptive_host": (C.c_int, [_vp, _vp, _i64, _i32, _dbl, _vp]),

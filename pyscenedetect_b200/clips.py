@@ -398,6 +398,39 @@ class _Pass:
         pc.tables, pc.cell_table = tables, cell_table
         return pc
 
+    def union(self, engine, pc: PassCuts, cell_offsets, cell_lists, max_cuts: int):
+        """Cells that are sets of `pc`'s cells: cell k's list on clip j is the sorted union of the lists (i, j) for i in
+        cell_lists[cell_offsets[k] .. cell_offsets[k + 1]) (host int32 arrays), as SceneManager.get_cut_list merges its
+        detectors' cuts.  psd_clip_union's counting call gives the exact size, its writing call fills a buffer of that
+        size.  `pc`'s lists are sorted in place and stay `pc`'s.  -> (PassCuts of the unions, sharing `pc`'s clip
+        table, -1), or (None, the lowest list * n_clips + clip of `pc` with more than max_cuts cuts)."""
+        c, n_cells = pc.n_clips, len(cell_offsets) - 1
+        m = n_cells * c
+        # offsets, their total, the overflow index, then every member list's unique length (int32)
+        obuf = DeviceBuffer((m + 2) * 8 + -(-pc.n_cells * c // 2) * 8, self.device)
+        cuts = None
+        try:
+            def call(out, cap):
+                check(self._lib.psd_clip_union(pc.cuts.ptr, pc.offsets.ptr, pc.n_cells, c, pc.total, max_cuts,
+                                               cell_offsets, cell_lists, n_cells, obuf.ptr + (m + 2) * 8, out, cap,
+                                               obuf.ptr, obuf.ptr + (m + 1) * 8, engine.compute_stream),
+                      "psd_clip_union")
+
+            call(None, 0)
+            engine.sync()
+            total, over = (int(x) for x in obuf.download(16, offset=m * 8).view(np.int64))
+            if over >= 0:
+                obuf.close()
+                return None, over
+            cuts = DeviceBuffer(max(8, total * 8), self.device)
+            call(cuts.ptr, total)
+        except BaseException:
+            obuf.close()
+            if cuts is not None:
+                cuts.close()
+            raise
+        return PassCuts(pc.clips, n_cells, pc.table, obuf, cuts, total, tables=pc.tables), -1
+
     def stats_csv(self, engine, pc: PassCuts) -> list:
         """The CSV of every clip of `pc` (header and rows), printed on the device by one psd_clip_stats_csv from the
         metric arrays `cuts` left, and brought back with one download."""

@@ -15,11 +15,15 @@
 //                    turned in place into its predicted list, every (cell, clip, tolerance) scored against clip j's
 //                    ground truth with score_predictions (sweep_eval.cuh), and the counts summed over the clips;
 //                    psd_clip_eval_tables ends each cell's lists at the end frames of the cell's clip table
+//   psd_clip_union   the cut list of a cell that is a set of detectors (SceneManager.get_cut_list over several
+//                    detectors): one thread per (list, clip) sorts psd_clip_cuts' list in place, one thread per
+//                    (cell, clip) counts the merged unique length of its member lists, an exclusive scan, then a
+//                    writing pass emits the strictly increasing union into one compact array
 //   psd_clip_stats_csv  every clip's StatsManager CSV rows (stats_csv.cuh formats them): one thread per frame counts
 //                    its row's bytes, an exclusive scan gives the row offsets, and the writing pass prints each row in
 //                    place, so one download carries every clip's text
-// Each is one launch (three for psd_clip_cuts, psd_clip_eval and psd_clip_stats_csv) per pass whatever the number of
-// cells and clips.
+// Each is one launch (three for psd_clip_cuts, psd_clip_eval and psd_clip_stats_csv, three and one for the counting and
+// the writing call of psd_clip_union) per pass whatever the number of cells and clips.
 #include <math_constants.h>
 
 #include <cstddef>
@@ -213,6 +217,74 @@ __global__ void __launch_bounds__(256) clip_totals_kernel(const int64_t* __restr
         for (int32_t j = 0; j < n_clips; ++j) s += fades[(k * n_clips + j) * 3 + (r - (int64_t)n_tol * 5)];
         totals_fades[k * 3 + (r - (int64_t)n_tol * 5)] = s;
     }
+}
+
+// One thread per (list, clip) t of psd_clip_cuts' output: the list sorted and de-duplicated in place (linear on the
+// strictly increasing lists of every automaton but a |fade_bias| > 1 ThresholdDetector), unique[t] its new length.
+// Many cells share one list, so this is the only writer of the lists.  A list longer than max_cuts is left as it is,
+// counts as empty, and the lowest such t goes to *over.
+__global__ void __launch_bounds__(128) clip_union_sort_kernel(int64_t* __restrict__ cuts,
+                                                              const int64_t* __restrict__ cut_offsets, int64_t m,
+                                                              int64_t cuts_total, int64_t max_cuts,
+                                                              int32_t* __restrict__ unique,
+                                                              unsigned long long* __restrict__ over) {
+    const int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+    if (t >= m) return;
+    int64_t b, e;
+    segment(cut_offsets, t, cuts_total, b, e);
+    if (e - b > max_cuts) {
+        unique[t] = 0;
+        atomicMin(over, (unsigned long long)t);
+        return;
+    }
+    unique[t] = sort_unique(cuts + b, (int32_t)(e - b));
+}
+
+// The first entry greater than v of the strictly increasing p[0, n), or INT64_MAX when there is none.
+__device__ __forceinline__ int64_t first_above(const int64_t* __restrict__ p, int32_t n, int64_t v) {
+    int32_t lo = 0, hi = n;
+    while (lo < hi) {
+        const int32_t mid = (lo + hi) >> 1;
+        if (p[mid] <= v) lo = mid + 1;
+        else hi = mid;
+    }
+    return lo < n ? p[lo] : INT64_MAX;
+}
+
+// One thread per (cell k, clip j), t = k * n_clips + j: the union of the lists cell_lists[cell_offsets[k] ..
+// cell_offsets[k + 1]) on clip j, walked in increasing order with no cursor array: each next value is the least
+// first_above(previous) over the member lists (a binary search in each).  Counting pass (WRITE = false):
+// out_offsets[t] = the union's length.  Writing pass: the union at out_cuts[out_offsets[t] ..], after
+// psd_clip_scan_kernel turned the lengths into offsets; nothing when the total exceeds out_cap.
+template <bool WRITE>
+__global__ void __launch_bounds__(128) clip_union_kernel(const int64_t* __restrict__ cuts,
+                                                         const int64_t* __restrict__ cut_offsets, int64_t cuts_total,
+                                                         const int32_t* __restrict__ unique, int32_t n_clips,
+                                                         const int32_t* __restrict__ cell_offsets,
+                                                         const int32_t* __restrict__ cell_lists, int32_t n_cells,
+                                                         int64_t* __restrict__ out_cuts, int64_t out_cap,
+                                                         int64_t* __restrict__ out_offsets) {
+    const int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+    const int64_t m = (int64_t)n_cells * n_clips;
+    if (t >= m) return;
+    if (WRITE && out_offsets[m] > out_cap) return;
+    const int64_t k = t / n_clips, j = t % n_clips;
+    const int32_t lb = cell_offsets[k], le = cell_offsets[k + 1];
+    int64_t* out = WRITE ? out_cuts + out_offsets[t] : nullptr;
+    int64_t n = 0, v = INT64_MIN;
+    for (;;) {
+        int64_t next = INT64_MAX;
+        for (int32_t i = lb; i < le; ++i) {
+            const int64_t l = (int64_t)cell_lists[i] * n_clips + j;
+            const int64_t b = min(max(cut_offsets[l], (int64_t)0), cuts_total);
+            next = min(next, first_above(cuts + b, unique[l], v));
+        }
+        if (next == INT64_MAX) break;
+        if (WRITE) out[n] = next;
+        ++n;
+        v = next;
+    }
+    if (!WRITE) out_offsets[t] = n;
 }
 
 // The clip that pass frame i belongs to: the last j with offsets[j] <= i (empty clips share their offset with the next
@@ -498,6 +570,65 @@ extern "C" int psd_clip_eval_tables(int64_t* cuts, const int64_t* cut_offsets, i
                      n_tables, cell_table, gt_offsets, gt_cuts, n_gt, fade_offsets, fades, n_fades, tolerances, n_tol,
                      workspace, workspace_bytes, out_n_pred, out_hard, out_fades, out_totals_hard, out_totals_fades,
                      out_over, stream);
+}
+
+extern "C" int psd_clip_union(int64_t* cuts, const int64_t* cut_offsets, int32_t n_lists, int32_t n_clips,
+                              int64_t cuts_total, int64_t max_cuts, const int32_t* cell_offsets,
+                              const int32_t* cell_lists, int32_t n_cells, int32_t* unique, int64_t* out_cuts,
+                              int64_t out_cap, int64_t* out_offsets, int64_t* out_over, void* stream) {
+    PSD_REQUIRE(n_lists >= 0 && n_clips >= 0 && n_cells >= 0 && cuts_total >= 0 && out_cap >= 0,
+                "psd_clip_union: bad args");
+    PSD_REQUIRE(max_cuts >= 0 && max_cuts <= INT32_MAX, "psd_clip_union: max_cuts must be 0 to %d", INT32_MAX);
+    PSD_REQUIRE(cell_offsets && out_offsets && out_over, "psd_clip_union: no cell table / out_offsets / out_over");
+    PSD_REQUIRE(cell_offsets[0] == 0, "psd_clip_union: cell_offsets[0] is %d, not 0", cell_offsets[0]);
+    for (int32_t k = 0; k < n_cells; ++k) {
+        const int64_t n = (int64_t)cell_offsets[k + 1] - cell_offsets[k];
+        PSD_REQUIRE(n >= 1 && n <= PSD_SWEEP_MAX_MEMBERS, "psd_clip_union: cell %d has %lld lists, not 1 to %d", k,
+                    (long long)n, PSD_SWEEP_MAX_MEMBERS);
+        PSD_REQUIRE(cell_lists, "psd_clip_union: no cell_lists");
+        for (int32_t i = cell_offsets[k]; i < cell_offsets[k + 1]; ++i)
+            PSD_REQUIRE(cell_lists[i] >= 0 && cell_lists[i] < n_lists, "psd_clip_union: cell %d names list %d of %d",
+                        k, cell_lists[i], n_lists);
+    }
+    PSD_REQUIRE(out_cuts || out_cap == 0, "psd_clip_union: no out_cuts array");
+    const int64_t m = (int64_t)n_cells * n_clips, lists = (int64_t)n_lists * n_clips;
+    PSD_REQUIRE(m == 0 || (cut_offsets && (cuts || cuts_total == 0)), "psd_clip_union: no cuts / cut_offsets");
+    PSD_REQUIRE(m == 0 || unique, "psd_clip_union: no unique workspace");
+    const bool write = out_cuts != nullptr;
+    cudaStream_t s = (cudaStream_t)stream;
+    if (!write) PSD_CUDA(cudaMemsetAsync(out_over, 0xFF, sizeof(int64_t), s));  // -1: no list longer than max_cuts
+    if (m == 0) {
+        if (!write) PSD_CUDA(cudaMemsetAsync(out_offsets, 0, sizeof(int64_t), s));
+        return PSD_OK;
+    }
+    // the cell table in one allocation (pageable: staged before return)
+    const size_t tb = sizeof(int32_t) * ((size_t)n_cells + 1 + (size_t)cell_offsets[n_cells]);
+    int32_t* d = nullptr;
+    PSD_CUDA(cudaMallocAsync((void**)&d, tb, s));
+    PSD_CUDA(cudaMemcpyAsync(d, cell_offsets, sizeof(int32_t) * ((size_t)n_cells + 1), cudaMemcpyHostToDevice, s));
+    PSD_CUDA(cudaMemcpyAsync(d + n_cells + 1, cell_lists, sizeof(int32_t) * (size_t)cell_offsets[n_cells],
+                             cudaMemcpyHostToDevice, s));
+    const int32_t* d_lists = d + n_cells + 1;
+    const unsigned blocks = (unsigned)((m + 127) / 128);
+    if (!write) {  // sort every list in place, count every union, scan the counts
+        clip_union_sort_kernel<<<(unsigned)((lists + 127) / 128), 128, 0, s>>>(cuts, cut_offsets, lists, cuts_total,
+                                                                              max_cuts, unique,
+                                                                              (unsigned long long*)out_over);
+        PSD_CHECK_LAUNCH();
+        clip_union_kernel<false><<<blocks, 128, 0, s>>>(cuts, cut_offsets, cuts_total, unique, n_clips, d, d_lists,
+                                                        n_cells, nullptr, 0, out_offsets);
+        PSD_CHECK_LAUNCH();
+        psd_clip_scan_kernel<<<1, 1024, 0, s>>>(out_offsets, m);
+        PSD_CHECK_LAUNCH();
+        count_launch(3);
+    } else {  // the unions, from what the counting call left in the lists, `unique` and out_offsets
+        clip_union_kernel<true><<<blocks, 128, 0, s>>>(cuts, cut_offsets, cuts_total, unique, n_clips, d, d_lists,
+                                                       n_cells, out_cuts, out_cap, out_offsets);
+        PSD_CHECK_LAUNCH();
+        count_launch();
+    }
+    PSD_CUDA(cudaFreeAsync(d, s));
+    return PSD_OK;
 }
 
 extern "C" int psd_clip_stats_csv(const psd_stats_column* columns, int32_t n_columns, const int64_t* clip_offsets,

@@ -28,13 +28,18 @@ Usage::
 `ParameterSweep(..., settings=[{}, {"frame_skip": 1}, {"crop": (0, 60, 1279, 659)}]).run_clips(videos, gts,
 duration="30s")` reads each clip once for every setting (fan_out.py) and evaluates every (setting, cell, clip) with
 one psd_clip_cuts_tables and one psd_clip_eval_tables per pass.
+
+`detector_sets` sweeps detectors of any classes, and SceneManagers with several detectors, instead of one class's grid:
+`ParameterSweep(detector_sets=[AdaptiveDetector(), [ContentDetector(), ThresholdDetector()], ...]).run_clips(videos,
+gts)`.  Each distinct detector configuration runs its automaton once per setting and clip, and psd_clip_union merges
+the members' cut lists into every set's list on the device before the evaluator scores it.
 """
 
 from __future__ import annotations
 
 import ctypes as C
 import time
-from dataclasses import dataclass, field
+from dataclasses import dataclass, field, replace
 
 import numpy as np
 
@@ -104,6 +109,7 @@ class CellTotals:
     hard: dict          # tolerance -> EventCounts
     hard_offset: dict   # tolerance -> (sum of |prediction - ground truth|, match count)
     fades: EventCounts
+    detectors: tuple | None = None  # the cell's detectors in a sweep over detector sets; None in a grid sweep
 
     def mean_abs_offset(self, tolerance: int) -> float:
         s, n = self.hard_offset[tolerance]
@@ -236,8 +242,9 @@ class _OneClipResult(SweepResult):
         return self._r.fades(k, 0)
 
 
-def _cell_totals(grid, tolerances, th, tf) -> list[CellTotals]:
-    """CellTotals per cell from summed counts th[cell][tolerance][5] and tf[cell][3], in grid order."""
+def _cell_totals(grid, tolerances, th, tf, sets=None) -> list[CellTotals]:
+    """CellTotals per cell from summed counts th[cell][tolerance][5] and tf[cell][3], in grid order; `sets` gives
+    every cell's detectors in a sweep over detector sets."""
     out = []
     for k, params in enumerate(grid):
         h, f = th[k], tf[k]
@@ -245,7 +252,8 @@ def _cell_totals(grid, tolerances, th, tf) -> list[CellTotals]:
             params=params,
             hard={t: EventCounts(int(h[q, 0]), int(h[q, 1]), int(h[q, 2])) for q, t in enumerate(tolerances)},
             hard_offset={t: (float(h[q, 3]), int(h[q, 4])) for q, t in enumerate(tolerances)},
-            fades=EventCounts(int(f[0]), int(f[1]), int(f[2]))))
+            fades=EventCounts(int(f[0]), int(f[1]), int(f[2])),
+            detectors=None if sets is None else sets[k]))
     return out
 
 
@@ -279,11 +287,13 @@ class ClipSweepResult:
     """Every (cell, clip) of one `ParameterSweep.run_clips` call.  Per-(cell, clip) counts and cut lists stay in
     device memory until an accessor reads them; `totals` holds this call's counts summed over its clips.  Cells are
     settings x grid, settings-major: cell k is setting k // n_grid's run of grid cell k % n_grid; `grid` holds every
-    cell's params ({**setting, **grid cell})."""
+    cell's params ({**setting, **grid cell}).  In a sweep over detector sets the grid cells are the sets: `grid` holds
+    every cell's setting and `sets` its detectors (None in a grid sweep)."""
 
     def __init__(self, grid, tolerances, passes, where, end_frames, totals_hard, totals_fades, grid_ms,
-                 n_grid: int | None = None, upload_bytes: int | None = None):
+                 n_grid: int | None = None, upload_bytes: int | None = None, sets=None):
         self.grid = grid
+        self.sets = sets
         self.tolerances = tuple(tolerances)
         self._passes = passes        # [_ClipPass]
         self._where = where          # clip -> (pass index, index within the pass)
@@ -334,7 +344,8 @@ class ClipSweepResult:
         return got + [self._end[k // self._n_grid][j]]
 
     def raw_count(self, k: int, j: int) -> int:
-        """How many cuts cell k's automaton emitted on clip j (before de-duplication)."""
+        """How many cuts cell k's automaton emitted on clip j (before de-duplication); for a set of detectors, the
+        length of the union of their cuts."""
         ps, t = self._at(k, j)
         o = ps.host("offsets")
         return int(o[t + 1] - o[t])
@@ -358,7 +369,7 @@ class ClipSweepResult:
 
     def totals(self) -> list[CellTotals]:
         """Every cell's counts summed over this call's clips, in grid order."""
-        return _cell_totals(self.grid, self.tolerances, self._th, self._tf)
+        return _cell_totals(self.grid, self.tolerances, self._th, self._tf, self.sets)
 
 
 SETTING_KEYS = ("auto_downscale", "downscale", "crop", "frame_skip")
@@ -386,6 +397,37 @@ def _setting_geometry(setting: dict, device: int, batch_size: int) -> SceneManag
     return sm
 
 
+def _detector_set(x) -> tuple:
+    """One element of `detector_sets` -> its detectors: one of this package's detectors, or a non-empty list of them,
+    configuration only (no stats_manager), as detect_clips takes them."""
+    dets = (x,) if isinstance(x, EngineDetector) else tuple(x) if isinstance(x, (list, tuple)) else None
+    if dets is None:
+        raise TypeError(f"a detector set is a detector or a list of detectors, not {type(x).__name__}")
+    if not dets:
+        raise ValueError("a detector set is empty")
+    for d in dets:
+        if not isinstance(d, EngineDetector):
+            raise TypeError("ParameterSweep sweeps the detectors of this package")
+        if d.stats_manager is not None:
+            raise ValueError("a sweep produces no per-frame metrics: detectors must not have a stats_manager")
+    return dets
+
+
+def _length_key(length) -> tuple:
+    """A min_scene_len as a key that keeps its meaning: the type decides the unit (an int counts frames, a float is
+    seconds, a string either), so 2 and 2.0 are different lengths although they compare equal; a timecode is its frame
+    number at its own rate."""
+    if hasattr(length, "frame_num") and hasattr(length, "framerate"):
+        return ("timecode", int(length.frame_num), float(length.framerate))
+    return (type(length).__qualname__, length)
+
+
+def _describe(detector) -> str:
+    """A detector by class and the parameters its automaton runs with."""
+    _, a = automaton_args(detector)
+    return f"{type(detector).__name__}({', '.join(f'{k}={v!r}' for k, v in a.items())})"
+
+
 class ParameterSweep:
     """Every cell of `grid` (a list of `detector_cls(**params)` keyword dicts, as the reference harness takes
     them) over each video `run` is given.  `detector_cls` is one of this package's detectors; each cell is
@@ -395,22 +437,46 @@ class ParameterSweep:
     `settings` sweeps how the frames are read and scored as well: a list of dicts with the keys `auto_downscale`,
     `downscale`, `crop` (SceneManager's properties) and `frame_skip` (detect_scenes'), each checked as those check
     it.  The cells are settings x grid, settings-major (cell s * len(grid) + g, params {**settings[s], **grid[g]}).
-    None means [{}]: one setting, SceneManager's defaults, and the cells of the grid alone."""
+    None means [{}]: one setting, SceneManager's defaults, and the cells of the grid alone.
 
-    def __init__(self, detector_cls, grid, tolerances=(0, 1), device: int = 0, batch_size: int = 64,
-                 max_cuts_per_cell: int = 4096, settings=None):
-        if not (isinstance(detector_cls, type) and issubclass(detector_cls, EngineDetector)):
-            raise TypeError("ParameterSweep sweeps the detectors of this package")
-        self.grid = [dict(p) for p in grid]
-        if not self.grid:
-            raise ValueError("the grid has no cells")
+    `detector_sets` (keyword-only, instead of `detector_cls` and `grid`) sweeps detectors of any classes and their
+    combinations: each element is one detector or a non-empty list of detectors, configuration only as `detect_clips`
+    takes them, and stands for a SceneManager with those detectors, whose cut list is the sorted union of theirs.  The
+    cells are settings x sets, settings-major (cell s * len(detector_sets) + k): `params[cell]` is the setting and
+    `sets[cell]` the detectors.  Every distinct detector configuration (a member) runs its automaton once per setting
+    and clip, however many sets hold it, and one psd_clip_union per pass merges the members' cuts into every set's
+    list.  A set holds at most `_capi.SWEEP_MAX_MEMBERS` distinct configurations."""
+
+    def __init__(self, detector_cls=None, grid=None, tolerances=(0, 1), device: int = 0, batch_size: int = 64,
+                 max_cuts_per_cell: int = 4096, settings=None, *, detector_sets=None):
+        if detector_sets is not None:
+            if detector_cls is not None or grid is not None:
+                raise TypeError("ParameterSweep takes detector_cls and grid, or detector_sets, not both")
+            self.detector_sets = [_detector_set(x) for x in detector_sets]
+            if not self.detector_sets:
+                raise ValueError("detector_sets is empty")
+            self.grid = None
+        elif detector_cls is None and grid is None:
+            raise TypeError("ParameterSweep needs detector_cls and grid, or detector_sets")
+        else:
+            if not (isinstance(detector_cls, type) and issubclass(detector_cls, EngineDetector)):
+                raise TypeError("ParameterSweep sweeps the detectors of this package")
+            self.grid = [dict(p) for p in grid]
+            if not self.grid:
+                raise ValueError("the grid has no cells")
+            self.detector_sets = None
         self.settings = [{}] if settings is None else [dict(x) for x in settings]
         if not self.settings:
             raise ValueError("settings is empty (None means one setting with SceneManager's defaults)")
         self._geometries = [_setting_geometry(x, int(device), int(batch_size)) for x in self.settings]
         self._frame_skips = [int(x.get("frame_skip", 0)) for x in self.settings]
         self._default_settings = self.settings == [{}]
-        self.params = [{**x, **g} for x in self.settings for g in self.grid]
+        if self.grid is not None:
+            self.params = [{**x, **g} for x in self.settings for g in self.grid]
+            self.sets = None
+        else:
+            self.params = [dict(x) for x in self.settings for _ in self.detector_sets]
+            self.sets = [d for _ in self.settings for d in self.detector_sets]
         tols = tuple(int(t) for t in tolerances)
         if not 1 <= len(tols) <= _capi.SWEEP_MAX_TOLERANCES or any(t < 0 for t in tols) or len(set(tols)) != len(tols):
             raise ValueError(f"tolerances must be 1 to {_capi.SWEEP_MAX_TOLERANCES} distinct non-negative frame counts")
@@ -420,16 +486,39 @@ class ParameterSweep:
         self.device = int(device)
         self.batch_size = int(batch_size)
         self.cap = int(max_cuts_per_cell)
-        detectors = [detector_cls(**p) for p in self.grid]
         self.groups: list[PixelGroup] = []
         group_index: dict = {}
         self.cells: list[CellPlan] = []
-        for d in detectors:
+
+        def plan(d) -> CellPlan:
             g = pixel_group_of(d)
             gi = group_index.setdefault(g, len(self.groups))
             if gi == len(self.groups):
                 self.groups.append(g)
-            self.cells.append(plan_cell(d, gi))
+            return plan_cell(d, gi)
+
+        if self.grid is not None:
+            self.cells = [plan(detector_cls(**p)) for p in self.grid]
+        else:
+            # the cells are the members: one automaton per distinct (CellPlan, pixel group); a set names its members
+            member_index: dict = {}
+            self._member_detectors = []
+            self._set_members = []
+            for dets in self.detector_sets:
+                own = []
+                for d in dets:
+                    c = plan(d)
+                    key = replace(c, min_scene_len=_length_key(c.min_scene_len))
+                    if key not in member_index:
+                        member_index[key] = len(self.cells)
+                        self.cells.append(c)
+                        self._member_detectors.append(d)
+                    if member_index[key] not in own:
+                        own.append(member_index[key])
+                if len(own) > _capi.SWEEP_MAX_MEMBERS:
+                    raise ValueError(f"a detector set holds {len(own)} distinct detectors, more than "
+                                     f"{_capi.SWEEP_MAX_MEMBERS}")
+                self._set_members.append(own)
         # metric keys in order of first use; cells sorted by the key they read (stable), so that the 32
         # cells of a warp share one metric array except where one key's run of cells ends inside the warp
         self.metric_keys: list[tuple] = []
@@ -457,8 +546,8 @@ class ParameterSweep:
 
         With settings other than the default, or a window (`duration` / `end_time`, as detect_scenes takes them),
         the video goes through `run_clips` as its one clip: cell k's results are run_clips' (k, 0), `end_frames`
-        holds every setting's end frame and `end_frame` setting 0's."""
-        if not self._default_settings or duration is not None or end_time is not None:
+        holds every setting's end frame and `end_frame` setting 0's.  So does a sweep over detector sets."""
+        if self.sets is not None or not self._default_settings or duration is not None or end_time is not None:
             gts = None if ground_truth is None else [ground_truth]
             return _OneClipResult(self._run_clips([video], gts, duration, end_time, "the video"))
         fw, fh = video.frame_size
@@ -494,6 +583,8 @@ class ParameterSweep:
         `self.groups[i]`'s results for the same frames, the first of which is frame `first_frame` - an Engine
         per group, or the group's view (`Engine.view`) of one engine that holds every group's slots.
         `end_frame` defaults to first_frame + frame count."""
+        if self.sets is not None:
+            raise TypeError("run_scored evaluates a grid; a sweep over detector sets runs through run or run_clips")
         if len(engines) != len(self.groups):
             raise ValueError(f"{len(self.groups)} pixel groups need as many engines, got {len(engines)}")
         lib = self._lib = self._lib or _capi.load()
@@ -610,8 +701,19 @@ class ParameterSweep:
                         raise ValueError(f"crop starts outside video boundary of clip {i} ({fw}x{fh}) in setting {s} "
                                          f"({self.settings[s]})")
         lib = self._lib = self._lib or _capi.load()
-        n_grid, n_set, n_tol, dev = len(self.cells), len(self.settings), len(self.tolerances), self.device
-        n_cells = n_set * n_grid
+        n_set, n_tol, dev = len(self.settings), len(self.tolerances), self.device
+        n_cells = len(self.params)
+        n_grid = n_cells // n_set
+        max_cuts = self.cap
+        if self.sets is not None:
+            # the set-cells over the member lists of psd_clip_cuts(_tables): list s * members + i is member i under
+            # setting s; a union of members that each keep within the cap keeps within cap x its member count
+            n_mem = len(self.cells)
+            lists = [[s * n_mem + i for i in own] for s in range(n_set) for own in self._set_members]
+            set_table = ((C.c_int32 * (n_cells + 1))(*np.concatenate([[0], np.cumsum([len(x) for x in lists])])),
+                         (C.c_int32 * sum(len(x) for x in lists))(*[i for x in lists for i in x]))
+            set_of_cell = (C.c_int32 * n_cells)(*[k // n_grid for k in range(n_cells)])
+            max_cuts = min(self.cap * max(len(x) for x in self._set_members), 2 ** 31 - 1)
         tols = (C.c_int32 * n_tol)(*self.tolerances)
         th = np.zeros((n_cells, n_tol, 5), dtype=np.int64)
         tf = np.zeros((n_cells, 3), dtype=np.int64)
@@ -641,6 +743,18 @@ class ParameterSweep:
                                                                    for s in range(n_set)], steps)
                     engine = engine[0]
                 indices = [index for index, _rs, _ms in done]
+                members = None
+                if self.sets is not None:
+                    members = pc
+                    try:
+                        pc, over = device_pass.union(engine, members, *set_table, self.cap)
+                    except BaseException:
+                        members.close()
+                        raise
+                    if over >= 0:
+                        self._member_overflow(members, over, indices)
+                    if pc.tables is not None:
+                        pc.cell_table = set_of_cell
                 c = pc.n_clips
                 ggt = [gts[i] for i in indices]
                 gt_off = np.concatenate([[0], np.cumsum([len(g.hard_cuts) for g in ggt])]).astype(np.int64)
@@ -663,23 +777,27 @@ class ParameterSweep:
                              sums.ptr + n_cells * n_tol * 40, sums.ptr + n_cells * (n_tol * 5 + 3) * 8,
                              engine.compute_stream)
                     if pc.tables is None:
-                        check(lib.psd_clip_eval(pc.cuts.ptr, pc.offsets.ptr, n_cells, c, pc.total, self.cap,
+                        check(lib.psd_clip_eval(pc.cuts.ptr, pc.offsets.ptr, n_cells, c, pc.total, max_cuts,
                                                 pc.end_frames, *truth), "psd_clip_eval")
                     else:
-                        check(lib.psd_clip_eval_tables(pc.cuts.ptr, pc.offsets.ptr, n_cells, c, pc.total, self.cap,
+                        check(lib.psd_clip_eval_tables(pc.cuts.ptr, pc.offsets.ptr, n_cells, c, pc.total, max_cuts,
                                                        pc.tables, n_set, pc.cell_table, *truth), "psd_clip_eval_tables")
                     engine.sync()
                     grid_ms += (time.perf_counter() - t0) * 1e3
                     got = sums.download(sums.nbytes).view(np.int64)
                 finally:
-                    for b in (gbuf, ws, sums, pc.table):
+                    done_with = (gbuf, ws, sums, pc.table)
+                    if members is not None:  # the member lists the unions were merged from
+                        done_with += (members.offsets, members.cuts)
+                    for b in done_with:
                         b.close()
                 over = int(got[-1])
                 if over >= 0:
                     k, jj = divmod(over, c)
                     o = pc.offsets.download(16, offset=over * 8).view(np.int64)
-                    where_k = f"({self.grid[k]})" if self._default_settings else \
-                        f"({self.grid[k % n_grid]}) of setting {k // n_grid} ({self.settings[k // n_grid]})"
+                    what = self.grid[k % n_grid] if self.sets is None else list(self.sets[k])
+                    where_k = f"({what})" if self._default_settings else \
+                        f"({what}) of setting {k // n_grid} ({self.settings[k // n_grid]})"
                     raise RuntimeError(f"cell {k} {where_k} found {int(o[1] - o[0])} cuts in clip "
                                        f"{indices[jj]}, more than max_cuts_per_cell={self.cap}")
                 th += got[:n_cells * n_tol * 5].reshape(n_cells, n_tol, 5)
@@ -697,11 +815,24 @@ class ParameterSweep:
             self._totals_fades += tf
             self.videos += len(videos)
         return ClipSweepResult(self.params, self.tolerances, passes, where, ends, th, tf, grid_ms, n_grid=n_grid,
-                               upload_bytes=None if self._default_settings else counters.get("uploaded", 0))
+                               upload_bytes=None if self._default_settings else counters.get("uploaded", 0),
+                               sets=self.sets)
+
+    def _member_overflow(self, members, over: int, indices) -> None:
+        """Raise for member list `over` of a pass (list * n_clips + clip of psd_clip_cuts' output), which has more than
+        max_cuts_per_cell cuts; releases the pass's member lists and clip table."""
+        try:
+            o = members.offsets.download(16, offset=over * 8).view(np.int64)
+        finally:
+            members.close()
+        i, jj = divmod(over, members.n_clips)
+        s, m = divmod(i, len(self.cells))
+        raise RuntimeError(f"detector {_describe(self._member_detectors[m])} of setting {s} ({self.settings[s]}) found "
+                           f"{int(o[1] - o[0])} cuts in clip {indices[jj]}, more than max_cuts_per_cell={self.cap}")
 
     def totals(self) -> list[CellTotals]:
         """Every cell's counts summed over the videos and clips run with ground truth so far, in grid order."""
-        return _cell_totals(self.params, self.tolerances, self._totals_hard, self._totals_fades)
+        return _cell_totals(self.params, self.tolerances, self._totals_hard, self._totals_fades, self.sets)
 
 
 __all__ = ["ParameterSweep", "SweepResult", "ClipSweepResult", "GroundTruth", "EventCounts", "CellTotals",
