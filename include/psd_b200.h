@@ -412,6 +412,26 @@ int psd_clip_stats_csv(const psd_stats_column* columns, int32_t n_columns, const
                        const int64_t* clip_first_frame, const double* clip_rate, int32_t n_clips, int64_t n,
                        int64_t* row_offsets, char* out, int64_t out_cap, int64_t* clip_bytes, void* stream);
 
+/* ---- JPEG scene images: scenedetect/output/image.py:317-319, cv2.imencode(".jpg", frame, [IMWRITE_JPEG_QUALITY, q])
+ *      for every selected frame ---- */
+/* One image: width x height pixels of 8-bit B, G, R at `base` in `layout` (frame_stride is not read). */
+typedef struct psd_jpeg_image {
+    const void* base; /* DEVICE (or managed) memory: channel B of pixel (0, 0) */
+    psd_frame_layout layout;
+    int32_t width, height; /* 1 to 65535 each */
+} psd_jpeg_image;
+/* The baseline JPEG file cv2.imencode writes for each image, byte for byte (libjpeg-turbo: jpeg_set_quality(quality,
+ * force_baseline) after cv2's clamp of quality to [0, 100], JFIF 1.01, 4:2:0, the T.81 Annex K Huffman tables, no
+ * restart interval).  images[n] is a HOST array; out, image_bytes[n + 1] are DEVICE memory.  out receives image 0's
+ * file, then image 1's, ...; image_bytes their exclusive byte offsets and the total.  A file that would end past
+ * out_cap is not written (the files are written in order, so those that are form a prefix): when image_bytes[n]
+ * exceeds out_cap, grow out and call again.  The images are encoded in sub-batches whose workspace (allocated on
+ * `stream`) stays within workspace_cap bytes (0: 512 MiB), each at least one image: about 65 350 bytes per tile of 32
+ * MCUs of 16x16 pixels, i.e. about 510 bytes per 8x8 luma block (a 1920x1080 image is 255 tiles, 16.7 MB); eight
+ * launches per sub-batch, queued on `stream` (a cudaStream_t or NULL), not waited for. */
+int psd_jpeg_encode(int device, const psd_jpeg_image* images, int32_t n, int32_t quality, int64_t workspace_cap,
+                    uint8_t* out, int64_t out_cap, int64_t* image_bytes, void* stream);
+
 /* host-convenience wrappers: engine-owned sums -> host arrays (numpy), implies sync */
 int psd_engine_scan_content_host(psd_engine* e, int64_t first, int64_t n, const double weights[4],
                                  double weight_abs_sum, double* out_components,

@@ -119,6 +119,19 @@ class PsdStatsColumn(C.Structure):
 assert C.sizeof(PsdStatsColumn) == 24
 
 
+class PsdJpegImage(C.Structure):
+    """psd_jpeg_image: one image of psd_jpeg_encode (48 bytes)."""
+    _fields_ = [
+        ("base", C.c_void_p),
+        ("layout", PsdFrameLayout),
+        ("width", C.c_int32),
+        ("height", C.c_int32),
+    ]
+
+
+assert C.sizeof(PsdJpegImage) == 48
+
+
 # numpy view of psd_frame_sums (64 bytes)
 SUMS_DTYPE = np.dtype([
     ("sad_hue", "<u8"), ("sad_sat", "<u8"), ("sad_lum", "<u8"), ("sad_edges", "<u8"),
@@ -202,6 +215,7 @@ SIGNATURES = {
     "psd_clip_union": (C.c_int, [_vp, _vp, _i32, _i32, _i64, _i64, _vp, _vp, _i32, _vp, _vp, _i64, _vp, _vp,
                                  _vp]),
     "psd_clip_stats_csv": (C.c_int, [_vp, _i32, _vp, _vp, _vp, _i32, _i64, _vp, _vp, _i64, _vp, _vp]),
+    "psd_jpeg_encode": (C.c_int, [C.c_int, C.POINTER(PsdJpegImage), _i32, _i32, _i64, _vp, _i64, _vp, _vp]),
     "psd_engine_scan_content_host": (C.c_int, [_vp, _i64, _i64, _dp, _dbl, _vp, _vp]),
     "psd_engine_scan_adaptive_host": (C.c_int, [_vp, _vp, _i64, _i32, _dbl, _vp]),
     "psd_engine_scan_average_host": (C.c_int, [_vp, _i64, _i64, _vp]),

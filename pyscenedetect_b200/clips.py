@@ -598,4 +598,6 @@ def clip_passes(videos, groups, geometry, batch_size: int, device: int, frame_sk
             engine.close()
 
 
-__all__ = ["detect_clips", "ClipResult", "MAX_PASS_FRAMES"]
+from .images import save_clip_images, save_images  # noqa: E402  (images of the scenes detect_clips finds)
+
+__all__ = ["detect_clips", "ClipResult", "MAX_PASS_FRAMES", "save_images", "save_clip_images"]

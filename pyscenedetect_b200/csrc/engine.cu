@@ -43,6 +43,20 @@ static void build_taps(int src, int dst, std::vector<int32_t>& ofs, std::vector<
     }
 }
 
+// PSD_OK if p is device or managed memory of `device`
+int require_device_memory(const void* p, int device, const char* what) {
+    cudaPointerAttributes at{};
+    if (cudaPointerGetAttributes(&at, p) != cudaSuccess) {
+        cudaGetLastError();
+        set_error("%s: %p is not CUDA memory", what, p);
+        return PSD_ERR_INVALID;
+    }
+    PSD_REQUIRE(at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged,
+                "%s: %p is not device or managed memory", what, p);
+    PSD_REQUIRE(at.device == device, "%s: %p is memory of device %d, not of device %d", what, p, at.device, device);
+    return PSD_OK;
+}
+
 }  // namespace psd
 
 using namespace psd;
@@ -525,20 +539,6 @@ int psd_engine_set_halo_host(psd_engine* e, const uint8_t* bgr, int64_t row_pitc
     rc = psd_engine_set_halo_device(e, e->dev_stage[slot]);
     if (rc) return rc;
     PSD_CUDA(cudaEventRecord(e->slot_free[slot], e->compute_stream));
-    return PSD_OK;
-}
-
-// PSD_OK if p is device or managed memory of `device`
-static int require_device_memory(const void* p, int device, const char* what) {
-    cudaPointerAttributes at{};
-    if (cudaPointerGetAttributes(&at, p) != cudaSuccess) {
-        cudaGetLastError();
-        set_error("%s: %p is not CUDA memory", what, p);
-        return PSD_ERR_INVALID;
-    }
-    PSD_REQUIRE(at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged,
-                "%s: %p is not device or managed memory", what, p);
-    PSD_REQUIRE(at.device == device, "%s: %p is memory of device %d, not of device %d", what, p, at.device, device);
     return PSD_OK;
 }
 

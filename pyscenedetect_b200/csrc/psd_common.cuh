@@ -45,6 +45,9 @@ inline void count_launch(uint64_t n = 1) { g_launches.fetch_add(n, std::memory_o
         }                                                                                        \
     } while (0)
 
+// PSD_OK if p is device or managed memory of `device`, else PSD_ERR_INVALID with a message prefixed by `what`
+int require_device_memory(const void* p, int device, const char* what);
+
 // ---- fused score pass (score_kernel.cu) ----
 struct ScoreArgs {
     const uint8_t* frames;   // n frames, frame_stride apart, tightly packed rows (3*W bytes); 16-byte aligned
@@ -157,6 +160,10 @@ int launch_hash_dist(const uint64_t* hashes, int64_t n, int size, const uint64_t
 // ---- cut automata over grid cells (sweep_kernels.cu) ----
 // the host-side checks of psd_sweep_cuts on an array of cells; `who` prefixes the error message
 int validate_sweep_cells(const psd_sweep_cell* cells, int32_t n_cells, const char* who);
+
+// ---- clip tables (clip_kernels.cu) ----
+// In place: v[0, m) counts -> exclusive offsets, v[m] = their sum (one block of 1024 threads)
+__global__ void __launch_bounds__(1024) psd_clip_scan_kernel(int64_t* __restrict__ v, int64_t m);
 
 // ---- synthetic generator (synth_kernel.cu) ----
 int launch_synth(uint8_t* out, const int32_t* d_params, int64_t n, int width, int height,
