@@ -320,6 +320,20 @@ int psd_clip_cuts_step(const psd_sweep_cell* cells, int32_t n_cells, const int64
                        const int64_t* clip_first_frame, int32_t n_clips, const int64_t* min_frames, int64_t* cuts,
                        int64_t cuts_cap, int64_t* cut_offsets, int64_t frame_step, const int64_t* clip_end_frame,
                        void* stream);
+/* psd_clip_cuts_step for clips read with different frame skips, each clip through its own window of
+ * SceneManager.detect_scenes(frame_skip = frame_step[j] - 1) (scene_manager.py:682-685): element i of clip j's slice
+ * is frame clip_first_frame[j] + i * frame_step[j], and the automata compare those true frame numbers with
+ * min_frames as psd_clip_cuts_step's do (detector.py:160-224, adaptive_detector.py:134-143,
+ * histogram_detector.py:87-112, hash_detector.py:79-109, threshold_detector.py:113-168).  post_process
+ * (threshold_detector.py:170-191) gets clip_end_frame[j] - 1, the stream's position after the loop
+ * (scene_manager.py:618-621), or the last processed frame when clip_end_frame is NULL.  frame_step is a HOST
+ * int64[n_clips], every entry >= 1 (validated, then copied on `stream` with the cells); the other arrays are as
+ * psd_clip_cuts_step's.  With every frame_step[j] equal to s it gives psd_clip_cuts_step(frame_step = s)'s results
+ * bit for bit.  Same kernels and launches as psd_clip_cuts. */
+int psd_clip_cuts_steps(const psd_sweep_cell* cells, int32_t n_cells, const int64_t* clip_offsets,
+                        const int64_t* clip_first_frame, int32_t n_clips, const int64_t* min_frames, int64_t* cuts,
+                        int64_t cuts_cap, int64_t* cut_offsets, const int64_t* frame_step,
+                        const int64_t* clip_end_frame, void* stream);
 /* benchmark/evaluator.py:227-331 (score_video) for every (cell, clip, tolerance) on psd_clip_cuts' output, and the
  * counts summed over the clips (evaluator.py:167-186).  cuts / cut_offsets are psd_clip_cuts' arrays and cuts_total
  * its total cut_offsets[n_cells * n_clips]; each (cell, clip) list is first turned, in place, into the predicted list

@@ -207,6 +207,7 @@ SIGNATURES = {
     "psd_clip_fill": (C.c_int, [_vp, _i64, _vp, _i32, _i32, _i32, _i32, _dbl, _vp]),
     "psd_clip_cuts": (C.c_int, [_vp, _i32, _vp, _vp, _i32, _vp, _vp, _i64, _vp, _vp]),
     "psd_clip_cuts_step": (C.c_int, [_vp, _i32, _vp, _vp, _i32, _vp, _vp, _i64, _vp, _i64, _vp, _vp]),
+    "psd_clip_cuts_steps": (C.c_int, [_vp, _i32, _vp, _vp, _i32, _vp, _vp, _i64, _vp, _vp, _vp, _vp]),
     "psd_clip_eval": (C.c_int, [_vp, _vp, _i32, _i32, _i64, _i64, _vp, _vp, _vp, _i32, _vp, _vp, _i32, _vp, _i32, _vp,
                                 C.c_size_t, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "psd_clip_cuts_tables": (C.c_int, [_vp, _i32, _vp, _i32, _vp, _i32, _vp, _vp, _i64, _vp, _vp]),

@@ -7,7 +7,9 @@ a new engine (device allocations, result arrays that grow through synchronising 
 state machines, and a device teardown.  `detect_clips` instead:
 
 * groups the clips by (frame size, host or CUDA, channel order) and builds one engine per group through
-  `shared_engine`, with every detector's edge and hash slots, exactly as SceneManager does for one video;
+  `shared_engine`, with every detector's edge and hash slots, exactly as SceneManager does for one video (with
+  `windows`, by cropped and scored size instead of frame size: clips of any source size cropped to one size share an
+  engine);
 * scores a group's clips back to back into that engine.  The fused pass scores a frame from that frame and its
   predecessor only, so every integer result is the clip's own except at the clip edges;
 * finishes a pass with one psd_scan_* per distinct metric array, each followed by psd_clip_fill, which gives every
@@ -26,7 +28,8 @@ and fresh detectors, running `detect_scenes(video, duration=, end_time=, frame_s
 lists and frame count.  Frame numbers are clip-local, frame-number timecodes at the clip's constant frame rate (as
 `DeviceCuts` gives them).  Each clip is read through its own `StreamWindow`, the one detect_scenes reads a stream
 through; with a frame skip, element i of a clip's metric slice is frame first + i * (frame_skip + 1), which
-psd_clip_cuts_step's automata walk.
+psd_clip_cuts_step's automata walk.  With `windows` every clip has its own crop, duration / end_time and frame_skip;
+a pass whose clips step differently runs psd_clip_cuts_steps, which takes one step per clip, in the same one launch.
 
 With `stats=True` each clip also gets the text a `StatsManager` attached to that SceneManager saves
 (`save_to_csv`): the metric arrays the cuts are made from are already on the device, so psd_clip_stats_csv prints
@@ -58,6 +61,20 @@ from .sweep import _KIND, plan_cell
 MAX_PASS_FRAMES = 1 << 16     # frames an engine holds before its pass is finished at the next clip boundary
 FIRST_CUTS_PER_FRAME = 0.25   # first cut buffer of a pass, in cuts per frame held; grown once if the cuts need more
 FIRST_STATS_BYTES = (32, 24)  # first CSV text buffer, in bytes per frame held: a + b * columns; grown once if short
+WINDOW_KEYS = ("crop", "duration", "end_time", "frame_skip")  # what an entry of detect_clips(windows=) may set
+
+
+@dataclass(frozen=True)
+class _ClipWindow:
+    """How one clip is read: its crop `box` (x0, y0, x1, y1) of cropped `size` (w, h), scored at `scored` (sw, sh), as
+    `SceneManager._geometry` gives them under the clip's crop; and its detect_scenes window."""
+
+    box: tuple
+    size: tuple
+    scored: tuple
+    frame_skip: int = 0
+    duration: object = None
+    end_time: object = None
 
 
 @dataclass
@@ -85,16 +102,15 @@ class ClipResult:
 
 class _ClipChain:
     """A group's streams read one after the other as one stream, for `FrameBatches`: `read()` gives the next frame to
-    process of the current clip's `StreamWindow` (with `frame_skip` and the clip's own end frame of `duration` /
+    process of the current clip's `StreamWindow` (with the clip's `frame_skip` and its own end frame of `duration` /
     `end_time`, as detect_scenes reads one stream) and moves on to the next clip when that window ends, recording each
-    clip's positions and frame count.  At a clip boundary, once the pass holds `bound` frames, it reports an end
-    (`paused`) until `resume()`."""
+    clip's positions and frame count; `box()` is the crop box of the clip the last frame came from.  At a clip
+    boundary, once the pass holds `bound` frames, it reports an end (`paused`) until `resume()`."""
 
-    def __init__(self, clips, bound: int, on_cuda: bool, frame_skip: int = 0, duration=None, end_time=None):
-        self._clips = clips       # [(input index, stream)]
+    def __init__(self, clips, bound: int, on_cuda: bool):
+        self._clips = clips       # [(input index, stream, _ClipWindow)]
         self._k = -1
         self._on_cuda = on_cuda
-        self._frame_skip, self._duration, self._end_time = frame_skip, duration, end_time
         self.bound = bound
         self.paused = False
         self.held = 0             # frames processed in this pass
@@ -110,16 +126,19 @@ class _ClipChain:
     def _next(self):
         self._k += 1
         if self._k < len(self._clips):
-            video = self._clips[self._k][1]
+            _, video, w = self._clips[self._k]
             self._start_num = video.frame_number
             self._result = ClipResult(fps=video.frame_rate)
             self._scored = 0
-            end = window_end_frame(base_timecode_of(video), self._start_num, self._duration, self._end_time)
-            self._window = StreamWindow(video, self._frame_skip, end)
+            end = window_end_frame(base_timecode_of(video), self._start_num, w.duration, w.end_time)
+            self._window = StreamWindow(video, w.frame_skip, end)
+
+    def box(self) -> tuple:
+        return self._clips[min(self._k, len(self._clips) - 1)][2].box
 
     def _end_clip(self) -> None:
         """Close the current clip; pause if the pass holds enough frames and another clip follows."""
-        index, video = self._clips[self._k]
+        index, video, _ = self._clips[self._k]
         r = self._result
         r.frames = video.frame_number - self._start_num
         if r.start is not None:
@@ -216,7 +235,7 @@ class _Pass:
                 if key is not None and key not in self.keys:
                     self.keys.append(key)
         self._bufs = {}
-        self.frame_step = 1         # frame_skip + 1 of the clips' windows: element i of a clip is frame first + i * step
+        self.frame_step = 1         # frame_skip + 1 of the clips' windows (`cuts` without per-clip steps)
         self.columns = None         # stats: [(CSV key, metric key, component or None, head, tail)] in CSV order
         self.components_key = None  # stats: the content_val key whose scan also writes the four components
         self.header = b""
@@ -321,11 +340,14 @@ class _Pass:
             cap = cuts.nbytes // 8
         return obuf, cuts, total
 
-    def cuts(self, engine, holders, clips: list) -> PassCuts | None:
+    def cuts(self, engine, holders, clips: list, steps: list | None = None) -> PassCuts | None:
         """Every (cell, clip) cut list of `clips` ((ClipResult, frames scored) of the frames `engine` holds, in
-        order), left in device memory; None when no clip has a frame.  Only the cut total comes back to the host."""
+        order), left in device memory; None when no clip has a frame.  Element i of clip j is frame start + i *
+        steps[j] (`frame_step` for every clip when `steps` is None).  Only the cut total comes back to the host."""
         lib = self._lib
         scored = [r for r, m in clips if m]
+        steps = [self.frame_step] * len(clips) if steps is None else list(steps)
+        steps = [s for s, (_, m) in zip(steps, clips) if m]
         n = engine.frame_count
         if not scored:
             return None
@@ -344,12 +366,18 @@ class _Pass:
         cells = self._cells([self._scan(holders, offsets, c, n)])
         st = engine.compute_stream
 
+        step = steps[0] if len(set(steps)) == 1 else None
+        per_clip = (C.c_int64 * c)(*steps) if step is None else None
+
         def launch(cuts, cap, obuf):
-            if self.frame_step == 1:
+            if step == 1:
                 check(lib.psd_clip_cuts(cells, k, offsets, first, c, min_frames, cuts, cap, obuf, st), "psd_clip_cuts")
-            else:  # post_process sees each clip's end position, past its last processed frame after skipped reads
-                check(lib.psd_clip_cuts_step(cells, k, offsets, first, c, min_frames, cuts, cap, obuf,
-                                             self.frame_step, first + c * 8, st), "psd_clip_cuts_step")
+            elif step is not None:  # post_process sees each clip's end position, past its last processed frame
+                check(lib.psd_clip_cuts_step(cells, k, offsets, first, c, min_frames, cuts, cap, obuf, step,
+                                             first + c * 8, st), "psd_clip_cuts_step")
+            else:                   # clips read with different frame skips: each clip's own step
+                check(lib.psd_clip_cuts_steps(cells, k, offsets, first, c, min_frames, cuts, cap, obuf, per_clip,
+                                              first + c * 8, st), "psd_clip_cuts_steps")
 
         obuf, cuts, total = self._cut_lists(engine, k * c, n, launch, "psd_clip_cuts")
         return PassCuts(scored, k, tbuf, obuf, cuts, total)
@@ -465,14 +493,15 @@ class _Pass:
             cbuf.close()
         return [self.header + data[offs[j]:offs[j + 1]] for j in range(c)]
 
-    def finish(self, engine, holders, clips: list) -> None:
-        """Every clip of `clips` ((ClipResult, frames scored) of the frames `engine` holds, in order) gets its cut
-        frames: the union of every cell's cuts, as SceneManager.get_cut_list gives them; and with a stats plan its
-        CSV (the header alone for a clip without frames)."""
+    def finish(self, engine, holders, clips: list, steps: list | None = None) -> None:
+        """Every clip of `clips` ((ClipResult, frames scored) of the frames `engine` holds, in order, each read with
+        its step of `steps`, as `cuts` takes them) gets its cut frames: the union of every cell's cuts, as
+        SceneManager.get_cut_list gives them; and with a stats plan its CSV (the header alone for a clip without
+        frames)."""
         for r, _ in clips:
             if self.columns is not None:
                 r.stats_csv = self.header
-        pc = self.cuts(engine, holders, clips)
+        pc = self.cuts(engine, holders, clips, steps)
         if pc is None:
             return
         try:
@@ -497,7 +526,7 @@ def _group_key(video) -> tuple:
 
 def detect_clips(videos, detectors, auto_downscale: bool = True, downscale: int = 1, device: int = 0,
                  batch_size: int = 64, stats: bool = False, crop=None, duration=None, end_time=None,
-                 frame_skip: int = 0) -> list[ClipResult]:
+                 frame_skip: int = 0, *, windows=None) -> list[ClipResult]:
     """Detect scenes in every stream of `videos` with every detector of `detectors`: for each clip, in input order,
     what a fresh `SceneManager(device=device, batch_size=batch_size)` with these `auto_downscale` / `downscale` /
     `crop` and fresh copies of the detectors give from `detect_scenes(video, duration=duration, end_time=end_time,
@@ -510,6 +539,12 @@ def detect_clips(videos, detectors, auto_downscale: bool = True, downscale: int 
     processed; `frame_skip` frames are read and not processed after each processed one, and `ClipResult.frames`
     counts them.  `crop` is SceneManager.crop's (X0, Y0, X1, Y1), inclusive, in every clip.
 
+    `windows` (keyword only) gives each clip its own window instead: one entry per video, None or a dict with keys
+    among `crop`, `duration`, `end_time` and `frame_skip`, meaning what the arguments of those names mean.  Clip i's
+    result is then that SceneManager's with `crop = windows[i].get("crop")`, from `detect_scenes(video,
+    duration=, end_time=, frame_skip=)` with the entry's values.  Clips cropped to one size share an engine and a pass
+    whatever their source sizes, and clips with different frame skips share the pass's one automaton launch.
+
     `stats=True`: every result also has `stats_csv`, the bytes `StatsManager.save_to_csv` writes (line terminator
     "\\n") after that SceneManager, built with a fresh `StatsManager()`, ran `detect_scenes(video)`: the header
     `Frame Number,Timecode,` and the sorted metric keys of the detectors, then one row per frame that has a metric.
@@ -520,7 +555,10 @@ def detect_clips(videos, detectors, auto_downscale: bool = True, downscale: int 
     an empty detector list or a detector with a `stats_manager` (the detectors take no StatsManager here: ask for
     `stats` instead), for the window arguments detect_scenes refuses (with its messages; `frame_skip` with `stats`
     included), and, before any frame is read, for a crop that starts outside some clip's frame; TypeError for a
-    malformed crop."""
+    malformed crop.  With `windows`, every entry is checked the same way before any frame is read; TypeError for
+    `windows` together with a window argument (`crop`, `duration` or `end_time` not None, `frame_skip` not 0), for
+    an entry that is not None or a dict and for an unknown key; ValueError for a number of entries other than the
+    number of videos."""
     detectors = list(detectors)
     if not detectors:
         raise ValueError("No detectors added")
@@ -529,6 +567,8 @@ def detect_clips(videos, detectors, auto_downscale: bool = True, downscale: int 
             raise TypeError("detect_clips drives the GPU detectors of this package")
         if d.stats_manager is not None:
             raise ValueError("detect_clips produces no per-frame metrics: detectors must not have a stats_manager")
+    if windows is not None and (crop is not None or duration is not None or end_time is not None or frame_skip != 0):
+        raise TypeError("detect_clips takes windows or crop / duration / end_time / frame_skip, not both")
     check_window(duration, end_time, frame_skip, stats)
     if downscale < 1:
         raise ValueError("Downscale factor must be a positive integer >= 1!")
@@ -536,7 +576,10 @@ def detect_clips(videos, detectors, auto_downscale: bool = True, downscale: int 
     geometry._auto_downscale, geometry._downscale = bool(auto_downscale), int(downscale)
     geometry.crop = crop
     videos = list(videos)
-    if crop is not None:
+    clip_windows = None
+    if windows is not None:
+        clip_windows = _clip_windows(videos, windows, geometry, stats)
+    elif crop is not None:
         for i, v in enumerate(videos):
             fw, fh = v.frame_size
             x0, y0 = geometry._crop[:2]
@@ -546,10 +589,11 @@ def detect_clips(videos, detectors, auto_downscale: bool = True, downscale: int 
     device_pass = _Pass.of_detectors(detectors, device, stats=stats)
     device_pass.frame_step = int(frame_skip) + 1
     passes = clip_passes(videos, device_pass.groups, geometry, batch_size, device, frame_skip=frame_skip,
-                         duration=duration, end_time=end_time)
+                         duration=duration, end_time=end_time, windows=clip_windows)
     try:
         for engine, holders, done in passes:
-            device_pass.finish(engine, holders, [(r, m) for _, r, m in done])
+            steps = () if clip_windows is None else ([int(clip_windows[i].frame_skip) + 1 for i, _, _ in done],)
+            device_pass.finish(engine, holders, [(r, m) for _, r, m in done], *steps)
             for index, r, _ in done:
                 results[index] = r
     finally:
@@ -558,23 +602,62 @@ def detect_clips(videos, detectors, auto_downscale: bool = True, downscale: int 
     return results
 
 
+def _clip_windows(videos, windows, geometry, stats: bool) -> list:
+    """The `_ClipWindow` of every clip from detect_clips' `windows`, each entry checked as SceneManager.crop and
+    detect_scenes check their arguments, and its crop against the clip's frame, before any geometry is computed
+    (`geometry`'s crop is left at the last clip's)."""
+    windows = list(windows)
+    if len(windows) != len(videos):
+        raise ValueError(f"windows has {len(windows)} entries for {len(videos)} videos")
+    checked = []
+    for i, (v, w) in enumerate(zip(videos, windows)):
+        w = {} if w is None else w
+        if not isinstance(w, dict):
+            raise TypeError(f"window {i} must be None or a dict, not {type(w).__name__}")
+        for key in w:
+            if key not in WINDOW_KEYS:
+                raise TypeError(f"window {i} has an unknown key {key!r}: the keys are {', '.join(WINDOW_KEYS)}")
+        skip = w.get("frame_skip", 0)
+        check_window(w.get("duration"), w.get("end_time"), skip, stats)
+        geometry.crop = w.get("crop")
+        if geometry._crop is not None:
+            fw, fh = v.frame_size
+            if geometry._crop[0] >= fw or geometry._crop[1] >= fh:
+                raise ValueError(f"crop starts outside video boundary of clip {i} ({fw}x{fh})")
+        checked.append((geometry._crop, skip, w.get("duration"), w.get("end_time")))
+    out = []
+    for v, (box, skip, duration, end_time) in zip(videos, checked):
+        geometry._crop = box
+        out.append(_ClipWindow(*geometry._geometry(*v.frame_size), skip, duration, end_time))  # its warning per clip
+    return out
+
+
 def clip_passes(videos, groups, geometry, batch_size: int, device: int, frame_skip: int = 0, duration=None,
-                end_time=None):
-    """Score the streams of `videos` pass by pass: clips grouped by `_group_key`, one engine per group built by
-    `shared_engine` with every pixel group of `groups` as a slot and `geometry._geometry` (a SceneManager's: its crop
-    and scored size), the clips of a group scored back to back, each through its own window of `frame_skip` /
-    `duration` / `end_time` (`_ClipChain`).  Frames scored are frames processed.  Yields (engine, holders, done) at the end of every pass, `done` being
-    [(input index, ClipResult, frames scored)] of the clips the engine holds, in order; the engine is reset for the
-    next pass when the consumer asks for it.  Close the generator to release the engine of an unfinished group."""
+                end_time=None, windows=None):
+    """Score the streams of `videos` pass by pass: one engine per group of clips built by `shared_engine` with every
+    pixel group of `groups` as a slot, the clips of a group scored back to back, each through its own window
+    (`_ClipChain`).  Without `windows`, clips are grouped by `_group_key` and read through `geometry._geometry` (a
+    SceneManager's: its crop and scored size) and the window of `frame_skip` / `duration` / `end_time`; with
+    `windows`, the `_ClipWindow` of every clip, they are grouped by cropped and scored size instead of frame size and
+    each is read through its own.  Frames scored are frames processed.  Yields (engine, holders, done) at the end of
+    every pass, `done` being [(input index, ClipResult, frames scored)] of the clips the engine holds, in order; the
+    engine is reset for the next pass when the consumer asks for it.  Close the generator to release the engine of an
+    unfinished group."""
     by_key: dict = {}
     for i, v in enumerate(videos):
-        by_key.setdefault(_group_key(v), []).append((i, v))
-    for (size, on_cuda, views, order), clips in by_key.items():
-        box, (w, h), (sw, sh) = geometry._geometry(*size)
+        key = _group_key(v) if windows is None else (windows[i].size, windows[i].scored) + _group_key(v)[1:]
+        by_key.setdefault(key, []).append((i, v))
+    for key, members in by_key.items():
+        on_cuda, views, order = key[-3:]
+        if windows is None:
+            group_window = _ClipWindow(*geometry._geometry(*key[0]), frame_skip, duration, end_time)
+            clips = [(i, v, group_window) for i, v in members]
+        else:
+            clips = [(i, v, windows[i]) for i, v in members]
+        (w, h), (sw, sh) = clips[0][2].size, clips[0][2].scored
         engine, holders = shared_engine(groups, w, h, sw, sh, device=device, max_batch=batch_size)
-        chain = (_DeviceClipChain if views else _ClipChain)(clips, MAX_PASS_FRAMES, on_cuda, frame_skip, duration,
-                                                           end_time)
-        gather = FrameBatches(chain, box, (w, h), batch_size)
+        chain = (_DeviceClipChain if views else _ClipChain)(clips, MAX_PASS_FRAMES, on_cuda)
+        gather = FrameBatches(chain, chain.box, (w, h), batch_size)
         try:
             while True:
                 item = gather.next()  # overlaps the GPU's work on the previous batch

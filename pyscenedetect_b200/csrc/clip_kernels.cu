@@ -8,9 +8,10 @@
 //                    of the metric arrays, with the clip's first frame number and min_frames: a counting pass, an
 //                    exclusive scan of the counts, then a writing pass into one compact cut array.
 //                    psd_clip_cuts_step runs the same kernels on clips read with a frame skip: slice element i is
-//                    frame first + i * step, and post_process sees each clip's end position; psd_clip_cuts_tables
-//                    gives each cell its own clip table (one per setting of a sweep over settings), and the other two
-//                    are its one-table calls
+//                    frame first + i * step, and post_process sees each clip's end position; psd_clip_cuts_steps
+//                    gives each clip its own step (clips read with different frame skips); psd_clip_cuts_tables
+//                    gives each cell its own clip table (one per setting of a sweep over settings), and the other
+//                    three are its one-table calls
 //   psd_clip_eval    the counterpart of psd_sweep_eval for psd_clip_cuts' compact output: every (cell, clip) list
 //                    turned in place into its predicted list, every (cell, clip, tolerance) scored against clip j's
 //                    ground truth with score_predictions (sweep_eval.cuh), and the counts summed over the clips;
@@ -63,12 +64,14 @@ __global__ void __launch_bounds__(256) psd_clip_fill_kernel(double* __restrict__
 // Counting pass (WRITE = false): cut_offsets[t] = how many cuts (cell, clip) t emits.  Writing pass: the cuts of t
 // at cuts[cut_offsets[t] ..], after psd_clip_scan_kernel turned the counts into offsets; nothing when the total
 // exceeds cap.  t = cell * n_clips + clip, so one cell's clips are adjacent threads.  Cell k reads clip table
-// tables[cell_table[k]] (tables[0] when cell_table is NULL): element i of clip j is frame first_frame[j] + i * step;
-// post_process's position is end_frame[j] - 1, or the last element's frame when end_frame is NULL.
+// tables[cell_table[k]] (tables[0] when cell_table is NULL): element i of clip j is frame first_frame[j] + i * step,
+// step being clip_step[j], or the table's frame_step when clip_step is NULL; post_process's position is
+// end_frame[j] - 1, or the last element's frame when end_frame is NULL.
 template <bool WRITE>
 __global__ void __launch_bounds__(128) psd_clip_cuts_kernel(const psd_sweep_cell* __restrict__ cells, int32_t n_cells,
                                                             const ClipTable* __restrict__ tables,
-                                                            const int32_t* __restrict__ cell_table, int32_t n_clips,
+                                                            const int32_t* __restrict__ cell_table,
+                                                            const int64_t* __restrict__ clip_step, int32_t n_clips,
                                                             const int64_t* __restrict__ min_frames,
                                                             int64_t* __restrict__ cuts, int64_t cap,
                                                             int64_t* __restrict__ cut_offsets) {
@@ -85,7 +88,7 @@ __global__ void __launch_bounds__(128) psd_clip_cuts_kernel(const psd_sweep_cell
         out.cuts = cuts + o;
         out.cap = (int32_t)(cut_offsets[t + 1] - o);
     }
-    const int64_t first = tb.first_frame[j], step = tb.frame_step;
+    const int64_t first = tb.first_frame[j], step = clip_step ? clip_step[j] : tb.frame_step;
     const int64_t last = tb.end_frame ? tb.end_frame[j] - 1 : first + (e - b - 1) * step;
     run_cell(cells[k], b, e - b, first, step, last, min_frames[t], out);
     if (!WRITE) cut_offsets[t] = out.n;
@@ -386,23 +389,26 @@ extern "C" int psd_clip_fill(double* values, int64_t n, const int64_t* clip_offs
     return PSD_OK;
 }
 
-// The cells, the clip tables and the cells' table indices, copied in one device allocation on `s` (pageable: staged
-// before return); *d_cells NULL when the copy failed.
+// The cells, the clip tables, the clips' steps and the cells' table indices, copied in one device allocation on `s`
+// (pageable: staged before return); *d_cells NULL when the copy failed.
 static int copy_tables(const psd_sweep_cell* cells, int32_t n_cells, const psd_clip_table* tables, int32_t n_tables,
-                       const int32_t* cell_table, cudaStream_t s, psd_sweep_cell** d_cells, ClipTable** d_tables,
-                       int32_t** d_cell_table) {
+                       const int64_t* clip_step, int32_t n_clips, const int32_t* cell_table, cudaStream_t s,
+                       psd_sweep_cell** d_cells, ClipTable** d_tables, int64_t** d_clip_step, int32_t** d_cell_table) {
     const size_t cb = sizeof(psd_sweep_cell) * (size_t)(cells ? n_cells : 0);
     const size_t tb = sizeof(psd_clip_table) * (size_t)n_tables;
+    const size_t sb = clip_step ? sizeof(int64_t) * (size_t)n_clips : 0;
     const size_t ib = cell_table ? sizeof(int32_t) * (size_t)n_cells : 0;
     char* d = nullptr;
     *d_cells = nullptr;
-    PSD_CUDA(cudaMallocAsync((void**)&d, cb + tb + ib, s));
+    PSD_CUDA(cudaMallocAsync((void**)&d, cb + tb + sb + ib, s));
     if (cb) PSD_CUDA(cudaMemcpyAsync(d, cells, cb, cudaMemcpyHostToDevice, s));
     PSD_CUDA(cudaMemcpyAsync(d + cb, tables, tb, cudaMemcpyHostToDevice, s));
-    if (ib) PSD_CUDA(cudaMemcpyAsync(d + cb + tb, cell_table, ib, cudaMemcpyHostToDevice, s));
+    if (sb) PSD_CUDA(cudaMemcpyAsync(d + cb + tb, clip_step, sb, cudaMemcpyHostToDevice, s));
+    if (ib) PSD_CUDA(cudaMemcpyAsync(d + cb + tb + sb, cell_table, ib, cudaMemcpyHostToDevice, s));
     *d_cells = (psd_sweep_cell*)d;
     *d_tables = (ClipTable*)(d + cb);
-    *d_cell_table = ib ? (int32_t*)(d + cb + tb) : nullptr;
+    *d_clip_step = sb ? (int64_t*)(d + cb + tb) : nullptr;
+    *d_cell_table = ib ? (int32_t*)(d + cb + tb + sb) : nullptr;
     return PSD_OK;
 }
 
@@ -415,13 +421,18 @@ static int check_tables(const char* name, int32_t n_tables, const int32_t* cell_
     return PSD_OK;
 }
 
+// clip_step: NULL (every clip steps by its table's frame_step), or a HOST int64[n_clips] step per clip.
 static int clip_cuts(const char* name, const psd_sweep_cell* cells, int32_t n_cells, const psd_clip_table* tables,
-                     int32_t n_tables, const int32_t* cell_table, int32_t n_clips, const int64_t* min_frames,
-                     int64_t* cuts, int64_t cuts_cap, int64_t* cut_offsets, void* stream) {
+                     int32_t n_tables, const int32_t* cell_table, const int64_t* clip_step, int32_t n_clips,
+                     const int64_t* min_frames, int64_t* cuts, int64_t cuts_cap, int64_t* cut_offsets, void* stream) {
     PSD_REQUIRE(tables && n_tables >= 1, "%s: no clip table", name);
     for (int32_t i = 0; i < n_tables; ++i) PSD_REQUIRE(tables[i].offsets, "%s: no clip table", name);
     PSD_REQUIRE(n_cells >= 0 && n_clips >= 0 && cuts_cap >= 0, "%s: bad args", name);
     for (int32_t i = 0; i < n_tables; ++i) PSD_REQUIRE(tables[i].frame_step >= 1, "%s: frame_step must be >= 1", name);
+    if (clip_step)
+        for (int32_t j = 0; j < n_clips; ++j)
+            PSD_REQUIRE(clip_step[j] >= 1, "%s: frame_step[%d] is %lld, must be >= 1", name, j,
+                        (long long)clip_step[j]);
     PSD_REQUIRE(cut_offsets, "%s: no cut_offsets array", name);
     int rc = check_tables(name, n_tables, cell_table, n_cells);
     if (rc != PSD_OK) return rc;
@@ -438,17 +449,19 @@ static int clip_cuts(const char* name, const psd_sweep_cell* cells, int32_t n_ce
     PSD_REQUIRE(cuts || cuts_cap == 0, "%s: no cut array", name);
     psd_sweep_cell* d_cells;
     ClipTable* d_tables;
+    int64_t* d_clip_step;
     int32_t* d_cell_table;
-    rc = copy_tables(cells, n_cells, tables, n_tables, cell_table, s, &d_cells, &d_tables, &d_cell_table);
+    rc = copy_tables(cells, n_cells, tables, n_tables, clip_step, n_clips, cell_table, s, &d_cells, &d_tables,
+                     &d_clip_step, &d_cell_table);
     if (rc != PSD_OK) return rc;
     const unsigned blocks = (unsigned)((m + 127) / 128);
-    psd_clip_cuts_kernel<false><<<blocks, 128, 0, s>>>(d_cells, n_cells, d_tables, d_cell_table, n_clips, min_frames,
-                                                       cuts, cuts_cap, cut_offsets);
+    psd_clip_cuts_kernel<false><<<blocks, 128, 0, s>>>(d_cells, n_cells, d_tables, d_cell_table, d_clip_step, n_clips,
+                                                       min_frames, cuts, cuts_cap, cut_offsets);
     PSD_CHECK_LAUNCH();
     psd_clip_scan_kernel<<<1, 1024, 0, s>>>(cut_offsets, m);
     PSD_CHECK_LAUNCH();
-    psd_clip_cuts_kernel<true><<<blocks, 128, 0, s>>>(d_cells, n_cells, d_tables, d_cell_table, n_clips, min_frames,
-                                                      cuts, cuts_cap, cut_offsets);
+    psd_clip_cuts_kernel<true><<<blocks, 128, 0, s>>>(d_cells, n_cells, d_tables, d_cell_table, d_clip_step, n_clips,
+                                                      min_frames, cuts, cuts_cap, cut_offsets);
     PSD_CHECK_LAUNCH();
     count_launch(3);
     PSD_CUDA(cudaFreeAsync(d_cells, s));
@@ -459,8 +472,8 @@ extern "C" int psd_clip_cuts(const psd_sweep_cell* cells, int32_t n_cells, const
                              const int64_t* clip_first_frame, int32_t n_clips, const int64_t* min_frames, int64_t* cuts,
                              int64_t cuts_cap, int64_t* cut_offsets, void* stream) {
     const psd_clip_table table{clip_offsets, clip_first_frame, nullptr, 1};
-    return clip_cuts("psd_clip_cuts", cells, n_cells, &table, 1, nullptr, n_clips, min_frames, cuts, cuts_cap,
-                     cut_offsets, stream);
+    return clip_cuts("psd_clip_cuts", cells, n_cells, &table, 1, nullptr, nullptr, n_clips, min_frames, cuts,
+                     cuts_cap, cut_offsets, stream);
 }
 
 extern "C" int psd_clip_cuts_step(const psd_sweep_cell* cells, int32_t n_cells, const int64_t* clip_offsets,
@@ -468,16 +481,26 @@ extern "C" int psd_clip_cuts_step(const psd_sweep_cell* cells, int32_t n_cells, 
                                   int64_t* cuts, int64_t cuts_cap, int64_t* cut_offsets, int64_t frame_step,
                                   const int64_t* clip_end_frame, void* stream) {
     const psd_clip_table table{clip_offsets, clip_first_frame, clip_end_frame, frame_step};
-    return clip_cuts("psd_clip_cuts_step", cells, n_cells, &table, 1, nullptr, n_clips, min_frames, cuts, cuts_cap,
-                     cut_offsets, stream);
+    return clip_cuts("psd_clip_cuts_step", cells, n_cells, &table, 1, nullptr, nullptr, n_clips, min_frames, cuts,
+                     cuts_cap, cut_offsets, stream);
+}
+
+extern "C" int psd_clip_cuts_steps(const psd_sweep_cell* cells, int32_t n_cells, const int64_t* clip_offsets,
+                                   const int64_t* clip_first_frame, int32_t n_clips, const int64_t* min_frames,
+                                   int64_t* cuts, int64_t cuts_cap, int64_t* cut_offsets, const int64_t* frame_step,
+                                   const int64_t* clip_end_frame, void* stream) {
+    PSD_REQUIRE(frame_step || n_clips <= 0, "psd_clip_cuts_steps: no frame_step array");
+    const psd_clip_table table{clip_offsets, clip_first_frame, clip_end_frame, 1};
+    return clip_cuts("psd_clip_cuts_steps", cells, n_cells, &table, 1, nullptr, frame_step, n_clips, min_frames, cuts,
+                     cuts_cap, cut_offsets, stream);
 }
 
 extern "C" int psd_clip_cuts_tables(const psd_sweep_cell* cells, int32_t n_cells, const psd_clip_table* tables,
                                     int32_t n_tables, const int32_t* cell_table, int32_t n_clips,
                                     const int64_t* min_frames, int64_t* cuts, int64_t cuts_cap, int64_t* cut_offsets,
                                     void* stream) {
-    return clip_cuts("psd_clip_cuts_tables", cells, n_cells, tables, n_tables, cell_table, n_clips, min_frames, cuts,
-                     cuts_cap, cut_offsets, stream);
+    return clip_cuts("psd_clip_cuts_tables", cells, n_cells, tables, n_tables, cell_table, nullptr, n_clips,
+                     min_frames, cuts, cuts_cap, cut_offsets, stream);
 }
 
 static int clip_eval(const char* name, int64_t* cuts, const int64_t* cut_offsets, int32_t n_cells, int32_t n_clips,
@@ -524,8 +547,10 @@ static int clip_eval(const char* name, int64_t* cuts, const int64_t* cut_offsets
     }
     psd_sweep_cell* d_alloc;
     ClipTable* d_tables;
+    int64_t* d_clip_step;
     int32_t* d_cell_table;
-    int rc = copy_tables(nullptr, n_cells, tables, n_tables, cell_table, s, &d_alloc, &d_tables, &d_cell_table);
+    int rc = copy_tables(nullptr, n_cells, tables, n_tables, nullptr, n_clips, cell_table, s, &d_alloc, &d_tables,
+                         &d_clip_step, &d_cell_table);
     if (rc != PSD_OK) return rc;
     clip_pred_kernel<<<(unsigned)((m + 127) / 128), 128, 0, s>>>(cuts, cut_offsets, m, cuts_total, max_cuts,
                                                                   out_n_pred, (unsigned long long*)out_over);

@@ -182,6 +182,8 @@ class StreamWindow:
 class FrameBatches:
     """The frame-gathering half of the detection loop (scene_manager.py:650-689): reads `video` in batches of
     up to `batch_size` frames, cropped to `box` = (x0, y0, x1, y1) of size `size` = (w, h), through a `StreamWindow`.
+    `box` may instead be a function that gives the box of the frames `video` has just returned (clips.py's chain of
+    clips, each with its own crop to the same size).
     A stream with `read_batch` and no crop / frame skip is read zero-copy; otherwise frames are copied into one of two
     page-locked buffers, so that a batch can be gathered while the GPU scores the previous one.
 
@@ -200,7 +202,7 @@ class FrameBatches:
     def __init__(self, video, box, size, batch_size: int, cropped: bool = False, frame_skip: int = 0,
                  end_frame: int | None = None):
         self._video = video
-        self._box, self._size = box, size
+        self._box, self._size = (box if callable(box) else lambda: box), size
         self._batch_size = int(batch_size)
         self._window = StreamWindow(video, frame_skip, end_frame)
         self._device_views = hasattr(video, "read_batch") and _dlpack.on_cuda(video)
@@ -220,7 +222,7 @@ class FrameBatches:
         tcs = [FrameTimecode(first + j * step, fps) for j in range(k)]
         if self._zero_copy:
             return tcs, chunk, bool(getattr(self._video, "is_pinned", False))
-        x0, y0, x1, y1 = self._box
+        x0, y0, x1, y1 = self._box()
         return tcs, chunk[:, y0:y1, x0:x1], False
 
     def next(self):
@@ -229,7 +231,6 @@ class FrameBatches:
         if self._device_views or self._zero_copy:
             return self._next_views()
         window = self._window
-        x0, y0, x1, y1 = self._box
         w, h = self._size
         tcs, batch = [], None
         which = self._which
@@ -240,6 +241,7 @@ class FrameBatches:
             if frame is False:
                 self._done = True
                 break
+            x0, y0, x1, y1 = self._box()
             if _dlpack.is_dlpack(frame):
                 views.append(frame[y0:y1, x0:x1])
             else:
