@@ -374,6 +374,24 @@ typedef struct psd_clip_table {
 int psd_clip_cuts_tables(const psd_sweep_cell* cells, int32_t n_cells, const psd_clip_table* tables, int32_t n_tables,
                          const int32_t* cell_table, int32_t n_clips, const int64_t* min_frames, int64_t* cuts,
                          int64_t cuts_cap, int64_t* cut_offsets, void* stream);
+/* A psd_clip_table whose clips each step by their own frame_step (clips read with different frame skips, the same
+ * step under every setting): element i of clip j is frame first_frame[j] + i * frame_step[j].  32 bytes, every pointer
+ * DEVICE memory; end_frame sits where psd_clip_table's does, so psd_clip_eval_tables takes the same three arrays as a
+ * psd_clip_table. */
+typedef struct psd_clip_steps_table {
+    const int64_t* offsets;     /* int64[n_clips + 1] */
+    const int64_t* first_frame; /* int64[n_clips] */
+    const int64_t* end_frame;   /* int64[n_clips]; NULL: post_process gets the last element */
+    const int64_t* frame_step;  /* int64[n_clips], every entry >= 1 (device memory: not validated; a smaller step
+                                   gives meaningless frame numbers and touches nothing outside the arrays) */
+} psd_clip_steps_table;
+/* psd_clip_cuts_tables with a step per (table, clip): cell k runs over tables[cell_table[k]] and clip j steps by that
+ * table's frame_step[j], as psd_clip_cuts_steps steps it for one table.  tables and cell_table are HOST arrays
+ * (validated, then copied on `stream` with the cells).  With every frame_step[j] of a table equal to s it gives
+ * psd_clip_cuts_tables with that table's frame_step = s bit for bit.  Same kernels and launches as psd_clip_cuts. */
+int psd_clip_cuts_tables_steps(const psd_sweep_cell* cells, int32_t n_cells, const psd_clip_steps_table* tables,
+                               int32_t n_tables, const int32_t* cell_table, int32_t n_clips, const int64_t* min_frames,
+                               int64_t* cuts, int64_t cuts_cap, int64_t* cut_offsets, void* stream);
 /* psd_clip_eval with a table per cell: (cell k, clip j)'s predicted list ends at tables[cell_table[k]].end_frame[j]
  * (cell_table NULL: tables[0]); only end_frame is read.  tables and cell_table are HOST arrays, copied on `stream`.
  * Ground truth, outputs and workspace as psd_clip_eval: the ground truth is per clip, shared by every table.  Same

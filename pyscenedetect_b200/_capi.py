@@ -102,6 +102,20 @@ class PsdClipTable(C.Structure):
 
 assert C.sizeof(PsdClipTable) == 32
 
+
+class PsdClipStepsTable(C.Structure):
+    """psd_clip_steps_table: a PsdClipTable whose clips each step by their own frame_step (32 bytes, DEVICE
+    pointers)."""
+    _fields_ = [
+        ("offsets", C.c_void_p),
+        ("first_frame", C.c_void_p),
+        ("end_frame", C.c_void_p),
+        ("frame_step", C.c_void_p),
+    ]
+
+
+assert C.sizeof(PsdClipStepsTable) == 32
+
 STATS_MAX_COLUMNS = 64
 F64_TEXT = 32  # bytes per value of psd_test_format_f64
 
@@ -211,6 +225,7 @@ SIGNATURES = {
     "psd_clip_eval": (C.c_int, [_vp, _vp, _i32, _i32, _i64, _i64, _vp, _vp, _vp, _i32, _vp, _vp, _i32, _vp, _i32, _vp,
                                 C.c_size_t, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "psd_clip_cuts_tables": (C.c_int, [_vp, _i32, _vp, _i32, _vp, _i32, _vp, _vp, _i64, _vp, _vp]),
+    "psd_clip_cuts_tables_steps": (C.c_int, [_vp, _i32, _vp, _i32, _vp, _i32, _vp, _vp, _i64, _vp, _vp]),
     "psd_clip_eval_tables": (C.c_int, [_vp, _vp, _i32, _i32, _i64, _i64, _vp, _i32, _vp, _vp, _vp, _i32, _vp, _vp,
                                        _i32, _vp, _i32, _vp, C.c_size_t, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "psd_clip_union": (C.c_int, [_vp, _vp, _i32, _i32, _i64, _i64, _vp, _vp, _i32, _vp, _vp, _i64, _vp, _vp,

@@ -382,14 +382,17 @@ class _Pass:
         obuf, cuts, total = self._cut_lists(engine, k * c, n, launch, "psd_clip_cuts")
         return PassCuts(scored, k, tbuf, obuf, cuts, total)
 
-    def cuts_tables(self, engines, holders, clips: list, steps: list) -> PassCuts:
+    def cuts_tables(self, engines, holders, clips: list, steps: list, clip_steps: list | None = None) -> PassCuts:
         """`cuts` for the same clips scored under several settings: setting s's engine `engines[s]` holds clip j's
-        clips[s][j] = (ClipResult, frames scored), element i of which is frame start + i * steps[s].  Each setting's
-        scans run on its engine with its own clip table; then ONE psd_clip_cuts_tables runs every (setting, cell, clip)
-        automaton, cell index s * len(cells) + k.  Every clip must have frames.  The result's `tables` hold each
-        setting's table, its `clips` are setting 0's."""
+        clips[s][j] = (ClipResult, frames scored), element i of which is frame start + i * steps[s], or start + i *
+        clip_steps[j] under every setting when `clip_steps` is given.  Each setting's scans run on its engine with its
+        own clip table; then ONE psd_clip_cuts_tables (psd_clip_cuts_tables_steps for clips that step differently)
+        runs every (setting, cell, clip) automaton, cell index s * len(cells) + k.  Every clip must have frames.  The
+        result's `tables` hold each setting's table, its `clips` are setting 0's."""
         lib = self._lib
         n_set, k, c = len(engines), len(self.cells), len(clips[0])
+        if clip_steps is not None and len(set(clip_steps)) == 1:  # clips that step alike: the table's frame_step
+            steps, clip_steps = [int(clip_steps[0])] * n_set, None
         parts, lens = [], []
         for s, e in enumerate(engines):
             sizes = np.array([m for _, m in clips[s]], dtype=np.int64)
@@ -400,16 +403,25 @@ class _Pass:
                       [r.end.frame_num + 1 for r, _ in clips[s]]]
             lens.append(e.frame_count)
         parts.append(np.tile([cell.min_frames(r.fps) for cell in self.cells for r, _ in clips[0]], n_set))
+        if clip_steps is not None:
+            parts.append(clip_steps)
         table = np.concatenate(parts).astype(np.int64)
         tbuf = DeviceBuffer(table.nbytes, self.device)
         tbuf.upload(table)
         per = (3 * c + 1) * 8  # bytes of one setting's offsets, first frames and end frames
+        min_frames = tbuf.ptr + n_set * per
+        # psd_clip_eval_tables reads a table's end frames only: with per-clip steps its frame_step is a placeholder
         tables = (_capi.PsdClipTable * n_set)()
         for s in range(n_set):
             base = tbuf.ptr + s * per
             tables[s] = _capi.PsdClipTable(offsets=base, first_frame=base + (c + 1) * 8,
-                                           end_frame=base + (2 * c + 1) * 8, frame_step=steps[s])
-        min_frames = tbuf.ptr + n_set * per
+                                           end_frame=base + (2 * c + 1) * 8,
+                                           frame_step=steps[s] if clip_steps is None else 1)
+        if clip_steps is not None:
+            step_ptr = min_frames + n_set * k * c * 8
+            steps_tables = (_capi.PsdClipStepsTable * n_set)(*[
+                _capi.PsdClipStepsTable(offsets=t.offsets, first_frame=t.first_frame, end_frame=t.end_frame,
+                                        frame_step=step_ptr) for t in tables])
         arrays = [self._scan(holders[s], tables[s].offsets, c, lens[s], tag=s if s else None) for s in range(n_set)]
         for e in engines[1:]:  # the automata read every setting's arrays: order them after every engine's scans
             e.sync()
@@ -418,8 +430,12 @@ class _Pass:
         st = engines[0].compute_stream
 
         def launch(cuts, cap, obuf):
-            check(lib.psd_clip_cuts_tables(cells, n_set * k, tables, n_set, cell_table, c, min_frames, cuts, cap, obuf,
-                                           st), "psd_clip_cuts_tables")
+            if clip_steps is None:
+                check(lib.psd_clip_cuts_tables(cells, n_set * k, tables, n_set, cell_table, c, min_frames, cuts, cap,
+                                               obuf, st), "psd_clip_cuts_tables")
+            else:
+                check(lib.psd_clip_cuts_tables_steps(cells, n_set * k, steps_tables, n_set, cell_table, c, min_frames,
+                                                     cuts, cap, obuf, st), "psd_clip_cuts_tables_steps")
 
         obuf, cuts, total = self._cut_lists(engines[0], n_set * k * c, sum(lens), launch, "psd_clip_cuts_tables")
         pc = PassCuts([r for r, _ in clips[0]], n_set * k, tbuf, obuf, cuts, total)
@@ -604,31 +620,37 @@ def detect_clips(videos, detectors, auto_downscale: bool = True, downscale: int 
 
 def _clip_windows(videos, windows, geometry, stats: bool) -> list:
     """The `_ClipWindow` of every clip from detect_clips' `windows`, each entry checked as SceneManager.crop and
-    detect_scenes check their arguments, and its crop against the clip's frame, before any geometry is computed
-    (`geometry`'s crop is left at the last clip's)."""
+    detect_scenes check their arguments, and its crop against the clip's frame, before any geometry is computed.  An
+    entry without a `crop` key keeps `geometry`'s crop; `geometry` is left as it was given."""
     windows = list(windows)
     if len(windows) != len(videos):
         raise ValueError(f"windows has {len(windows)} entries for {len(videos)} videos")
-    checked = []
-    for i, (v, w) in enumerate(zip(videos, windows)):
-        w = {} if w is None else w
-        if not isinstance(w, dict):
-            raise TypeError(f"window {i} must be None or a dict, not {type(w).__name__}")
-        for key in w:
-            if key not in WINDOW_KEYS:
-                raise TypeError(f"window {i} has an unknown key {key!r}: the keys are {', '.join(WINDOW_KEYS)}")
-        skip = w.get("frame_skip", 0)
-        check_window(w.get("duration"), w.get("end_time"), skip, stats)
-        geometry.crop = w.get("crop")
-        if geometry._crop is not None:
-            fw, fh = v.frame_size
-            if geometry._crop[0] >= fw or geometry._crop[1] >= fh:
-                raise ValueError(f"crop starts outside video boundary of clip {i} ({fw}x{fh})")
-        checked.append((geometry._crop, skip, w.get("duration"), w.get("end_time")))
-    out = []
-    for v, (box, skip, duration, end_time) in zip(videos, checked):
-        geometry._crop = box
-        out.append(_ClipWindow(*geometry._geometry(*v.frame_size), skip, duration, end_time))  # its warning per clip
+    base = geometry._crop
+    try:
+        checked = []
+        for i, (v, w) in enumerate(zip(videos, windows)):
+            w = {} if w is None else w
+            if not isinstance(w, dict):
+                raise TypeError(f"window {i} must be None or a dict, not {type(w).__name__}")
+            for key in w:
+                if key not in WINDOW_KEYS:
+                    raise TypeError(f"window {i} has an unknown key {key!r}: the keys are {', '.join(WINDOW_KEYS)}")
+            skip = w.get("frame_skip", 0)
+            check_window(w.get("duration"), w.get("end_time"), skip, stats)
+            geometry._crop = base
+            if "crop" in w:
+                geometry.crop = w["crop"]
+            if geometry._crop is not None:
+                fw, fh = v.frame_size
+                if geometry._crop[0] >= fw or geometry._crop[1] >= fh:
+                    raise ValueError(f"crop starts outside video boundary of clip {i} ({fw}x{fh})")
+            checked.append((geometry._crop, skip, w.get("duration"), w.get("end_time")))
+        out = []
+        for v, (box, skip, duration, end_time) in zip(videos, checked):
+            geometry._crop = box
+            out.append(_ClipWindow(*geometry._geometry(*v.frame_size), skip, duration, end_time))  # its warning per clip
+    finally:
+        geometry._crop = base
     return out
 
 

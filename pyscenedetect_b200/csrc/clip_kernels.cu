@@ -11,7 +11,7 @@
 //                    frame first + i * step, and post_process sees each clip's end position; psd_clip_cuts_steps
 //                    gives each clip its own step (clips read with different frame skips); psd_clip_cuts_tables
 //                    gives each cell its own clip table (one per setting of a sweep over settings), and the other
-//                    three are its one-table calls
+//                    three are its one-table calls; psd_clip_cuts_tables_steps gives each (table, clip) its own step
 //   psd_clip_eval    the counterpart of psd_sweep_eval for psd_clip_cuts' compact output: every (cell, clip) list
 //                    turned in place into its predicted list, every (cell, clip, tolerance) scored against clip j's
 //                    ground truth with score_predictions (sweep_eval.cuh), and the counts summed over the clips;
@@ -37,15 +37,23 @@ namespace psd {
 
 // A psd_clip_table as the kernels read it, under a name of this namespace: every symbol that starts psd_clip_ is then
 // a clip_kernels.cu kernel or entry, never a parameter type.
+// The last field is a psd_clip_table's frame_step, or a psd_clip_steps_table's per-clip steps: every table of a call is
+// one kind or the other.
 struct ClipTable {
     const int64_t* offsets;
     const int64_t* first_frame;
     const int64_t* end_frame;
-    int64_t frame_step;
+    union {
+        int64_t frame_step;
+        const int64_t* frame_steps;
+    };
 };
 static_assert(sizeof(ClipTable) == sizeof(psd_clip_table) && offsetof(ClipTable, end_frame) ==
                   offsetof(psd_clip_table, end_frame) && offsetof(ClipTable, frame_step) ==
                   offsetof(psd_clip_table, frame_step), "ClipTable must be laid out as psd_clip_table");
+static_assert(sizeof(ClipTable) == sizeof(psd_clip_steps_table) && offsetof(ClipTable, end_frame) ==
+                  offsetof(psd_clip_steps_table, end_frame) && offsetof(ClipTable, frame_steps) ==
+                  offsetof(psd_clip_steps_table, frame_step), "ClipTable must be laid out as psd_clip_steps_table");
 
 __global__ void __launch_bounds__(256) psd_clip_fill_kernel(double* __restrict__ values, int64_t n,
                                                             const int64_t* __restrict__ offsets, int32_t n_clips,
@@ -65,13 +73,13 @@ __global__ void __launch_bounds__(256) psd_clip_fill_kernel(double* __restrict__
 // at cuts[cut_offsets[t] ..], after psd_clip_scan_kernel turned the counts into offsets; nothing when the total
 // exceeds cap.  t = cell * n_clips + clip, so one cell's clips are adjacent threads.  Cell k reads clip table
 // tables[cell_table[k]] (tables[0] when cell_table is NULL): element i of clip j is frame first_frame[j] + i * step,
-// step being clip_step[j], or the table's frame_step when clip_step is NULL; post_process's position is
+// step being the table's frame_steps[j] when clip_steps is set, else its frame_step; post_process's position is
 // end_frame[j] - 1, or the last element's frame when end_frame is NULL.
 template <bool WRITE>
 __global__ void __launch_bounds__(128) psd_clip_cuts_kernel(const psd_sweep_cell* __restrict__ cells, int32_t n_cells,
                                                             const ClipTable* __restrict__ tables,
                                                             const int32_t* __restrict__ cell_table,
-                                                            const int64_t* __restrict__ clip_step, int32_t n_clips,
+                                                            int clip_steps, int32_t n_clips,
                                                             const int64_t* __restrict__ min_frames,
                                                             int64_t* __restrict__ cuts, int64_t cap,
                                                             int64_t* __restrict__ cut_offsets) {
@@ -88,7 +96,7 @@ __global__ void __launch_bounds__(128) psd_clip_cuts_kernel(const psd_sweep_cell
         out.cuts = cuts + o;
         out.cap = (int32_t)(cut_offsets[t + 1] - o);
     }
-    const int64_t first = tb.first_frame[j], step = clip_step ? clip_step[j] : tb.frame_step;
+    const int64_t first = tb.first_frame[j], step = clip_steps ? tb.frame_steps[j] : tb.frame_step;
     const int64_t last = tb.end_frame ? tb.end_frame[j] - 1 : first + (e - b - 1) * step;
     run_cell(cells[k], b, e - b, first, step, last, min_frames[t], out);
     if (!WRITE) cut_offsets[t] = out.n;
@@ -390,24 +398,30 @@ extern "C" int psd_clip_fill(double* values, int64_t n, const int64_t* clip_offs
 }
 
 // The cells, the clip tables, the clips' steps and the cells' table indices, copied in one device allocation on `s`
-// (pageable: staged before return); *d_cells NULL when the copy failed.
-static int copy_tables(const psd_sweep_cell* cells, int32_t n_cells, const psd_clip_table* tables, int32_t n_tables,
+// (pageable: staged before return); *d_cells NULL when the copy failed.  clip_step, a HOST int64[n_clips] for one
+// table, is copied too, and the copied table steps each clip by it.
+static int copy_tables(const psd_sweep_cell* cells, int32_t n_cells, const ClipTable* tables, int32_t n_tables,
                        const int64_t* clip_step, int32_t n_clips, const int32_t* cell_table, cudaStream_t s,
-                       psd_sweep_cell** d_cells, ClipTable** d_tables, int64_t** d_clip_step, int32_t** d_cell_table) {
+                       psd_sweep_cell** d_cells, ClipTable** d_tables, int32_t** d_cell_table) {
     const size_t cb = sizeof(psd_sweep_cell) * (size_t)(cells ? n_cells : 0);
-    const size_t tb = sizeof(psd_clip_table) * (size_t)n_tables;
+    const size_t tb = sizeof(ClipTable) * (size_t)n_tables;
     const size_t sb = clip_step ? sizeof(int64_t) * (size_t)n_clips : 0;
     const size_t ib = cell_table ? sizeof(int32_t) * (size_t)n_cells : 0;
     char* d = nullptr;
     *d_cells = nullptr;
     PSD_CUDA(cudaMallocAsync((void**)&d, cb + tb + sb + ib, s));
     if (cb) PSD_CUDA(cudaMemcpyAsync(d, cells, cb, cudaMemcpyHostToDevice, s));
-    PSD_CUDA(cudaMemcpyAsync(d + cb, tables, tb, cudaMemcpyHostToDevice, s));
-    if (sb) PSD_CUDA(cudaMemcpyAsync(d + cb + tb, clip_step, sb, cudaMemcpyHostToDevice, s));
+    if (clip_step) {
+        ClipTable t = tables[0];
+        t.frame_steps = (const int64_t*)(d + cb + tb);
+        PSD_CUDA(cudaMemcpyAsync(d + cb, &t, sizeof(t), cudaMemcpyHostToDevice, s));
+        if (sb) PSD_CUDA(cudaMemcpyAsync(d + cb + tb, clip_step, sb, cudaMemcpyHostToDevice, s));
+    } else {
+        PSD_CUDA(cudaMemcpyAsync(d + cb, tables, tb, cudaMemcpyHostToDevice, s));
+    }
     if (ib) PSD_CUDA(cudaMemcpyAsync(d + cb + tb + sb, cell_table, ib, cudaMemcpyHostToDevice, s));
     *d_cells = (psd_sweep_cell*)d;
     *d_tables = (ClipTable*)(d + cb);
-    *d_clip_step = sb ? (int64_t*)(d + cb + tb) : nullptr;
     *d_cell_table = ib ? (int32_t*)(d + cb + tb + sb) : nullptr;
     return PSD_OK;
 }
@@ -421,14 +435,21 @@ static int check_tables(const char* name, int32_t n_tables, const int32_t* cell_
     return PSD_OK;
 }
 
-// clip_step: NULL (every clip steps by its table's frame_step), or a HOST int64[n_clips] step per clip.
-static int clip_cuts(const char* name, const psd_sweep_cell* cells, int32_t n_cells, const psd_clip_table* tables,
-                     int32_t n_tables, const int32_t* cell_table, const int64_t* clip_step, int32_t n_clips,
-                     const int64_t* min_frames, int64_t* cuts, int64_t cuts_cap, int64_t* cut_offsets, void* stream) {
+// Each clip steps by its table's frame_step (clip_step NULL, table_steps false), by a HOST int64[n_clips] clip_step
+// (one table), or by its table's DEVICE frame_steps (table_steps true: psd_clip_steps_table).
+static int clip_cuts(const char* name, const psd_sweep_cell* cells, int32_t n_cells, const ClipTable* tables,
+                     int32_t n_tables, const int32_t* cell_table, const int64_t* clip_step, bool table_steps,
+                     int32_t n_clips, const int64_t* min_frames, int64_t* cuts, int64_t cuts_cap,
+                     int64_t* cut_offsets, void* stream) {
     PSD_REQUIRE(tables && n_tables >= 1, "%s: no clip table", name);
     for (int32_t i = 0; i < n_tables; ++i) PSD_REQUIRE(tables[i].offsets, "%s: no clip table", name);
     PSD_REQUIRE(n_cells >= 0 && n_clips >= 0 && cuts_cap >= 0, "%s: bad args", name);
-    for (int32_t i = 0; i < n_tables; ++i) PSD_REQUIRE(tables[i].frame_step >= 1, "%s: frame_step must be >= 1", name);
+    for (int32_t i = 0; i < n_tables; ++i) {
+        if (table_steps)
+            PSD_REQUIRE(tables[i].frame_steps || n_clips == 0, "%s: table %d has no frame_step array", name, i);
+        else
+            PSD_REQUIRE(tables[i].frame_step >= 1, "%s: frame_step must be >= 1", name);
+    }
     if (clip_step)
         for (int32_t j = 0; j < n_clips; ++j)
             PSD_REQUIRE(clip_step[j] >= 1, "%s: frame_step[%d] is %lld, must be >= 1", name, j,
@@ -449,18 +470,18 @@ static int clip_cuts(const char* name, const psd_sweep_cell* cells, int32_t n_ce
     PSD_REQUIRE(cuts || cuts_cap == 0, "%s: no cut array", name);
     psd_sweep_cell* d_cells;
     ClipTable* d_tables;
-    int64_t* d_clip_step;
     int32_t* d_cell_table;
     rc = copy_tables(cells, n_cells, tables, n_tables, clip_step, n_clips, cell_table, s, &d_cells, &d_tables,
-                     &d_clip_step, &d_cell_table);
+                     &d_cell_table);
     if (rc != PSD_OK) return rc;
+    const int steps = clip_step || table_steps;
     const unsigned blocks = (unsigned)((m + 127) / 128);
-    psd_clip_cuts_kernel<false><<<blocks, 128, 0, s>>>(d_cells, n_cells, d_tables, d_cell_table, d_clip_step, n_clips,
+    psd_clip_cuts_kernel<false><<<blocks, 128, 0, s>>>(d_cells, n_cells, d_tables, d_cell_table, steps, n_clips,
                                                        min_frames, cuts, cuts_cap, cut_offsets);
     PSD_CHECK_LAUNCH();
     psd_clip_scan_kernel<<<1, 1024, 0, s>>>(cut_offsets, m);
     PSD_CHECK_LAUNCH();
-    psd_clip_cuts_kernel<true><<<blocks, 128, 0, s>>>(d_cells, n_cells, d_tables, d_cell_table, d_clip_step, n_clips,
+    psd_clip_cuts_kernel<true><<<blocks, 128, 0, s>>>(d_cells, n_cells, d_tables, d_cell_table, steps, n_clips,
                                                       min_frames, cuts, cuts_cap, cut_offsets);
     PSD_CHECK_LAUNCH();
     count_launch(3);
@@ -468,12 +489,16 @@ static int clip_cuts(const char* name, const psd_sweep_cell* cells, int32_t n_ce
     return PSD_OK;
 }
 
+// A psd_clip_table or psd_clip_steps_table as the kernels read it (the layouts are asserted above).
+static const ClipTable* clip_tables(const psd_clip_table* t) { return reinterpret_cast<const ClipTable*>(t); }
+static const ClipTable* clip_tables(const psd_clip_steps_table* t) { return reinterpret_cast<const ClipTable*>(t); }
+
 extern "C" int psd_clip_cuts(const psd_sweep_cell* cells, int32_t n_cells, const int64_t* clip_offsets,
                              const int64_t* clip_first_frame, int32_t n_clips, const int64_t* min_frames, int64_t* cuts,
                              int64_t cuts_cap, int64_t* cut_offsets, void* stream) {
     const psd_clip_table table{clip_offsets, clip_first_frame, nullptr, 1};
-    return clip_cuts("psd_clip_cuts", cells, n_cells, &table, 1, nullptr, nullptr, n_clips, min_frames, cuts,
-                     cuts_cap, cut_offsets, stream);
+    return clip_cuts("psd_clip_cuts", cells, n_cells, clip_tables(&table), 1, nullptr, nullptr, false, n_clips,
+                     min_frames, cuts, cuts_cap, cut_offsets, stream);
 }
 
 extern "C" int psd_clip_cuts_step(const psd_sweep_cell* cells, int32_t n_cells, const int64_t* clip_offsets,
@@ -481,8 +506,8 @@ extern "C" int psd_clip_cuts_step(const psd_sweep_cell* cells, int32_t n_cells, 
                                   int64_t* cuts, int64_t cuts_cap, int64_t* cut_offsets, int64_t frame_step,
                                   const int64_t* clip_end_frame, void* stream) {
     const psd_clip_table table{clip_offsets, clip_first_frame, clip_end_frame, frame_step};
-    return clip_cuts("psd_clip_cuts_step", cells, n_cells, &table, 1, nullptr, nullptr, n_clips, min_frames, cuts,
-                     cuts_cap, cut_offsets, stream);
+    return clip_cuts("psd_clip_cuts_step", cells, n_cells, clip_tables(&table), 1, nullptr, nullptr, false, n_clips,
+                     min_frames, cuts, cuts_cap, cut_offsets, stream);
 }
 
 extern "C" int psd_clip_cuts_steps(const psd_sweep_cell* cells, int32_t n_cells, const int64_t* clip_offsets,
@@ -491,16 +516,24 @@ extern "C" int psd_clip_cuts_steps(const psd_sweep_cell* cells, int32_t n_cells,
                                    const int64_t* clip_end_frame, void* stream) {
     PSD_REQUIRE(frame_step || n_clips <= 0, "psd_clip_cuts_steps: no frame_step array");
     const psd_clip_table table{clip_offsets, clip_first_frame, clip_end_frame, 1};
-    return clip_cuts("psd_clip_cuts_steps", cells, n_cells, &table, 1, nullptr, frame_step, n_clips, min_frames, cuts,
-                     cuts_cap, cut_offsets, stream);
+    return clip_cuts("psd_clip_cuts_steps", cells, n_cells, clip_tables(&table), 1, nullptr, frame_step, false,
+                     n_clips, min_frames, cuts, cuts_cap, cut_offsets, stream);
 }
 
 extern "C" int psd_clip_cuts_tables(const psd_sweep_cell* cells, int32_t n_cells, const psd_clip_table* tables,
                                     int32_t n_tables, const int32_t* cell_table, int32_t n_clips,
                                     const int64_t* min_frames, int64_t* cuts, int64_t cuts_cap, int64_t* cut_offsets,
                                     void* stream) {
-    return clip_cuts("psd_clip_cuts_tables", cells, n_cells, tables, n_tables, cell_table, nullptr, n_clips,
-                     min_frames, cuts, cuts_cap, cut_offsets, stream);
+    return clip_cuts("psd_clip_cuts_tables", cells, n_cells, clip_tables(tables), n_tables, cell_table, nullptr, false,
+                     n_clips, min_frames, cuts, cuts_cap, cut_offsets, stream);
+}
+
+extern "C" int psd_clip_cuts_tables_steps(const psd_sweep_cell* cells, int32_t n_cells,
+                                          const psd_clip_steps_table* tables, int32_t n_tables,
+                                          const int32_t* cell_table, int32_t n_clips, const int64_t* min_frames,
+                                          int64_t* cuts, int64_t cuts_cap, int64_t* cut_offsets, void* stream) {
+    return clip_cuts("psd_clip_cuts_tables_steps", cells, n_cells, clip_tables(tables), n_tables, cell_table, nullptr,
+                     true, n_clips, min_frames, cuts, cuts_cap, cut_offsets, stream);
 }
 
 static int clip_eval(const char* name, int64_t* cuts, const int64_t* cut_offsets, int32_t n_cells, int32_t n_clips,
@@ -547,10 +580,9 @@ static int clip_eval(const char* name, int64_t* cuts, const int64_t* cut_offsets
     }
     psd_sweep_cell* d_alloc;
     ClipTable* d_tables;
-    int64_t* d_clip_step;
     int32_t* d_cell_table;
-    int rc = copy_tables(nullptr, n_cells, tables, n_tables, nullptr, n_clips, cell_table, s, &d_alloc, &d_tables,
-                         &d_clip_step, &d_cell_table);
+    int rc = copy_tables(nullptr, n_cells, clip_tables(tables), n_tables, nullptr, n_clips, cell_table, s, &d_alloc,
+                         &d_tables, &d_cell_table);
     if (rc != PSD_OK) return rc;
     clip_pred_kernel<<<(unsigned)((m + 127) / 128), 128, 0, s>>>(cuts, cut_offsets, m, cuts_total, max_cuts,
                                                                   out_n_pred, (unsigned long long*)out_over);

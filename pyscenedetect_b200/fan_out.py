@@ -44,8 +44,9 @@ def _runs(slots: list) -> list:
 
 
 class _HostFeed:
-    """Host frames of one group: copied into a page-locked batch of full frames, uploaded once per batch, then scored
-    by every setting's engine from the device copy, each through its crop and its own frames' slots."""
+    """Host frames of one group: copied into a page-locked batch of full frames (or of each frame's `crop` region, the
+    part of the current clip's frame that any setting reads), uploaded once per batch, then scored by every setting's
+    engine from the device copy, each through its crop and its own frames' slots."""
 
     def __init__(self, engines, boxes, frame_size, batch_size: int, device: int):
         fw, fh = frame_size
@@ -58,8 +59,12 @@ class _HostFeed:
         self.k = 0
         self.slots = [[] for _ in engines]
         self.uploaded = 0  # bytes copied to the device
+        self.crop = None   # (x0, y0, x1, y1) of the current clip's frames that the batch holds; None: the whole frame
 
     def add(self, frame, users) -> None:
+        if self.crop is not None:
+            x0, y0, x1, y1 = self.crop
+            frame = frame[y0:y1, x0:x1]
         np.copyto(self.frames[self.k], frame)
         for s in users:
             self.slots[s].append(self.k)
@@ -88,24 +93,33 @@ class _HostFeed:
 
 
 class _DeviceFeed:
-    """CUDA frames of one group: every setting's engine takes its own cropped view of the frames it processes."""
+    """CUDA frames of one group: every setting's engine takes its own cropped view of the frames it processes, its box
+    counted from the corner of the current clip's `crop` (None: of the whole frame)."""
 
     def __init__(self, engines, boxes, order: str, batch_size: int):
         self.engines, self.boxes, self.order = engines, boxes, order
         self.batch_size = batch_size
         self.held = 0
         self.uploaded = 0
+        self.crop = None
+
+    def _box(self, s: int) -> tuple:
+        x0, y0, x1, y1 = self.boxes[s]
+        if self.crop is None:
+            return x0, y0, x1, y1
+        ox, oy = self.crop[:2]
+        return ox + x0, oy + y0, ox + x1, oy + y1
 
     def add(self, frame, users) -> None:
         for s in users:
-            x0, y0, x1, y1 = self.boxes[s]
+            x0, y0, x1, y1 = self._box(s)
             self.engines[s].submit(frame[y0:y1, x0:x1], channel_order=self.order)
         self.held += 1
         if self.held >= self.batch_size:
             self.flush()
 
     def add_views(self, s: int, view) -> None:
-        x0, y0, x1, y1 = self.boxes[s]
+        x0, y0, x1, y1 = self._box(s)
         self.engines[s].submit(view[:, y0:y1, x0:x1], channel_order=self.order)
         self.held += view.shape[0]
 
@@ -179,25 +193,41 @@ def _read_clip(video, steps, feed, batch_size: int, views: bool, duration, end_t
     return i, results, scored
 
 
+def _clip_plan(windows) -> tuple:
+    """One clip's `clips._ClipWindow` under every setting -> (the box of its frames that some setting reads, the group
+    key of its geometry: that box's size and every setting's box within it, cropped size and scored size)."""
+    boxes = [w.box for w in windows]
+    feed = (min(b[0] for b in boxes), min(b[1] for b in boxes), max(b[2] for b in boxes), max(b[3] for b in boxes))
+    x0, y0 = feed[:2]
+    inner = tuple(((b[0] - x0, b[1] - y0, b[2] - x0, b[3] - y0), w.size, w.scored) for b, w in zip(boxes, windows))
+    return feed, ((feed[2] - x0, feed[3] - y0), inner)
+
+
 def settings_passes(videos, groups, geometries, frame_skips, batch_size: int, device: int, duration=None,
-                    end_time=None, counters: dict | None = None):
+                    end_time=None, counters: dict | None = None, windows=None):
     """Score the streams of `videos` once for every setting, pass by pass: clips grouped by `clips._group_key`, one
     engine per (group, setting) built by `shared_engine` with every pixel group of `groups` as a slot and
     `geometries[s]._geometry`, each clip read once (`_read_clip`) with the window of `duration` / `end_time` and
-    setting s's `frame_skips[s]`.  Yields (engines, holders, done) at the end of every pass, one engine and one holder
-    list per setting, `done` being [(input index, [ClipResult per setting], [frames processed per setting])] of the
-    clips the pass holds, in order; the engines are reset for the next pass when the consumer asks for it.
-    `counters["uploaded"]` accumulates the host frame bytes copied to the device.  Close the generator to release
-    the engines of an unfinished group."""
+    setting s's `frame_skips[s]`.  With `windows`, clip i's `clips._ClipWindow` under every setting (windows[i][s]: its
+    crop box, sizes, frame skip, duration and end_time) replaces those: clips are grouped by the region of their frames
+    that the settings read and by every setting's box in it, cropped size and scored size, so clips of any source size
+    cropped alike share a group; host frames are cropped to that region as they are copied.  Yields (engines, holders,
+    done) at the end of every pass, one engine and one holder list per setting, `done` being [(input index, [ClipResult
+    per setting], [frames processed per setting])] of the clips the pass holds, in order; the engines are reset for the
+    next pass when the consumer asks for it.  `counters["uploaded"]` accumulates the host frame bytes copied to the
+    device.  Close the generator to release the engines of an unfinished group."""
     steps = [int(f) + 1 for f in frame_skips]
     by_key: dict = {}
     for i, v in enumerate(videos):
-        by_key.setdefault(_group_key(v), []).append((i, v))
-    for (size, on_cuda, views, order), members in by_key.items():
+        key = _group_key(v) if windows is None else _clip_plan(windows[i])[1] + _group_key(v)[1:]
+        by_key.setdefault(key, []).append((i, v))
+    for key, members in by_key.items():
+        size, (on_cuda, views, order) = key[0], key[-3:]
         engines, holders, boxes, feed = [], [], [], None
         try:
-            for g in geometries:
-                box, (w, h), (sw, sh) = g._geometry(*size)
+            geometry = ([g._geometry(*size) for g in geometries] if windows is None else
+                        [(box, w_h, scored) for box, w_h, scored in key[1]])
+            for box, (w, h), (sw, sh) in geometry:
                 e, hs = shared_engine(groups, w, h, sw, sh, device=device, max_batch=batch_size)
                 engines.append(e)
                 holders.append(hs)
@@ -208,9 +238,15 @@ def settings_passes(videos, groups, geometries, frame_skips, batch_size: int, de
             for n, (index, video) in enumerate(members):
                 if _dlpack.on_cuda(video) != on_cuda:
                     raise ValueError("a stream's frames are not where its group's are (host or CUDA)")
-                got, results, scored = _read_clip(video, steps, feed, batch_size,
+                clip_steps, clip_duration, clip_end = steps, duration, end_time
+                if windows is not None:
+                    ws = windows[index]
+                    feed.crop = _clip_plan(ws)[0]
+                    clip_steps = [int(w.frame_skip) + 1 for w in ws]
+                    clip_duration, clip_end = ws[0].duration, ws[0].end_time
+                got, results, scored = _read_clip(video, clip_steps, feed, batch_size,
                                                   views or (not on_cuda and hasattr(video, "read_batch")),
-                                                  duration, end_time)
+                                                  clip_duration, clip_end)
                 done.append((index, results, scored))
                 read += got
                 if read >= clips.MAX_PASS_FRAMES or n + 1 == len(members):

@@ -652,7 +652,7 @@ class ParameterSweep:
                            grid_ms)
 
     # -- many clips per pass --
-    def run_clips(self, videos, ground_truths=None, duration=None, end_time=None) -> ClipSweepResult:
+    def run_clips(self, videos, ground_truths=None, duration=None, end_time=None, *, windows=None) -> ClipSweepResult:
         """Every cell over every stream of `videos`: for each (cell, clip), what `run(videos[j], ground_truths[j])`
         gives on a fresh ParameterSweep with this grid, tolerances and batch size; `totals` and `videos` afterwards
         are what a loop of `run` leaves.  Streams are anything `detect_clips` reads (host or CUDA `ArrayVideoStream`s
@@ -676,10 +676,40 @@ class ParameterSweep:
         GroundTruth per video.  ValueError for a length mismatch, a clip without frames, a window detect_scenes
         refuses (its messages) or, before any frame is read, a crop that starts outside some clip's frame (naming
         the clip and the setting); RuntimeError for a (cell, clip) with more than max_cuts_per_cell cuts; `totals`
-        only changes when the call returns."""
-        return self._run_clips(videos, ground_truths, duration, end_time, "clip {}")
+        only changes when the call returns.
 
-    def _run_clips(self, videos, ground_truths, duration, end_time, clip_name: str) -> ClipSweepResult:
+        `windows` (keyword only) gives each clip its own window, as `detect_clips(windows=)` takes it: one entry per
+        video, None or a dict with keys among `crop`, `duration`, `end_time` and `frame_skip`, checked as detect_clips
+        checks them.  Cell (s, g) on clip j is then what a one-clip ParameterSweep with this grid (or these
+        detector_sets) and `settings=[{**settings[s], **w}]` gives on it from `run_clips([videos[j]], [ground_truths[j]],
+        duration=, end_time=)`, w being the entry's `crop` and `frame_skip` and the other two its window: counts, cut
+        lists, end frames and totals.  A window does not change a clip's ground truth: cuts and fades past the window's
+        end are scored against the frames it reads, so those cuts count as missed; give the truth of the window alone to
+        score the window alone.  Per setting, clips whose crops and downscale give one scored size share an engine and a
+        pass whatever their source sizes, every clip is still read once for every setting, ending at its own window's
+        end, and a pass whose clips step differently runs psd_clip_cuts_tables_steps in place of psd_clip_cuts_tables,
+        with the same launches.  TypeError, before any frame is read, for `windows` together with `duration` or
+        `end_time`, and for a key (`crop`, `frame_skip`) that both some setting and some window set."""
+        return self._run_clips(videos, ground_truths, duration, end_time, "clip {}", windows)
+
+    def _window_plan(self, videos, windows) -> tuple:
+        """detect_clips' checks of `windows`, then every clip's `clips._ClipWindow` under every setting (windows[j][s]:
+        the setting's geometry under the window's crop, the window's frame skip or else the setting's) and the clips'
+        own steps, or None when the windows set no frame_skip."""
+        from .clips import _clip_windows
+        windows = list(windows)
+        set_keys = {k for x in self.settings for k in x}
+        both = sorted(set_keys & {k for w in windows if isinstance(w, dict) for k in w})
+        if both:
+            raise TypeError(f"{', '.join(both)} set both by a setting and by a window: a clip takes each from one or "
+                            f"the other")
+        per_setting = [_clip_windows(videos, windows, g, False) for g in self._geometries]
+        skips = any(isinstance(w, dict) and "frame_skip" in w for w in windows)
+        plan = [[w if skips else replace(w, frame_skip=f) for w, f in zip(ws, self._frame_skips)]
+                for ws in zip(*per_setting)]
+        return plan, [int(ws[0].frame_skip) + 1 for ws in plan] if skips else None
+
+    def _run_clips(self, videos, ground_truths, duration, end_time, clip_name: str, windows=None) -> ClipSweepResult:
         from .clips import _Pass, clip_passes
         from .fan_out import settings_passes
         videos = list(videos)
@@ -691,6 +721,8 @@ class ParameterSweep:
                 raise ValueError(f"{len(videos)} videos need as many ground truths, got {len(gts)}")
             if not all(isinstance(g, GroundTruth) for g in gts):
                 raise ValueError("every ground truth must be a GroundTruth (GroundTruth([]) for a clip without cuts)")
+        if windows is not None and (duration is not None or end_time is not None):
+            raise TypeError("run_clips takes windows or duration / end_time, not both")
         check_window(duration, end_time)
         for s, g in enumerate(self._geometries):
             if g._crop is not None:
@@ -700,6 +732,10 @@ class ParameterSweep:
                     if x0 >= fw or y0 >= fh:
                         raise ValueError(f"crop starts outside video boundary of clip {i} ({fw}x{fh}) in setting {s} "
                                          f"({self.settings[s]})")
+        plan = clip_steps = None
+        if windows is not None:
+            plan, clip_steps = self._window_plan(videos, windows)
+        fanned = plan is not None or not self._default_settings  # through fan_out.settings_passes
         lib = self._lib = self._lib or _capi.load()
         n_set, n_tol, dev = len(self.settings), len(self.tolerances), self.device
         n_cells = len(self.params)
@@ -721,26 +757,27 @@ class ParameterSweep:
         grid_ms = 0.0
         counters = {}
         device_pass = _Pass(self.cells, self.groups, dev)
-        if self._default_settings:
+        if not fanned:
             scoring = clip_passes(videos, self.groups, SceneManager(device=dev, batch_size=self.batch_size),
                                   self.batch_size, dev, duration=duration, end_time=end_time)
         else:
             scoring = settings_passes(videos, self.groups, self._geometries, self._frame_skips, self.batch_size, dev,
-                                      duration=duration, end_time=end_time, counters=counters)
+                                      duration=duration, end_time=end_time, counters=counters, windows=plan)
         steps = [f + 1 for f in self._frame_skips]
         try:
             for engine, holders, done in scoring:
-                if self._default_settings:
+                if not fanned:
                     done = [(index, [r], [m]) for index, r, m in done]
                 for index, _rs, ms in done:
                     if not ms[0]:
                         raise ValueError(f"{clip_name.format(index)} has no frames")
                 t0 = time.perf_counter()
-                if self._default_settings:
+                if not fanned:
                     pc = device_pass.cuts(engine, holders, [(rs[0], ms[0]) for _, rs, ms in done])
                 else:
+                    own = () if clip_steps is None else ([clip_steps[i] for i, _, _ in done],)
                     pc = device_pass.cuts_tables(engine, holders, [[(rs[s], ms[s]) for _, rs, ms in done]
-                                                                   for s in range(n_set)], steps)
+                                                                   for s in range(n_set)], steps, *own)
                     engine = engine[0]
                 indices = [index for index, _rs, _ms in done]
                 members = None
@@ -815,7 +852,7 @@ class ParameterSweep:
             self._totals_fades += tf
             self.videos += len(videos)
         return ClipSweepResult(self.params, self.tolerances, passes, where, ends, th, tf, grid_ms, n_grid=n_grid,
-                               upload_bytes=None if self._default_settings else counters.get("uploaded", 0),
+                               upload_bytes=counters.get("uploaded", 0) if fanned else None,
                                sets=self.sets)
 
     def _member_overflow(self, members, over: int, indices) -> None:
