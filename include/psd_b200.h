@@ -495,6 +495,10 @@ int psd_gather_bgr(int device, const void* base, const psd_frame_layout* layout,
 /* device BGR (n pixels, a multiple of 16) -> H,S,V and Y planes with the device functions the fused pass uses */
 int psd_test_hsv(int device, const uint8_t* bgr_host, int64_t n_pixels, uint8_t* h_out, uint8_t* s_out,
                  uint8_t* v_out, uint8_t* y_out);
+/* The INTER_LINEAR tap tables the engine builds for resizing one axis from src to dst pixels: ofs[dst] (the first
+ * source index; the second is ofs + 1, clamped to src - 1) and coef[dst][2] (11-bit coefficients).  Host only: no
+ * CUDA call, so it runs without a device. */
+int psd_test_resize_taps(int32_t src, int32_t dst, int32_t* ofs, int16_t* coef);
 /* str() of n host doubles with the device formatter psd_clip_stats_csv prints values with: text_out[n][32], each
  * value's text followed by NUL bytes */
 int psd_test_format_f64(int device, const double* values_host, int64_t n, char* text_out);

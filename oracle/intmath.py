@@ -85,28 +85,23 @@ def mean_from_sum(total: int, count: int) -> np.float64:
 INTER_RESIZE_COEF_SCALE = 2048
 
 
-def linear_taps(src: int, dst: int) -> tuple[np.ndarray, np.ndarray, np.ndarray]:
+def linear_taps(src, dst: int) -> tuple[np.ndarray, np.ndarray, np.ndarray]:
     """Per destination index: source index s (second tap is s+1 clamped) and the two 11-bit
-    coefficients (a0, a1).  float32 coefficient generation as in resize.cpp."""
-    scale = 1.0 / (dst / float(src)) if dst != src else 1.0
-    scale = float(src) / float(dst)
-    idx = np.zeros(dst, dtype=np.int32)
-    a0 = np.zeros(dst, dtype=np.int32)
-    a1 = np.zeros(dst, dtype=np.int32)
-    for d in range(dst):
-        f = np.float32((d + 0.5) * scale - 0.5)
-        s = int(math.floor(float(f)))
-        f = np.float32(f - np.float32(s))
-        if s < 0:
-            s, f = 0, np.float32(0.0)
-        if s >= src - 1:
-            s, f = src - 1, np.float32(0.0)
-        idx[d] = s
-        c0 = np.float32(np.float32(1.0) - f) * np.float32(INTER_RESIZE_COEF_SCALE)
-        c1 = np.float32(f) * np.float32(INTER_RESIZE_COEF_SCALE)
-        a0[d] = int(np.rint(c0))
-        a1[d] = int(np.rint(c1))
-    return idx, a0, a1
+    coefficients (a0, a1).  float32 coefficient generation as in resize.cpp, where the scale is
+    1 / inv_scale_x with inv_scale_x = dst / src (not src / dst, which can differ in the last bit).
+    `src` may be an array of source sizes: the tables then have shape (*src.shape, dst)."""
+    src = np.asarray(src, dtype=np.int64)[..., None]
+    scale = 1.0 / (dst / src.astype(np.float64))
+    f = ((np.arange(dst, dtype=np.float64) + 0.5) * scale - 0.5).astype(np.float32)
+    s = np.floor(f)
+    f = (f - s).astype(np.float32)
+    idx = s.astype(np.int64)
+    low, high = idx < 0, idx >= src - 1
+    idx = np.minimum(np.maximum(idx, 0), src - 1).astype(np.int32)
+    f[low | high] = 0
+    c0 = (np.float32(1.0) - f) * np.float32(INTER_RESIZE_COEF_SCALE)
+    c1 = f * np.float32(INTER_RESIZE_COEF_SCALE)
+    return idx, np.rint(c0).astype(np.int32), np.rint(c1).astype(np.int32)
 
 
 def resize_linear(img: np.ndarray, dw: int, dh: int) -> np.ndarray:

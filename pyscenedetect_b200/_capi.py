@@ -242,6 +242,7 @@ SIGNATURES = {
     "psd_synth_frames": (C.c_int, [C.c_int, _vp, _vp, _i64, _i32, _i32, _i64, _vp]),
     "psd_gather_bgr": (C.c_int, [C.c_int, _vp, C.POINTER(PsdFrameLayout), _i64, _i32, _i32, _vp, _i64, _vp]),
     "psd_test_hsv": (C.c_int, [C.c_int, _vp, _i64, _vp, _vp, _vp, _vp]),
+    "psd_test_resize_taps": (C.c_int, [_i32, _i32, _vp, _vp]),
     "psd_test_format_f64": (C.c_int, [C.c_int, _vp, _i64, _vp]),
     "psd_test_hash_stages": (C.c_int, [C.c_int, _vp, _i64, _i32, _i32, _i64, _vp, _i32, _vp, _vp, _vp, _vp]),
 }

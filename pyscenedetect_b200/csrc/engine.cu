@@ -26,10 +26,12 @@ void set_error(const char* fmt, ...) {
 }
 
 // OpenCV resize.cpp tap generation for INTER_LINEAR (float32 coefficient math, 11-bit fixed point).
+// The scale is 1 / (dst / src), as cv::resize derives it from inv_scale_x: it can differ from src / dst in the last
+// bit, and at sides above 10 240 pixels that bit can survive the float cast and move a coefficient by one.
 static void build_taps(int src, int dst, std::vector<int32_t>& ofs, std::vector<int16_t>& coef) {
     ofs.resize(dst);
     coef.resize(2 * (size_t)dst);
-    const double scale = (double)src / (double)dst;
+    const double scale = 1.0 / ((double)dst / (double)src);
     for (int d = 0; d < dst; ++d) {
         float f = (float)((d + 0.5) * scale - 0.5);
         int s = (int)floorf(f);
@@ -903,6 +905,17 @@ int psd_gather_bgr(int device, const void* base, const psd_frame_layout* layout,
     if (!rc) rc = launch_gather((const uint8_t*)base, *layout, n, width, height, (uint8_t*)dst, dst_frame_stride,
                                 (cudaStream_t)stream);
     return rc;
+}
+
+int psd_test_resize_taps(int32_t src, int32_t dst, int32_t* ofs, int16_t* coef) {
+    PSD_REQUIRE(src > 0 && dst > 0, "psd_test_resize_taps: sizes must be positive");
+    PSD_REQUIRE(ofs && coef, "psd_test_resize_taps: null argument");
+    std::vector<int32_t> o;
+    std::vector<int16_t> c;
+    build_taps(src, dst, o, c);
+    memcpy(ofs, o.data(), o.size() * sizeof(int32_t));
+    memcpy(coef, c.data(), c.size() * sizeof(int16_t));
+    return PSD_OK;
 }
 
 }  // extern "C"
