@@ -464,6 +464,52 @@ typedef struct psd_jpeg_image {
 int psd_jpeg_encode(int device, const psd_jpeg_image* images, int32_t n, int32_t quality, int64_t workspace_cap,
                     uint8_t* out, int64_t out_cap, int64_t* image_bytes, void* stream);
 
+/* ---- JPEG image sequences: cv2.imread(path, IMREAD_COLOR) of every file, decoded on the device ---- */
+/* Why psd_jpeg_probe refuses a file (refusal): */
+#define PSD_JPEG_OK 0
+#define PSD_JPEG_TRUNCATED 1    /* a marker segment or the scan runs past the end, or there is no EOI after the scan */
+#define PSD_JPEG_NOT_JPEG 2     /* no SOI */
+#define PSD_JPEG_PROCESS 3      /* progressive, lossless, hierarchical or arithmetic-coded (SOF2-SOF15) */
+#define PSD_JPEG_PRECISION 4    /* not 8-bit samples */
+#define PSD_JPEG_COMPONENTS 5   /* not 1 or 3 components, or 3 that libjpeg takes as RGB: no JFIF marker, and an
+                                   Adobe transform of 0 or (no Adobe marker) component ids 'R', 'G', 'B' */
+#define PSD_JPEG_SAMPLING 6     /* luma not 1x1, 2x1 or 2x2 over 1x1 chroma (4:1:1, 4:4:0, ...) */
+#define PSD_JPEG_MULTI_SCAN 7   /* a scan that does not hold every component (non-interleaved), or a second frame */
+#define PSD_JPEG_ORIENTATION 8  /* an EXIF orientation other than 1: imread would rotate the image */
+#define PSD_JPEG_TABLES 9       /* a missing or malformed quantisation or Huffman table */
+typedef struct psd_jpeg_info {
+    int32_t width, height, components;
+    int32_t h_samp, v_samp;        /* luma sampling factors (chroma is 1x1); 1, 1 for gray */
+    int32_t restart_interval;      /* MCUs per restart interval, 0 for none */
+    int32_t refusal;               /* PSD_JPEG_* */
+    int32_t reserved;
+    int64_t scan_begin, scan_end;  /* the entropy-coded data: bytes [scan_begin, scan_end), up to the last EOI */
+} psd_jpeg_info;
+/* Parses one file's markers up to its scan (host only: no CUDA call).  Returns PSD_OK and fills *info; info->refusal
+ * says whether psd_jpeg_decode takes the file.  Baseline (SOF0) and extended-sequential Huffman (SOF1) 8-bit files
+ * of 1 or 3 components in one interleaved scan, with 4:4:4, 4:2:2 or 4:2:0 sampling, any restart interval and any
+ * (optimised) Huffman tables. */
+int psd_jpeg_probe(const uint8_t* data, int64_t size, psd_jpeg_info* info);
+/* One file: the same `size` bytes at `host` (its markers are parsed there) and at `device` (DEVICE memory, decoded). */
+typedef struct psd_jpeg_source {
+    const void* host;
+    const void* device;
+    int64_t size;
+} psd_jpeg_source;
+/* Decodes n files into images[n] (a HOST array; each image's base is DEVICE memory and its width and height must be
+ * the file's), byte for byte what cv2.imread gives (libjpeg-turbo 3.1: jdhuff.c decode_mcu, jidctint.c
+ * jpeg_idct_islow with IDCT_range_limit's & RANGE_MASK wrap, jdsample.c h2v1 / h2v2 fancy upsampling when the
+ * downsampled width is above 2 and h2v1 / h2v2 replication otherwise (jinit_upsampler), jdmainct.c context rows
+ * replicating the first and last chroma rows, jdcolor.c build_ycc_rgb_table / ycc_rgb_convert, gray replicated to
+ * B, G, R).  A file psd_jpeg_probe refuses is PSD_ERR_INVALID, and nothing is queued.  error_flags[n] (DEVICE) is
+ * set to 0 for a file that decodes and nonzero for one whose entropy-coded data does not (its image is then
+ * unspecified): read it after `stream`.  The files are decoded in sub-batches whose workspace (allocated on `stream`)
+ * stays within workspace_cap bytes (0: 512 MiB), each at least one file: about 1.2 times the file's bytes, 132 bytes
+ * per 8x8 block and 64 per block of component samples (a 1920x1080 4:2:0 file of 500 KB takes about 11 MB); thirteen
+ * launches per sub-batch, queued on `stream` (a cudaStream_t or NULL), not waited for. */
+int psd_jpeg_decode(int device, const psd_jpeg_source* srcs, int32_t n, const psd_jpeg_image* images,
+                    int64_t workspace_cap, int32_t* error_flags, void* stream);
+
 /* host-convenience wrappers: engine-owned sums -> host arrays (numpy), implies sync */
 int psd_engine_scan_content_host(psd_engine* e, int64_t first, int64_t n, const double weights[4],
                                  double weight_abs_sum, double* out_components,

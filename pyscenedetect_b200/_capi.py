@@ -146,6 +146,49 @@ class PsdJpegImage(C.Structure):
 assert C.sizeof(PsdJpegImage) == 48
 
 
+class PsdJpegInfo(C.Structure):
+    """psd_jpeg_info: what psd_jpeg_probe reads of one file's markers (48 bytes)."""
+    _fields_ = [
+        ("width", C.c_int32),
+        ("height", C.c_int32),
+        ("components", C.c_int32),
+        ("h_samp", C.c_int32),
+        ("v_samp", C.c_int32),
+        ("restart_interval", C.c_int32),
+        ("refusal", C.c_int32),
+        ("reserved", C.c_int32),
+        ("scan_begin", C.c_int64),
+        ("scan_end", C.c_int64),
+    ]
+
+
+assert C.sizeof(PsdJpegInfo) == 48
+
+
+class PsdJpegSource(C.Structure):
+    """psd_jpeg_source: one file of psd_jpeg_decode, its bytes on the host and on the device (24 bytes)."""
+    _fields_ = [
+        ("host", C.c_void_p),
+        ("device", C.c_void_p),
+        ("size", C.c_int64),
+    ]
+
+
+assert C.sizeof(PsdJpegSource) == 24
+
+# psd_jpeg_probe refusals (PSD_JPEG_*)
+JPEG_REFUSALS = {
+    1: "truncated, or no EOI after its scan",
+    2: "not a JPEG file",
+    3: "progressive, lossless, hierarchical or arithmetic-coded",
+    4: "not 8-bit samples",
+    5: "not 1 or 3 YCbCr components (3 components without a JFIF marker may be RGB)",
+    6: "sampling other than 4:4:4, 4:2:2 or 4:2:0",
+    7: "not one interleaved scan",
+    8: "an EXIF orientation other than 1",
+    9: "a missing or malformed table",
+}
+
 # numpy view of psd_frame_sums (64 bytes)
 SUMS_DTYPE = np.dtype([
     ("sad_hue", "<u8"), ("sad_sat", "<u8"), ("sad_lum", "<u8"), ("sad_edges", "<u8"),
@@ -232,6 +275,8 @@ SIGNATURES = {
                                  _vp]),
     "psd_clip_stats_csv": (C.c_int, [_vp, _i32, _vp, _vp, _vp, _i32, _i64, _vp, _vp, _i64, _vp, _vp]),
     "psd_jpeg_encode": (C.c_int, [C.c_int, C.POINTER(PsdJpegImage), _i32, _i32, _i64, _vp, _i64, _vp, _vp]),
+    "psd_jpeg_probe": (C.c_int, [_vp, _i64, C.POINTER(PsdJpegInfo)]),
+    "psd_jpeg_decode": (C.c_int, [C.c_int, C.POINTER(PsdJpegSource), _i32, C.POINTER(PsdJpegImage), _i64, _vp, _vp]),
     "psd_engine_scan_content_host": (C.c_int, [_vp, _i64, _i64, _dp, _dbl, _vp, _vp]),
     "psd_engine_scan_adaptive_host": (C.c_int, [_vp, _vp, _i64, _i32, _dbl, _vp]),
     "psd_engine_scan_average_host": (C.c_int, [_vp, _i64, _i64, _vp]),

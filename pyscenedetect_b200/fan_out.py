@@ -143,6 +143,10 @@ def _read_clip(video, steps, feed, batch_size: int, views: bool, duration, end_t
     positions = {}  # local frame -> stream position after reading it, where some setting needs one
     needed = {0} | {e - 1 for e in ext if e is not None}
     i = 0
+    # a stream that recycles its CUDA batches (`batches_kept`, e.g. a decoder's pool) is read at most that many
+    # chunks ahead of the engines' last synchronisation
+    kept = getattr(video, "batches_kept", None)
+    chunks = 0
     if views:  # read_batch: chunks of the union, each setting's view [o::step] of them
         while union is None or i < union:
             chunk = video.read_batch(batch_size if union is None else min(batch_size, union - i))
@@ -166,8 +170,10 @@ def _read_clip(video, steps, feed, batch_size: int, views: bool, duration, end_t
                     if users:
                         feed.add(chunk[r], users)
             i += n
-            if on_cuda and feed.held >= batch_size:
+            chunks += 1
+            if on_cuda and (feed.held >= batch_size or (kept is not None and chunks >= kept)):
                 feed.flush()
+                chunks = 0
         pos_of = lambda j: FrameTimecode(start + j, fps)  # noqa: E731  (as StreamWindow.read_views numbers them)
     else:
         while union is None or i < union:

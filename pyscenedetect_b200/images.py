@@ -19,7 +19,7 @@ import numpy as np
 from . import _capi, _dlpack
 from ._capi import check
 from .compat import FrameTimecode
-from .engine import DeviceBuffer
+from .engine import DeviceBuffer, gather_bgr
 from .video import ArrayVideoStream
 
 logger = logging.getLogger("pyscenedetect")
@@ -119,8 +119,9 @@ class _Plan:
                 ), "jpg")
                 self.images.append((i, file_path, _output_path(file_path, output_dir), tc))
 
-    def frames(self):
-        """(output path, frame) of each image as it is read; a failed read skips the rest of its scene"""
+    def frames(self, device: int = 0):
+        """(output path, frame) of each image as it is read; a failed read skips the rest of its scene.  A CUDA frame
+        of a stream read through seek and read is copied out on `device` (a _DeviceCopy)."""
         video = self.video
         video.reset()
         skip = None
@@ -136,6 +137,10 @@ class _Plan:
                     self.completed = False
                     skip = i
                     continue
+                if _dlpack.is_dlpack(frame):
+                    self.filenames[i].append(file_path)
+                    yield path, _DeviceCopy(frame, getattr(video, "channel_order", "bgr"), device)
+                    continue
                 frame = np.asarray(frame)
                 if frame.ndim != 3 or frame.shape[2] != 3 or frame.dtype != np.uint8:
                     raise ValueError(f"frame {tc.frame_num} of {file_path!r} is {frame.dtype} {frame.shape}: only "
@@ -144,7 +149,27 @@ class _Plan:
             yield path, frame
 
 
+class _DeviceCopy:
+    """A CUDA frame read through a stream's seek and read, gathered at once to packed BGR24 in HBM of its own: the
+    stream may decode its next frame into the same memory (a decoder's pool of output buffers)."""
+
+    def __init__(self, frame, channel_order: str, device: int):
+        meta = _dlpack.import_frames(frame, device=device)
+        if meta.ndim != 3:
+            raise ValueError(f"a CUDA frame of shape {tuple(frame.shape)}: only (height, width, 3) uint8 BGR frames "
+                             "are encoded")
+        self.width, self.height = meta.width, meta.height
+        self.buf = DeviceBuffer(max(1, self.width * self.height * 3), device)
+        gather_bgr(frame, self.buf.ptr, None, channel_order, device)
+        self.buf.download(1)   # cudaMemcpy: the gather is done before the stream's next read can overwrite the frame
+
+    def close(self) -> None:
+        self.buf.close()
+
+
 def _frame_bytes(ref) -> int:
+    if isinstance(ref, _DeviceCopy):
+        return ref.width * ref.height * 3
     if isinstance(ref, np.ndarray):
         return ref.shape[0] * ref.shape[1] * 3
     return ref[0]._shape[1] * ref[0]._shape[2] * 3
@@ -154,6 +179,8 @@ def _host_frame(ref):
     """the BGR array of a frame reference that is not in CUDA memory, else None"""
     if isinstance(ref, np.ndarray):
         return ref
+    if isinstance(ref, _DeviceCopy):
+        return None
     video, index = ref
     if _dlpack.is_dlpack(video._frames):
         return None
@@ -184,6 +211,11 @@ def _encode_frames(refs, quality: int, device: int = 0) -> list[bytes]:
             images[k].width, images[k].height = w, h
     views = {}
     for k, r in enumerate(refs):
+        if isinstance(r, _DeviceCopy):
+            images[k].base = r.buf.ptr
+            images[k].layout = _capi.PsdFrameLayout(r.width * r.height * 3, r.width * 3, 3, 1)
+            images[k].width, images[k].height = r.width, r.height
+            continue
         if isinstance(r, np.ndarray) or not _dlpack.is_dlpack(r[0]._frames):
             continue
         video, index = r[0], r[1] % r[0]._shape[0]
@@ -244,14 +276,19 @@ def save_clip_images(clips, num_images: int = 3, frame_margin=1, image_extension
     group, group_bytes = [], 0
 
     def flush():
-        for (path, _), data in zip(group, _encode_frames([ref for _, ref in group], quality, device)):
-            os.makedirs(os.path.split(os.path.abspath(path))[0], exist_ok=True)
-            with open(path, "wb") as f:
-                f.write(data)
-        group.clear()
+        try:
+            for (path, _), data in zip(group, _encode_frames([ref for _, ref in group], quality, device)):
+                os.makedirs(os.path.split(os.path.abspath(path))[0], exist_ok=True)
+                with open(path, "wb") as f:
+                    f.write(data)
+        finally:
+            for _, ref in group:
+                if isinstance(ref, _DeviceCopy):
+                    ref.close()
+            group.clear()
 
     for plan in plans:
-        for path, ref in plan.frames():
+        for path, ref in plan.frames(device):
             nbytes = _frame_bytes(ref)
             if group and group_bytes + nbytes > GROUP_BYTES:
                 flush()
